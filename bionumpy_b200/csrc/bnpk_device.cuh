@@ -16,11 +16,7 @@ namespace bnpk {
 
 constexpr int kTileBytes = 16384;          // bytes owned by one tile
 constexpr int kHaloBytes = 2048;           // extra bytes staged so in-tile rows can finish
-constexpr int kTileThreads = 512;
-constexpr int kTileWarps = kTileThreads / 32;
-constexpr int kTileUnits = kTileBytes / 16;                  // 1024
 constexpr int kStagedUnits = (kTileBytes + kHaloBytes) / 16; // 1152
-constexpr int kRowCap = 512;               // rows of one tile kept in shared memory (more: deferred)
 constexpr int kSmemMaxBins = 32768;        // u32 bins that fit next to the tile staging
 
 constexpr uint64_t kFlagAgg = 1ull << 62;
@@ -49,11 +45,6 @@ __device__ __forceinline__ uint4 ld_stream(const uint4 *p) {
     return r;
 }
 
-__device__ __forceinline__ uint32_t warp_sum_u32(uint32_t v) {
-#pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 __device__ __forceinline__ uint64_t warp_sum_u64(uint64_t v) {
 #pragma unroll
     for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -275,25 +266,6 @@ __device__ __forceinline__ void hist_add(const HistTarget &t, uint64_t value) {
         atomicAdd(t.smem + (uint32_t)b, 1u);
     else
         atomicAdd(t.global + b, t.delta);
-}
-
-// first newline at or after tile-relative byte `from`, below `limit`; -1 if none.  Warp-wide.
-__device__ __forceinline__ int find_newline(const uint32_t *s_flags, int from, int limit, int lane) {
-    int unit0 = from >> 4;
-    const int last_unit = (limit + 15) >> 4;
-    for (; unit0 < last_unit; unit0 += 32) {
-        const int u = unit0 + lane;
-        uint32_t m = (u < last_unit) ? (s_flags[u] & 0xFFFFu) : 0u;
-        if (u == (from >> 4)) m &= 0xFFFFu << (from & 15);
-        const unsigned b = __ballot_sync(0xffffffffu, m != 0);
-        if (b) {
-            const int src = __ffs(b) - 1;
-            const int pos = (u << 4) + __ffs(m) - 1;
-            const int e = __shfl_sync(0xffffffffu, pos, src);
-            return e < limit ? e : -1;
-        }
-    }
-    return -1;
 }
 
 // first invalid byte in [from, to) (tile-relative), -1 if all valid.  Warp-wide.

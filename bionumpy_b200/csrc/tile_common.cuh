@@ -1,6 +1,7 @@
 // tile_common.cuh -- pieces shared by the tile kernels (tile_kernels.cu: split + register-staged count;
-// tile_tma_kernel.cu: the shared-memory-staged count): launch arguments, exact byte tests, the
-// 16-byte unit encoder and the two-level decoupled look-back over the tile newline counts.
+// tile_ws_kernel.cu: the warp-specialised counts; tile_tma_kernel.cu: the count into global tables): launch
+// arguments, exact byte tests, the 16-byte unit encoder, the rare-path helpers, the bulk-copy / mbarrier wrappers and
+// the two-level decoupled look-back over the tile newline counts.
 #pragma once
 #include "bnpk_host.h"
 
@@ -100,6 +101,85 @@ __device__ __forceinline__ uint32_t encode_unit_seq(const uint32_t *w, uint32_t 
     return codes;
 }
 
+// Rare: the first byte of bytes[p0, p1) outside the alphabet, reported as (entry << 32 | offset from the row's first
+// byte b0).  Called only when an encoder flagged a bad byte in that range.
+template <int ENC>
+__device__ __forceinline__ void report_bad_base(const TileArgs &a, const uint8_t *bytes, int p0, int p1, int b0, int64_t entry,
+                                                const uint8_t *s_lut) {
+    for (int p = p0; p < p1; ++p) {
+        const uint32_t c = bytes[p];
+        bool okb;
+        if (ENC == BNPK_ENC_CODES) okb = c < 4;
+        else if (ENC == BNPK_ENC_LUT) okb = s_lut[c] < 4;
+        else { const uint32_t uu = c | 0x20u; okb = (uu == 'a' || uu == 'c' || uu == 'g' || uu == 't'); }
+        if (!okb) {
+            atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE], (long long)((entry << 32) | (int64_t)(p - b0)));
+            break;
+        }
+    }
+}
+
+// A row the kernel cannot finish (no newline inside the staged bytes, or too long for its row walk): (first byte, entry)
+// goes to the deferred list that count_fixups_impl counts afterwards.
+__device__ __forceinline__ void defer_row(const TileArgs &a, uint64_t start, uint64_t r) {
+    const unsigned long long d = atomicAdd((unsigned long long *)(a.ws + kWsDeferred), 1ull);
+    if (d < a.deferred_cap) {
+        a.deferred[2 * d] = start;
+        a.deferred[2 * d + 1] = r;
+    } else {
+        a.status[BNPK_ST_OVERFLOW] = 1;
+    }
+}
+
+// ---- shared-memory staging by bulk copies (tile_ws_kernel.cu, tile_tma_kernel.cu) ------------------------------
+__device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// try_wait with a suspend-time hint; sleeping between the tests (nanosleep 64) costs more in wake-up latency than the
+// polling costs in issue slots, so the loop polls.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "WAIT_%=:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n"
+        "@p bra DONE_%=;\n"
+        "bra WAIT_%=;\n"
+        "DONE_%=:\n"
+        "}\n" ::"r"(bar), "r"(parity), "r"(20000u)
+        : "memory");
+}
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
+                 "l"(src), "r"(bytes), "r"(bar)
+                 : "memory");
+}
+__device__ __forceinline__ uint4 lds128(const uint8_t *p) { return *reinterpret_cast<const uint4 *>(p); }
+// PRMT without the selector clean-up __byte_perm adds (all selectors used here are in range)
+__device__ __forceinline__ uint32_t prmt(uint32_t lo, uint32_t hi, uint32_t sel) {
+    uint32_t d;
+    asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(lo), "r"(hi), "r"(sel));
+    return d;
+}
+// one count into the CTA-private table (32-bit shared address)
+__device__ __forceinline__ void hist_inc(uint32_t addr) { asm volatile("red.shared.add.u32 [%0], 1;" ::"r"(addr) : "memory"); }
+// ptxas never predicates ATOMS (it branches around it), so a masked count adds 0 or 1 instead
+__device__ __forceinline__ void hist_add_val(uint32_t addr, uint32_t val) { asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(addr), "r"(val) : "memory"); }
+// bit 7 of every byte that equals '\n' (bit 7 of the pattern is clear, so the last term can use w itself)
+__device__ __forceinline__ uint32_t newline_msb(uint32_t w) {
+    uint32_t x;                                                     // (w ^ 0x0A..) & 0x7F.. as ONE LOP3
+    asm("lop3.b32 %0, %1, 0x0A0A0A0A, 0x7F7F7F7F, 0x28;" : "=r"(x) : "r"(w));
+    const uint32_t s = x + 0x7F7F7F7Fu;
+    return ~(s | w) & 0x80808080u;
+}
+
 // ---- two-level look-back state in the workspace ------------------------------------------------
 //   tile_state[t]  : flag|value, AGG = newlines of tile t, PREFIX = newlines of tiles 0..t
 //   block_cnt[b]   : atomic (count << 56 | sum) over the 32 tiles of block b
@@ -173,15 +253,18 @@ __device__ __forceinline__ uint64_t lookback_finish(const LookbackArrays &l, int
     return excl;
 }
 
-
-// the shared-memory-staged fused count (tile_tma_kernel.cu).  Returns -1 when the launch does not
-// qualify (minimizers, unaligned chunk, too many bins for its table) and the caller must fall back.
-bool tma_count_eligible(const TileArgs &a, bool smem_hist);
-constexpr int64_t kScratch32MaxBins = 1ll << 24;   // 64 MiB of u32 counters at the end of the workspace
-int launch_tma_count(const TileArgs &a, int enc_mode, bool smem_hist, cudaStream_t st);
-// the warp-specialised fused count (tile_ws_kernel.cu): same eligibility, the default
-int launch_ws_count(const TileArgs &a, int enc_mode, bool smem_hist, cudaStream_t st);
+// The fused-count kernels besides the register-staged tile_kernel, which takes every call none of them is eligible for.
+// smem_hist = the table is counted in a CTA-private shared-memory table (use_smem_hist).
+// warp-specialised, minimizers (tile_ws_kernel.cu): windows of up to 12 k-mers, CTA-private table of up to 2^14 bins,
+// 16-byte-aligned chunk
 bool wsm_count_eligible(const TileArgs &a, bool smem_hist);
-int launch_wsm_count(const TileArgs &a, int enc_mode, bool smem_hist, cudaStream_t st);
+int launch_wsm_count(const TileArgs &a, int enc_mode, cudaStream_t st);
+// warp-specialised, k-mers: CTA-private table of up to 2^14 bins, aligned chunk
+bool ws_count_eligible(const TileArgs &a, bool smem_hist);
+int launch_ws_count(const TileArgs &a, int enc_mode, cudaStream_t st);
+// shared-memory-staged (tile_tma_kernel.cu), k-mers: global table, aligned chunk
+bool tma_count_eligible(const TileArgs &a, bool smem_hist);
+int launch_tma_count(const TileArgs &a, int enc_mode, cudaStream_t st);
+constexpr int64_t kScratch32MaxBins = 1ll << 24;   // 64 MiB of u32 counters at the end of the workspace
 
 }  // namespace bnpk

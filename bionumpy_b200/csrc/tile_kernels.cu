@@ -6,13 +6,12 @@
 //   1. 64 B/thread -> registers; exact '\n' mask per thread (SWAR zero-byte test)
 //   2. block scan of newline counts + decoupled look-back -> global line index of every byte,
 //      so every thread knows which of its bytes lie on a sequence line (the row-offset vector
-//      never leaves the SM: row starts/ends go to shared memory)
+//      never leaves the SM: the newline positions go to shared memory)
 //   3. only sequence bytes are turned into 2-bit codes (and validated) -> packed stream in smem
 //   4. four threads per read row walk the packed stream: funnel-shift = rolling 2-bit hash,
 //      one shared-memory atomic per k-mer into the CTA-private histogram
 //   5. at the end of the grid-stride loop the private histogram is flushed with global atomics.
 // Minimizers use one warp per row and a warp-shuffle sliding minimum.
-#include <cstdlib>
 #include "tile_common.cuh"
 
 namespace bnpk {
@@ -47,17 +46,17 @@ __global__ void cr_detect_kernel(const uint8_t *chunk, size_t n, int lpe, int tr
 constexpr int kCtaThreads = (kTileBytes + kHaloBytes) / 64;      // one thread per 64 staged bytes
 constexpr int kCtaWarps = kCtaThreads / 32;
 constexpr int kMainThreads = kTileBytes / 64;
-constexpr int kNl0Bytes = (kCtaThreads + 4 + 15) & ~15;
 static_assert(kCtaThreads % 32 == 0 && kMainThreads % 32 == 0 && kCtaWarps <= 32, "tile geometry");
-// shared-memory layout of the tile kernel, in 32-bit words
-constexpr int kOffCodes = 0;
-constexpr int kOffRowEnd = kOffCodes + kStagedUnits + 4;
-constexpr int kOffRowStart = kOffRowEnd + kRowCap;
-constexpr int kOffWarp = kOffRowStart + kRowCap / 2;
+constexpr int kNlCap = 1024;              // newline positions of one staged tile kept in shared memory
+constexpr int kNlStep = kNlCap - 8;       // window advance when a tile holds more (lines shorter than ~18 bytes)
+// shared-memory layout of the tile kernel behind the private histogram (n_bins words, count mode with SMEM_HIST only),
+// in 32-bit words
+constexpr int kOffCodes = 0;                                    // packed 2-bit stream
+constexpr int kOffNlPos = kOffCodes + kStagedUnits + 4;         // sorted newline list (kNlCap u16)
+constexpr int kOffWarp = kOffNlPos + kNlCap / 2;                // warp totals of the newline scan
 constexpr int kOffMisc = kOffWarp + 32;
-constexpr int kOffNl0 = kOffMisc + 16;
-constexpr int kOffLut = kOffNl0 + kNl0Bytes / 4;
-constexpr int kOffHist = kOffLut + 64;
+constexpr int kOffLut = kOffMisc + 16;                          // 256-byte LUT
+constexpr int kFixedWords = kOffLut + 64;
 
 // Software pipeline (per CTA): front(T+3) | look-back loads(T+1) | main(T)
 //   front : take a ticket, load 64 B/thread from HBM, exact newline mask, block scan, publish the tile's count
@@ -66,19 +65,17 @@ constexpr int kOffHist = kOffLut + 64;
 //           rows are read straight off the list (row s starts after newline jr0 + s*lpe and ends at the next one);
 //           four threads per read row load the row's 16-byte units (L2 hits), encode + validate only those,
 //           then walk the packed stream for the k-mers.
-constexpr int kNlCap = 1024;              // newline positions of one staged tile kept in shared memory
-constexpr int kNlStep = kNlCap - 8;       // window advance when a tile holds more (lines shorter than ~18 bytes)
 
 template <int MODE, int ENC, bool SMEM_HIST, bool MINIMIZER>
 __global__ void __launch_bounds__(kCtaThreads, MODE == 0 ? 4 : 3) tile_kernel(const TileArgs a) {
     extern __shared__ __align__(16) uint32_t smem[];
-    // layout: [private histogram (n_bins u32, SMEM_HIST only)] [packed stream] [newline list] [small stuff]
     uint32_t *s_hist = smem;
-    uint32_t *s_codes = smem + ((MODE == 1 && SMEM_HIST) ? a.n_bins : 0);          // kStagedUnits + 4
-    uint16_t *s_nlpos = reinterpret_cast<uint16_t *>(s_codes + kStagedUnits + 4);  // kNlCap
-    uint32_t *s_warp = reinterpret_cast<uint32_t *>(s_nlpos + kNlCap);             // 32
-    uint32_t *s_misc = s_warp + 32;                                                // 16
-    uint8_t *s_lut = reinterpret_cast<uint8_t *>(s_misc + 16);                     // 256
+    uint32_t *s_fixed = smem + ((MODE == 1 && SMEM_HIST) ? a.n_bins : 0);
+    uint32_t *s_codes = s_fixed + kOffCodes;
+    uint16_t *s_nlpos = reinterpret_cast<uint16_t *>(s_fixed + kOffNlPos);
+    uint32_t *s_warp = s_fixed + kOffWarp;
+    uint32_t *s_misc = s_fixed + kOffMisc;
+    uint8_t *s_lut = reinterpret_cast<uint8_t *>(s_fixed + kOffLut);
     __shared__ int64_t s_line_base;
     __shared__ int64_t s_tk[3];
 
@@ -172,15 +169,6 @@ __global__ void __launch_bounds__(kCtaThreads, MODE == 0 ? 4 : 3) tile_kernel(co
     };
     auto take_ticket = [&]() -> int64_t {
         return a.tile_begin + (int64_t)atomicAdd((unsigned long long *)(a.ws + kWsTicket), 1ull);
-    };
-    auto defer_row = [&](uint64_t start, uint64_t r) {
-        const unsigned long long d = atomicAdd((unsigned long long *)(a.ws + kWsDeferred), 1ull);
-        if (d < a.deferred_cap) {
-            a.deferred[2 * d] = start;
-            a.deferred[2 * d + 1] = r;
-        } else {
-            a.status[BNPK_ST_OVERFLOW] = 1;
-        }
     };
 
     // ---- prologue: fill the pipeline: all three first tickets are counted and published before any
@@ -329,7 +317,7 @@ __global__ void __launch_bounds__(kCtaThreads, MODE == 0 ? 4 : 3) tile_kernel(co
                     const int li = (int)(jr0 + ((uint32_t)slot << ls)) - win_lo;   // list index of the row's start newline
                     const int b0 = (int)s_nlpos[li] + 1 + a.start_offset;
                     if ((uint32_t)(win_lo + li) + 1u >= all_nl) {   // no terminating newline in the staged region
-                        if (sub == 0 && byte0 + staged_len < a.n) defer_row(byte0 + b0, (uint64_t)(r_first + slot));   // long row
+                        if (sub == 0 && byte0 + staged_len < a.n) defer_row(a, byte0 + b0, (uint64_t)(r_first + slot));   // long row
                         continue;                                    // (else: unterminated last line, not an entry)
                     }
                     int e = s_nlpos[li + 1];
@@ -350,20 +338,7 @@ __global__ void __launch_bounds__(kCtaThreads, MODE == 0 ? 4 : 3) tile_kernel(co
                             const uint32_t seq16 = (0xFFFFu >> (16 - hi)) & (0xFFFFu << lo);
                             uint32_t bad;
                             s_codes[u] = encode_unit_seq<ENC>(w, seq16, s_lut, bad);
-                            if (bad) {                                // rare: exact position, byte by byte
-                                for (int p = 16 * u + lo; p < 16 * u + hi; ++p) {
-                                    const uint32_t c = a.chunk[byte0 + p];
-                                    bool okb;
-                                    if (ENC == BNPK_ENC_CODES) okb = c < 4;
-                                    else if (ENC == BNPK_ENC_LUT) okb = s_lut[c] < 4;
-                                    else { const uint32_t uu = c | 0x20u; okb = (uu == 'a' || uu == 'c' || uu == 'g' || uu == 't'); }
-                                    if (!okb) {
-                                        atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE],
-                                                  (long long)(((r_first + slot) << 32) | (int64_t)(p - b0)));
-                                        break;
-                                    }
-                                }
-                            }
+                            if (bad) report_bad_base<ENC>(a, a.chunk + byte0, 16 * u + lo, 16 * u + hi, b0, r_first + slot, s_lut);
                         }
                     }
                     __syncwarp(gmask);
@@ -470,7 +445,7 @@ __global__ void finalize_status_kernel(int64_t *status, int lpe) {
 }
 
 static size_t tile_smem_bytes(int mode, uint64_t n_bins, bool smem_hist) {
-    size_t bytes = (size_t)kOffHist * 4;
+    size_t bytes = (size_t)kFixedWords * 4;
     if (mode == 1 && smem_hist) bytes += n_bins * 4;
     return bytes;
 }
@@ -500,28 +475,11 @@ static int launch_count_enc(const TileArgs &a, bool smem_hist, cudaStream_t st) 
     return mz ? launch_tile<1, ENC, false, true>(a, st) : launch_tile<1, ENC, false, false>(a, st);
 }
 
-// BNPK_TILE_KERNEL selects the fused-count kernel (A/B runs, tests of every path): "reg" = register-staged
-// everywhere, "tma" = the round-1 shared-memory-staged kernel, anything else = the warp-specialised one
-static int tile_kernel_choice() {
-    static const int choice = [] {
-        const char *e = std::getenv("BNPK_TILE_KERNEL");
-        if (e && e[0] == 'r') return 0;
-        if (e && e[0] == 't') return 1;
-        if (e && e[0] == 'w') return 3;                              // "ws": the warp-specialised kernel for every table
-        return 2;
-    }();
-    return choice;
-}
-static bool tma_kernel_allowed() { return tile_kernel_choice() != 0; }
-
+// One kernel per call, chosen from the call alone (every route counts the same table)
 static int launch_count(const TileArgs &a, int enc_mode, bool smem_hist, cudaStream_t st) {
-    if (tma_kernel_allowed() && tile_kernel_choice() != 1 && wsm_count_eligible(a, smem_hist))
-        return launch_wsm_count(a, enc_mode, smem_hist, st);          // minimizers, windows of up to 12 k-mers
-    if (tma_kernel_allowed() && tma_count_eligible(a, smem_hist))
-        // the warp-specialised kernel for CTA-private tables; global tables are bound by L2 atomics, where the round-1
-        // kernel's 21 row warps per SM keep more of them in flight
-        return (tile_kernel_choice() == 1 || (!smem_hist && tile_kernel_choice() != 3)) ? launch_tma_count(a, enc_mode, smem_hist, st)
-                                                                                       : launch_ws_count(a, enc_mode, smem_hist, st);
+    if (wsm_count_eligible(a, smem_hist)) return launch_wsm_count(a, enc_mode, st);
+    if (ws_count_eligible(a, smem_hist)) return launch_ws_count(a, enc_mode, st);
+    if (tma_count_eligible(a, smem_hist)) return launch_tma_count(a, enc_mode, st);
     switch (enc_mode) {
         case BNPK_ENC_ASCII_ACGT: return launch_count_enc<BNPK_ENC_ASCII_ACGT>(a, smem_hist, st);
         case BNPK_ENC_ASCII_ACTG: return launch_count_enc<BNPK_ENC_ASCII_ACTG>(a, smem_hist, st);
@@ -593,8 +551,7 @@ int chunk_kmer_count_impl(const uint8_t *chunk, size_t n, size_t slice_begin, si
     BNPK_CUDA(cudaMemsetAsync(a.ws + kWsTicket, 0, sizeof(uint64_t), st));
     const bool smem_hist = use_smem_hist(n_bins, hist_mode);
     // tables between 32 MiB and 128 MiB of int64: count in the 32-bit scratch (a bin cannot overflow: n < 2^32 bytes)
-    const bool scratch32 = !smem_hist && n_bins > (1ll << 22) && n_bins <= kScratch32MaxBins && n < (1ull << 32) &&
-                           tma_kernel_allowed() && tma_count_eligible(a, smem_hist);
+    const bool scratch32 = n_bins > (1ll << 22) && n_bins <= kScratch32MaxBins && n < (1ull << 32) && tma_count_eligible(a, smem_hist);
     if (scratch32) {
         a.hist32 = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(workspace) + ws_core_bytes(n));
         if (slice_begin == 0) BNPK_CUDA(cudaMemsetAsync(a.hist32, 0, (size_t)n_bins * sizeof(uint32_t), st));

@@ -1,7 +1,9 @@
-// tile_tma_kernel.cu -- fused count (K6) with the chunk staged in shared memory by bulk async copies (TMA).
+// tile_tma_kernel.cu -- fused count (K6) into global tables, the chunk staged in shared memory by bulk async
+// copies (TMA).  Global tables are bound by L2 atomics: this kernel's 21 row warps per SM keep more of them in flight
+// than the warp-specialised kernel's 8 (H100 80 GB HBM3 at 700 W: 14.3 instead of 18.7 ms for 2^20 bins, DESIGN.md).
 //
 // One persistent CTA per SM; the CTA's kGroups thread groups (256 threads each) are independent tile
-// pipelines that only share the CTA-private histogram.  A group owns three 16.5 KiB slots (tile + 512 B
+// pipelines.  A group owns three 16.5 KiB slots (tile + 512 B
 // of halo so that the one row crossing the tile end can finish in it); slots are filled by
 // cp.async.bulk and signalled on mbarriers, so no thread ever holds raw bytes in registers across stages.
 //
@@ -14,7 +16,7 @@
 //      that tile i-1 just left, ask for the next ticket; warp 0 issues P's look-back loads
 //   d. one thread per newline validates the entry structure of M; warps 1..7 take the rows in chunks of eight: four
 //      threads per row read the row's 16-byte units from the slot, encode + validate them and pass the 2-bit code
-//      words round with shuffles; every k-mer is one funnel shift, one mask and one shared-memory atomic
+//      words round with shuffles; every k-mer is one funnel shift, one mask and one global RED
 //   e. warp 0 resolves P's line prefix (its loads had the whole of d to land).  Warp 0 has no rows: it is the group's
 //      lowest scheduling priority (the SM arbiter favours high warp ids), so its wait for the predecessors' counts
 //      overlaps the other warps' rows instead of following its own.
@@ -34,7 +36,6 @@ constexpr int kSlots = 3;
 constexpr int kRowMax = 1024;                   // longer rows go to the deferred (one warp per segment) pass
 constexpr int kNlCap = 1024;                    // newline positions of one tile kept in shared memory
 constexpr int kNlStep = kNlCap - 8;
-constexpr int kMaxBins = 16384;
 constexpr uint32_t kNoCross = 0xFFFFFFFFu;
 static_assert(kGT == 256 && kGW == 8, "group geometry");
 
@@ -44,7 +45,7 @@ constexpr int kCtlCross = 24;                   // [kSlots] first newline of the
 constexpr int kCtlTk = 28;                      // [2] ticket broadcast
 constexpr int kCtlBase = 32;                    // int64 [2] line index of the tile's first byte
 constexpr int kCtlWords = 48;
-// shared memory after the histogram (bytes)
+// shared memory (bytes)
 constexpr int kOffSlots = 0;
 constexpr int kOffList = kOffSlots + kGroups * kSlots * kSlot;
 constexpr int kOffCtl = kOffList + kGroups * 2 * kNlCap * 2;
@@ -52,60 +53,16 @@ constexpr int kOffBar = kOffCtl + kGroups * kCtlWords * 4;
 constexpr int kOffLut = kOffBar + ((kGroups * kSlots * 8 + 15) & ~15);
 constexpr int kFixedBytes = kOffLut + 256;
 
-__device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_%=:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE_%=;\n"
-        "bra WAIT_%=;\n"
-        "DONE_%=:\n"
-        "}\n" ::"r"(bar), "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-                 "l"(src), "r"(bytes), "r"(bar)
-                 : "memory");
-}
 __device__ __forceinline__ void group_bar(int g) { asm volatile("bar.sync %0, %1;" ::"r"(g + 1), "n"(kGT) : "memory"); }
-__device__ __forceinline__ uint4 lds128(const uint8_t *p) { return *reinterpret_cast<const uint4 *>(p); }
-// PRMT without the selector clean-up __byte_perm adds (all selectors used here have nibbles < 8)
-__device__ __forceinline__ uint32_t prmt(uint32_t lo, uint32_t hi, uint32_t sel) {
-    uint32_t d;
-    asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(lo), "r"(hi), "r"(sel));
-    return d;
-}
-// one count into the CTA-private table (32-bit shared address)
-__device__ __forceinline__ void hist_inc(uint32_t addr) { asm volatile("red.shared.add.u32 [%0], 1;" ::"r"(addr) : "memory"); }
-// ptxas never predicates ATOMS (it branches around it), so a masked count adds 0 or 1 instead
-__device__ __forceinline__ void hist_add_val(uint32_t addr, uint32_t val) { asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(addr), "r"(val) : "memory"); }
 
 // tools/micro/pipe_bench.cu measures the integer pipes: LOP3/SHF/PRMT/IADD3 (ALU pipe) and IMAD (FMA pipe) each issue one
 // warp instruction every two cycles per SM sub-partition, a 50:50 mix reaches 0.65/clk and IMAD.HI only 0.23/clk.
 // This path is all integer work, so instruction count -- not bytes -- is what the kernel time follows.
 
-// bit 7 of every byte that equals '\n' (bit 7 of the pattern is clear, so the last term can use w itself)
-__device__ __forceinline__ uint32_t newline_msb(uint32_t w) {
-    uint32_t x;                                                     // (w ^ 0x0A..) & 0x7F.. as ONE LOP3 (ptxas keeps one
-    asm("lop3.b32 %0, %1, 0x0A0A0A0A, 0x7F7F7F7F, 0x28;" : "=r"(x) : "r"(w));   // constant in a uniform register)
-    const uint32_t s = x + 0x7F7F7F7Fu;
-    return ~(s | w) & 0x80808080u;
-}
 // exact '\n' flags of a 16-byte unit, bit i = byte i.  Per word: the zero-byte test, one IMAD that lines the four
-// flags up in the top nibble of the product and one funnel shift that pushes them into the accumulator.
-__device__ __forceinline__ uint32_t newline_mask16(const uint4 q) {
+// flags up in the top nibble of the product and one funnel shift that pushes them into the accumulator.  (The
+// warp-specialised kernel weighs the flags with IDP.4A instead; that variant has not been timed in this kernel.)
+__device__ __forceinline__ uint32_t newline_mask16_imad(const uint4 q) {
     const uint32_t w[4] = {q.x, q.y, q.z, q.w};
     uint32_t acc = 0;
 #pragma unroll
@@ -114,9 +71,11 @@ __device__ __forceinline__ uint32_t newline_mask16(const uint4 q) {
 }
 
 // 16-byte unit -> 32 bits of 2-bit codes (+ exact validation of the bytes selected by seq16).  Same result
-// as encode_unit_seq; the ASCII alphabets gather the four packed bytes with byte permutes.
+// as encode_unit_seq; the ASCII alphabets gather the four packed bytes with byte permutes and gather the validation
+// flags with IMAD + funnel shift.  (The warp-specialised kernel's encoder packs Gray codes and weighs the flags with
+// IDP.4A; that variant has not been timed in this kernel.)
 template <int ENC>
-__device__ __forceinline__ uint32_t encode_unit(const uint4 q, uint32_t seq16, const uint8_t *s_lut, uint32_t &bad) {
+__device__ __forceinline__ uint32_t encode_unit_imad(const uint4 q, uint32_t seq16, const uint8_t *s_lut, uint32_t &bad) {
     const uint32_t w[4] = {q.x, q.y, q.z, q.w};
     if constexpr (ENC == BNPK_ENC_ASCII_ACGT || ENC == BNPK_ENC_ASCII_ACTG) {
         uint32_t dif[4], pk[4];
@@ -135,7 +94,7 @@ __device__ __forceinline__ uint32_t encode_unit(const uint4 q, uint32_t seq16, c
         if (seq16 == 0xFFFFu) {
             bad = dif[0] | dif[1] | dif[2] | dif[3];
         } else {
-            uint32_t acc = 0;                                       // bit i = byte i of the unit differs (as in newline_mask16)
+            uint32_t acc = 0;                                       // bit i = byte i of the unit differs (as in newline_mask16_imad)
 #pragma unroll
             for (int j = 3; j >= 0; --j) {
                 const uint32_t nz = (((dif[j] & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | dif[j]) & 0x80808080u;  // byte != 0
@@ -149,13 +108,10 @@ __device__ __forceinline__ uint32_t encode_unit(const uint4 q, uint32_t seq16, c
     }
 }
 
-// HIST: 0 = global int64 table, 1 = CTA-private u32 table in shared memory, 2 = global u32 scratch table
+// HIST: 0 = global int64 table, 2 = global u32 scratch table (the numbering of the other fused-count kernels)
 template <int ENC, int HIST>
 __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
-    constexpr bool SMEM_HIST = HIST == 1;
-    extern __shared__ __align__(128) uint8_t smem_raw[];
-    uint32_t *s_hist = reinterpret_cast<uint32_t *>(smem_raw);
-    uint8_t *s_fixed = smem_raw + (SMEM_HIST ? ((a.n_bins * 4 + 127) & ~(uint64_t)127) : 0);
+    extern __shared__ __align__(128) uint8_t s_fixed[];
     const int tid = threadIdx.x, g = tid / kGT, gt = tid % kGT, lane = gt & 31, gw = gt >> 5;
     uint8_t *g_slots = s_fixed + kOffSlots + g * (kSlots * kSlot);
     uint16_t *g_list = reinterpret_cast<uint16_t *>(s_fixed + kOffList) + g * (2 * kNlCap);
@@ -168,8 +124,6 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
     const bool cr = a.status[BNPK_ST_CR] != 0;
 
     if (ENC == BNPK_ENC_LUT && tid < 256) s_lut[tid] = a.lut[tid];
-    if (SMEM_HIST)
-        for (uint32_t b = tid; b < a.n_bins; b += kCta) s_hist[b] = 0;
     if (gt == 0) {
 #pragma unroll
         for (int s = 0; s < kSlots; ++s) mbar_init(g_bar + 8 * s, 1);
@@ -181,7 +135,6 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
     const uint64_t kmask = (1ull << (2 * a.k)) - 1;
     const bool fast = hmask && hmask <= 0x3FFFFFFFull;
     const uint32_t m32x4 = (uint32_t)(hmask & kmask) << 2;       // byte-offset mask into the table
-    const uint32_t hist_sa = smem_addr(s_hist);
     uint32_t acc_bases = 0, acc_values = 0;                         // per thread: well inside 32 bits for any chunk
     const uint32_t ls = (uint32_t)a.lpe_shift, pm = (1u << ls) - 1u;
     const uint32_t fl = (uint32_t)a.field_line;
@@ -222,15 +175,6 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
             mbar_arrive(bar);
         }
     };
-    auto defer_row = [&](uint64_t start, uint64_t r) {
-        const unsigned long long d = atomicAdd((unsigned long long *)(a.ws + kWsDeferred), 1ull);
-        if (d < a.deferred_cap) {
-            a.deferred[2 * d] = start;
-            a.deferred[2 * d + 1] = r;
-        } else {
-            a.status[BNPK_ST_OVERFLOW] = 1;
-        }
-    };
     // front end of one tile (every thread of the group)
     auto front = [&](int32_t tile, int slot, uint32_t parity, uint64_t &nl, uint32_t &ex) {
         const uint8_t *sp = g_slots + slot * kSlot;
@@ -244,7 +188,7 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
         uint32_t m[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            m[j] = newline_mask16(lds128(sp + f_off[j]));
+            m[j] = newline_mask16_imad(lds128(sp + f_off[j]));
         }
         const uint32_t A = m[1] * 65536u + m[0], B = m[3] * 65536u + m[2];
         nl = ((uint64_t)prmt(A, B, sel_hi) << 32) | prmt(A, B, sel_lo);
@@ -261,7 +205,7 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
         if (lane == 31) g_ctl[kCtlWsum + 8 * slot + gw] = inc;
         if (gw == 0) {                                              // first newline of the halo: end of the crossing row
             const int valid = min(max(staged - kTileBytes - 16 * lane, 0), 16);
-            const uint32_t mm = newline_mask16(lds128(sp + kTileBytes + 16 * lane)) & ((1u << valid) - 1u);
+            const uint32_t mm = newline_mask16_imad(lds128(sp + kTileBytes + 16 * lane)) & ((1u << valid) - 1u);
             const unsigned b = __ballot_sync(0xffffffffu, mm != 0);
             const int srcl = b ? __ffs(b) - 1 : 0;
             const uint32_t pos = (uint32_t)(kTileBytes + 16 * lane + __ffs(mm) - 1);
@@ -414,12 +358,12 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
                     } else if (crossM != kNoCross) {
                         e = (int)crossM;
                     } else {                                        // not terminated inside the slot
-                        if (sub == 0 && byte0 + staged < a.n) defer_row(byte0 + b0, (uint64_t)(r_first + s));
+                        if (sub == 0 && byte0 + staged < a.n) defer_row(a, byte0 + b0, (uint64_t)(r_first + s));
                         act = false;                                // (else: unterminated last line, not an entry)
                     }
                     if (act && cr && e > b0 && sp[e - 1] == '\r') e -= 1;
                     if (act && e - b0 > kRowMax) {
-                        if (sub == 0) defer_row(byte0 + b0, (uint64_t)(r_first + s));
+                        if (sub == 0) defer_row(a, byte0 + b0, (uint64_t)(r_first + s));
                         act = false;
                     }
                 }
@@ -444,20 +388,8 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
                     const int lo = max(b0 - 16 * u, 0), hi = min(e - 16 * u, 16);
                     const uint32_t seq16 = (0xFFFFu >> (16 - hi)) & (0xFFFFu << lo);
                     uint32_t bad;
-                    const uint32_t codes = encode_unit<ENC>(q, seq16, s_lut, bad);
-                    if (bad) {                                      // rare: exact position, byte by byte
-                        for (int p = 16 * u + lo; p < 16 * u + hi; ++p) {
-                            const uint32_t c = sp[p];
-                            bool okb;
-                            if (ENC == BNPK_ENC_CODES) okb = c < 4;
-                            else if (ENC == BNPK_ENC_LUT) okb = s_lut[c] < 4;
-                            else { const uint32_t uu = c | 0x20u; okb = (uu == 'a' || uu == 'c' || uu == 'g' || uu == 't'); }
-                            if (!okb) {
-                                atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE], (long long)(((r_first + s) << 32) | (int64_t)(p - b0)));
-                                break;
-                            }
-                        }
-                    }
+                    const uint32_t codes = encode_unit_imad<ENC>(q, seq16, s_lut, bad);
+                    if (bad) report_bad_base<ENC>(a, sp, 16 * u + lo, 16 * u + hi, b0, r_first + s, s_lut);
                     return codes;
                 };
                 uint32_t c_cur = enc(0);
@@ -475,24 +407,12 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
                             const uint32_t p0 = z ? 0u : c_cur, p1 = z ? c_cur : w1, p2 = z ? w1 : w2;
                             const uint32_t sh = (2u * o + 30u) & 31u;
                             const uint32_t a0 = __funnelshift_r(p0, p1, sh), a1 = __funnelshift_r(p1, p2, sh);
-                            if constexpr (SMEM_HIST) {
-                                if (__all_sync(0xffffffffu, left >= 16)) {          // every lane has a full block
 #pragma unroll
-                                    for (int t = 0; t < 16; ++t)
-                                        hist_inc(hist_sa + ((t == 0 ? a0 : __funnelshift_r(a0, a1, 2 * t)) & m32x4));
-                                } else {
-#pragma unroll
-                                    for (int t = 0; t < 16; ++t)
-                                        hist_add_val(hist_sa + ((t == 0 ? a0 : __funnelshift_r(a0, a1, 2 * t)) & m32x4), (uint32_t)(t - left) >> 31);
-                                }
-                            } else {
-#pragma unroll
-                                for (int t = 0; t < 16; ++t) {
-                                    const uint32_t v = (t == 0 ? a0 : __funnelshift_r(a0, a1, 2 * t)) & m32x4;
-                                    if (t < left) {
-                                        if constexpr (HIST == 2) atomicAdd(reinterpret_cast<uint32_t *>(reinterpret_cast<char *>(a.hist32) + v), 1u);
-                                        else atomicAdd(reinterpret_cast<unsigned long long *>(reinterpret_cast<char *>(a.hist) + 2 * (size_t)v), 1ull);
-                                    }
+                            for (int t = 0; t < 16; ++t) {
+                                const uint32_t v = (t == 0 ? a0 : __funnelshift_r(a0, a1, 2 * t)) & m32x4;
+                                if (t < left) {
+                                    if constexpr (HIST == 2) atomicAdd(reinterpret_cast<uint32_t *>(reinterpret_cast<char *>(a.hist32) + v), 1u);
+                                    else atomicAdd(reinterpret_cast<unsigned long long *>(reinterpret_cast<char *>(a.hist) + 2 * (size_t)v), 1ull);
                                 }
                             }
                         }
@@ -510,7 +430,6 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
                                     const uint64_t h = (((uint64_t)hi32 << 32) | lo32) & kmask;
                                     const uint64_t b = hmask ? (h & hmask) : (h % a.n_bins);
                                     if constexpr (HIST == 2) atomicAdd(a.hist32 + b, 1u);
-                                    else if constexpr (HIST == 1) atomicAdd(s_hist + (uint32_t)b, 1u);
                                     else atomicAdd(a.hist + b, 1ull);
                                 }
                             }
@@ -536,13 +455,6 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
     }
 
     // ---- flush ---------------------------------------------------------------------------------------------
-    if (SMEM_HIST) {
-        __syncthreads();
-        for (uint32_t b = tid; b < a.n_bins; b += kCta) {
-            const uint32_t c = s_hist[b];
-            if (c) atomicAdd(a.hist + b, (unsigned long long)c);
-        }
-    }
     const uint64_t sum_bases = warp_sum_u64(acc_bases), sum_values = warp_sum_u64(acc_values);
     if (lane == 0) {
         if (sum_bases) atomicAdd((unsigned long long *)&a.status[BNPK_ST_N_BASES], sum_bases);
@@ -553,8 +465,8 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
 template <int ENC, int HIST>
 static int launch_t(const TileArgs &a, cudaStream_t st) {
     auto kern = tile_tma_kernel<ENC, HIST>;
-    const size_t smem = (size_t)kFixedBytes + (HIST == 1 ? ((a.n_bins * 4 + 127) & ~(uint64_t)127) : 0);
-    BNPK_DYN_SMEM(kern, kFixedBytes + kMaxBins * 4);
+    const size_t smem = (size_t)kFixedBytes;
+    BNPK_DYN_SMEM(kern, kFixedBytes);
     const int64_t n_tiles = a.tile_end - a.tile_begin;
     if (n_tiles <= 0) return 0;
     const int64_t grid = std::min<int64_t>((n_tiles + kGroups - 1) / kGroups, (int64_t)sm_count());
@@ -566,27 +478,25 @@ static int launch_t(const TileArgs &a, cudaStream_t st) {
 }
 
 template <int ENC>
-static int launch_enc(const TileArgs &a, bool smem_hist, cudaStream_t st) {
-    if (smem_hist) return launch_t<ENC, 1>(a, st);
+static int launch_enc(const TileArgs &a, cudaStream_t st) {
     return a.hist32 ? launch_t<ENC, 2>(a, st) : launch_t<ENC, 0>(a, st);
 }
 
 }  // namespace tma
 
+// k-mer counts into global tables; bulk copies need a 16-byte-aligned chunk, tile indices stay in 31 bits
 bool tma_count_eligible(const TileArgs &a, bool smem_hist) {
-    if (a.window != 0) return false;                                        // minimizers: register-staged kernel
-    if ((reinterpret_cast<uintptr_t>(a.chunk) & 15) != 0) return false;     // bulk copies need 16-byte alignment
-    if (smem_hist && a.n_bins > (uint64_t)tma::kMaxBins) return false;
-    if (a.tile_end > 0x7FFFFFF0ll || a.n < 16) return false;
-    return true;
+    if (a.window != 0 || smem_hist) return false;
+    if ((reinterpret_cast<uintptr_t>(a.chunk) & 15) != 0) return false;
+    return a.tile_end <= 0x7FFFFFF0ll && a.n >= 16;
 }
 
-int launch_tma_count(const TileArgs &a, int enc_mode, bool smem_hist, cudaStream_t st) {
+int launch_tma_count(const TileArgs &a, int enc_mode, cudaStream_t st) {
     switch (enc_mode) {
-        case BNPK_ENC_ASCII_ACGT: return tma::launch_enc<BNPK_ENC_ASCII_ACGT>(a, smem_hist, st);
-        case BNPK_ENC_ASCII_ACTG: return tma::launch_enc<BNPK_ENC_ASCII_ACTG>(a, smem_hist, st);
-        case BNPK_ENC_CODES: return tma::launch_enc<BNPK_ENC_CODES>(a, smem_hist, st);
-        case BNPK_ENC_LUT: return tma::launch_enc<BNPK_ENC_LUT>(a, smem_hist, st);
+        case BNPK_ENC_ASCII_ACGT: return tma::launch_enc<BNPK_ENC_ASCII_ACGT>(a, st);
+        case BNPK_ENC_ASCII_ACTG: return tma::launch_enc<BNPK_ENC_ASCII_ACTG>(a, st);
+        case BNPK_ENC_CODES: return tma::launch_enc<BNPK_ENC_CODES>(a, st);
+        case BNPK_ENC_LUT: return tma::launch_enc<BNPK_ENC_LUT>(a, st);
     }
     return set_err(BNPK_E_BADARG, "bad enc_mode");
 }

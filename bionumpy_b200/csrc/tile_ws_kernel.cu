@@ -26,13 +26,17 @@
 #include "tile_ws_kernel.inl"
 
 namespace bnpk {
-// minimizer counts the wsm build takes: CTA-private table, windows of at most kMinzW k-mers; the rest (and global
-// tables) stay with the register-staged kernel
-bool wsm_count_eligible(const TileArgs &a, bool smem_hist) {
-    if (a.window == 0 || !smem_hist || a.n_bins > (uint64_t)wsm::kMaxBins) return false;
-    if (a.window - a.k + 1 > wsm::kMinzW) return false;
+// Both builds count into a CTA-private table of at most kMaxBins bins and stage the chunk by bulk copies, which need a
+// 16-byte-aligned chunk; tile indices stay in 31 bits.
+static bool ws_common_eligible(const TileArgs &a, bool smem_hist) {
+    if (!smem_hist || a.n_bins > (uint64_t)ws::kMaxBins) return false;
     if ((reinterpret_cast<uintptr_t>(a.chunk) & 15) != 0) return false;
-    if (a.tile_end > 0x7FFFFFF0ll || a.n < 16) return false;
-    return true;
+    return a.tile_end <= 0x7FFFFFF0ll && a.n >= 16;
+}
+// k-mer counts
+bool ws_count_eligible(const TileArgs &a, bool smem_hist) { return a.window == 0 && ws_common_eligible(a, smem_hist); }
+// minimizer counts with windows of at most kMinzW k-mers
+bool wsm_count_eligible(const TileArgs &a, bool smem_hist) {
+    return a.window != 0 && a.window - a.k + 1 <= wsm::kMinzW && ws_common_eligible(a, smem_hist);
 }
 }  // namespace bnpk

@@ -81,7 +81,7 @@ def test_dominant_kernels_are_sm90a_code_without_spills():
     assert "sm_90a" in out
     blocks = out.split(" Function ")
     seen = {}
-    for name, regs_max in (("_ZN4bnpk2ws14tile_ws_kernelILi0ELi1EEEvNS_8TileArgsE", 112), ("_ZN4bnpk3wsm14tile_ws_kernelILi0ELi1EEEvNS_8TileArgsE", 88)):
+    for name, regs_max in (("_ZN4bnpk2ws14tile_ws_kernelILi0EEEvNS_8TileArgsE", 112), ("_ZN4bnpk3wsm14tile_ws_kernelILi0EEEvNS_8TileArgsE", 88)):
         blk = next(b for b in blocks if b.startswith(name))
         m = re.search(r"REG:(\d+) STACK:(\d+)", blk)
         assert m, blk[:200]
