@@ -27,6 +27,10 @@ constexpr uint64_t kValueMask = (1ull << 62) - 1;
 constexpr int kWsTicket = 0;        // per-launch tile ticket
 constexpr int kWsDeferred = 1;      // number of deferred (long) rows
 constexpr int kWsCarry = 2;         // newlines in all tiles of the earlier launches (slices) of this chunk
+constexpr int kWsRedo = 3;          // ranges the warp-specialised count counted twice (first line phase guessed wrong)
+// Deferred rows of one 16 KiB tile the warp-specialised count can produce: rows longer than its 1024-byte row walk
+// start more than 1024 bytes apart (<= 16), plus the tile's last row when it ends beyond the slot (1)
+constexpr int kWsDeferPerTile = 17;
 constexpr int kWsHeaderWords = 16;
 
 __device__ __forceinline__ uint64_t ld_relaxed(const uint64_t *p) {

@@ -101,22 +101,26 @@ __device__ __forceinline__ uint32_t encode_unit_seq(const uint32_t *w, uint32_t 
     return codes;
 }
 
-// Rare: the first byte of bytes[p0, p1) outside the alphabet, reported as (entry << 32 | offset from the row's first
-// byte b0).  Called only when an encoder flagged a bad byte in that range.
+// Rare: the first byte of bytes[p0, p1) outside the alphabet, as (entry << 32 | offset from the row's first byte b0)
+// for the BAD_BASE status word (a minimum); INT64_MAX if there is none.  Called only when an encoder flagged a bad
+// byte in that range.
 template <int ENC>
-__device__ __forceinline__ void report_bad_base(const TileArgs &a, const uint8_t *bytes, int p0, int p1, int b0, int64_t entry,
-                                                const uint8_t *s_lut) {
+__device__ __forceinline__ long long first_bad_base(const uint8_t *bytes, int p0, int p1, int b0, int64_t entry, const uint8_t *s_lut) {
     for (int p = p0; p < p1; ++p) {
         const uint32_t c = bytes[p];
         bool okb;
         if (ENC == BNPK_ENC_CODES) okb = c < 4;
         else if (ENC == BNPK_ENC_LUT) okb = s_lut[c] < 4;
         else { const uint32_t uu = c | 0x20u; okb = (uu == 'a' || uu == 'c' || uu == 'g' || uu == 't'); }
-        if (!okb) {
-            atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE], (long long)((entry << 32) | (int64_t)(p - b0)));
-            break;
-        }
+        if (!okb) return (long long)((entry << 32) | (int64_t)(p - b0));
     }
+    return INT64_MAX;
+}
+template <int ENC>
+__device__ __forceinline__ void report_bad_base(const TileArgs &a, const uint8_t *bytes, int p0, int p1, int b0, int64_t entry,
+                                                const uint8_t *s_lut) {
+    const long long v = first_bad_base<ENC>(bytes, p0, p1, b0, entry, s_lut);
+    if (v != INT64_MAX) atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE], v);
 }
 
 // A row the kernel cannot finish (no newline inside the staged bytes, or too long for its row walk): (first byte, entry)

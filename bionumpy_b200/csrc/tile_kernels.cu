@@ -491,13 +491,15 @@ static int launch_count(const TileArgs &a, int enc_mode, bool smem_hist, cudaStr
 
 static size_t deferred_capacity(size_t n) { return n / kHaloBytes + n / 1024 + 16; }
 
-// workspace (uint64 words): header | tile_state[n_tiles+1] | block_cnt[nb] | block_state[nb] | deferred[2*cap]
+// workspace (uint64 words): header | tile_state[n_tiles+1] | block_cnt[nb] | block_state[nb] | deferred[2*cap] |
+// deferred sub-lists[2*kWsDeferPerTile*n_tiles] (the warp-specialised count: one per CTA range, at its first tile)
 static size_t ws_lookback_words(size_t n_tiles) { return kWsHeaderWords + (n_tiles + 1) + 2 * ((n_tiles >> 5) + 2); }
 // ... | u32 scratch[2^24]: large global tables are accumulated in 32-bit counters that stay in L2 (64 MiB instead of
 // 128 MiB of int64: half the traffic per update) and added to the int64 table at the end
 static size_t ws_core_bytes(size_t n) {
     const size_t n_tiles = (n + kTileBytes - 1) / kTileBytes;
-    return (((ws_lookback_words(n_tiles) + 2 * deferred_capacity(n)) * sizeof(uint64_t)) + 255) & ~(size_t)255;
+    return (((ws_lookback_words(n_tiles) + 2 * deferred_capacity(n) + 2 * (size_t)kWsDeferPerTile * n_tiles) * sizeof(uint64_t)) + 255) &
+           ~(size_t)255;
 }
 size_t tile_workspace_bytes(size_t n) { return ws_core_bytes(n) + (size_t)kScratch32MaxBins * sizeof(uint32_t); }
 
