@@ -21,6 +21,7 @@ from .sequence import (get_kmers, get_minimizers, count_encoded, count_kmers, co
 from .streams import streamable, bincount, BnpStream
 from .io import bnp_open, FormatException, IndexedFasta
 from .sequence import KmerIndex, KmerLookup, BloomFilter
+from .sequence import count_kmers_exact, KmerCounter, KmerCounts
 from .io.buffers import CudaFastQBuffer, CudaTwoLineFastaBuffer, FastQBuffer, TwoLineFastaBuffer
 from .io.multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
 from .datatypes import SequenceEntry, SequenceEntryWithQuality

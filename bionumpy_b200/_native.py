@@ -17,7 +17,8 @@ ENC_ASCII_ACGT, ENC_ASCII_ACTG, ENC_CODES, ENC_LUT = 0, 1, 2, 3
 HIST_AUTO, HIST_SMEM, HIST_GLOBAL = 0, 1, 2
 E_BADARG, E_K, E_WINDOW, E_WORKSPACE, E_BINS = -1, -2, -3, -4, -5
 (ST_N_LINES, ST_N_RECORDS, ST_N_COMPLETE_BYTES, ST_BAD_HEADER_ENTRY, ST_BAD_PLUS_ENTRY, ST_BAD_BASE,
- ST_N_BASES, ST_N_VALUES, ST_N_LONG_ROWS, ST_CR, ST_LAST_ROW_START, ST_LAST_ROW_INDEX, ST_OVERFLOW) = range(13)
+ ST_N_BASES, ST_N_VALUES, ST_N_LONG_ROWS, ST_CR, ST_LAST_ROW_START, ST_LAST_ROW_INDEX, ST_OVERFLOW,
+ ST_TABLE_FULL) = range(14)
 ST_WORDS = 16
 INT64_MAX = (1 << 63) - 1
 SMEM_MAX_BINS = 32768
@@ -49,6 +50,8 @@ SIGNATURES = {
     "bnpk_rows_reverse_complement": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
     "bnpk_rows_kmer_hash_canonical": (_i, [_vp, _sz, _vp, _vp, _sz, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "bnpk_rows_kmer_count_canonical": (_i, [_vp, _sz, _vp, _vp, _sz, _i, _vp, _i, _i, _i64, _i, _vp, _vp, _vp]),
+    "bnpk_rows_kmer_table_insert": (_i, [_vp, _sz, _vp, _vp, _sz, _i, _vp, _i, _i, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "bnpk_kmer_table_rehash": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
     "bnpk_bincount": (_i, [_vp, _sz, _i64, _i, _vp, _vp, _vp]),
     "bnpk_bincount_rows": (_i, [_vp, _vp, _sz, _i64, _vp, _vp, _vp]),
     "bnpk_pipeline_create": (_i, [ctypes.POINTER(_vp), _sz, _sz]),

@@ -254,6 +254,64 @@ __device__ __forceinline__ uint64_t canonical_hash(uint64_t h, int k, uint64_t c
     return x < h ? x : h;
 }
 
+// 64-bit mixer (Steele, Lea, Flood: SplitMix64's output function after one increment): the synthetic reads' generator and
+// the home slot of a key in the k-mer table
+__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
+    uint64_t z = x + 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Exact k-mer table: open addressing with linear probing, structure of arrays in global memory.
+// keys[slot] == kTableEmpty marks a free slot; a k-mer hash (k <= 31) is below 2^62, so it never equals -1.
+// The home slot mixes the key: a raw hash's low bits are its first bases, far from uniform on real genomes.
+//
+// Why a plain relaxed load of keys[] is enough (no lock, no second pass):
+//   * a key slot is written at most once, by the CAS that moves it from EMPTY to a key, and never changes afterwards.
+//     So a load that returns a key returns the slot's final value: comparing it with ours is decided for good.
+//   * a load that returns EMPTY may be stale (another thread's CAS has landed since).  We then CAS EMPTY -> key; the
+//     CAS is atomic at L2 and returns the slot's true value: EMPTY (we claimed the slot), our key (someone else
+//     inserted the same k-mer first) or another key (the slot is taken: probe on).  Stale EMPTY is resolved there.
+//   * two threads inserting the same k-mer both probe the same sequence from the same home slot, and every slot before
+//     the one that holds it is already occupied by another key for good, so they cannot end up in different slots.
+//   * counts are only ever incremented with atomicAdd after the slot holds the key; nothing reads them while inserts
+//     run (results and rehash are later kernels on the same stream).
+// ---------------------------------------------------------------------------------------------
+constexpr unsigned long long kTableEmpty = ~0ull;
+
+struct KmerTable {
+    unsigned long long *keys;    // int64[capacity], kTableEmpty = free
+    unsigned long long *counts;  // int64[capacity]
+    uint64_t mask;               // capacity - 1 (capacity a power of two)
+    unsigned long long *n_used;  // slots claimed (device counter, aggregated per warp by the callers)
+};
+
+__device__ __forceinline__ uint64_t table_home(uint64_t key, uint64_t mask) { return splitmix64(key) & mask; }
+
+// add `count` to `key`'s slot.  Returns 1 if this call claimed a free slot, 0 otherwise; probing every slot without
+// finding room drops the key and sets status[BNPK_ST_TABLE_FULL].
+__device__ __forceinline__ uint32_t table_insert(const KmerTable &t, uint64_t key, unsigned long long count,
+                                                 int64_t *status) {
+    uint64_t slot = table_home(key, t.mask);
+    for (uint64_t probes = 0; probes <= t.mask; ++probes) {
+        unsigned long long cur = ld_relaxed(reinterpret_cast<const uint64_t *>(t.keys + slot));
+        uint32_t claimed = 0;
+        if (cur == kTableEmpty) {
+            cur = atomicCAS(t.keys + slot, kTableEmpty, (unsigned long long)key);
+            if (cur == kTableEmpty) { cur = key; claimed = 1; }
+        }
+        if (cur == key) {
+            atomicAdd(t.counts + slot, count);
+            return claimed;
+        }
+        slot = (slot + 1) & t.mask;
+    }
+    atomicExch((unsigned long long *)&status[BNPK_ST_TABLE_FULL], 1ull);
+    return 0;
+}
+
 struct HistTarget {
     unsigned long long *global;  // int64 table in HBM/L2
     uint32_t *smem;              // privatised table (or nullptr)

@@ -299,15 +299,8 @@ __global__ void __launch_bounds__(256) bloom_query_kernel(const int64_t *values,
 }
 
 // ------------------------------------------------------------------------------------------
-// synthetic FASTQ (bit-identical to oracle/bnp_oracle.py:synthetic_fastq)
+// synthetic FASTQ (bit-identical to oracle/bnp_oracle.py:synthetic_fastq; splitmix64 is in bnpk_device.cuh)
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
-    uint64_t z = x + 0x9E3779B97F4A7C15ull;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
-}
-
 __global__ void __launch_bounds__(256) synth_fastq_kernel(uint8_t *out, uint64_t first_record, uint64_t n_records,
                                                           uint64_t seed) {
     const int lane = threadIdx.x & 31;

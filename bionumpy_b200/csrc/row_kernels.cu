@@ -5,6 +5,7 @@
 //   K3 rows_kmer_hash   get_kmers/_get_dna_kmers   sequence/kmers.py:36-126
 //   K4 rows_minimizers  get_minimizers             sequence/minimizers.py:20-54
 //   K3/K4+K5 rows_kmer_count   count_kmers         sequence/kmers.py:129-145
+//   K3 + table rows_kmer_table_insert  exact distinct-k-mer counts (extension, like `jellyfish count`)
 // plus the clean-up passes of the fused chunk count (long rows, trailing incomplete entry).
 #include <climits>
 #include "bnpk_host.h"
@@ -17,7 +18,7 @@ constexpr int kSegUnits = 128;               // 2 KiB staged per warp and segmen
 constexpr int kSegBytes = kSegUnits * 16;
 constexpr int kWarpWords = 2 * kSegUnits + 4;
 
-enum { RM_ENCODE = 0, RM_HASH = 1, RM_MINIMIZER = 2, RM_COUNT = 3, RM_COUNT_MIN = 4 };
+enum { RM_ENCODE = 0, RM_HASH = 1, RM_MINIMIZER = 2, RM_COUNT = 3, RM_COUNT_MIN = 4, RM_TABLE = 5 };
 
 struct RowArgs {
     const uint8_t *base;
@@ -37,13 +38,14 @@ struct RowArgs {
     const uint64_t *deferred;
     size_t deferred_cap;
     int lpe;
-    uint64_t canon_xor;          // != 0: canonical k-mers (hash / count modes without a minimizer window)
+    uint64_t canon_xor;          // != 0: canonical k-mers (hash / count / table modes without a minimizer window)
+    KmerTable table;             // table mode
 };
 
 template <int RM, int ENC, bool SMEM_HIST>
 __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_flags, const uint8_t *s_lut,
                          const HistTarget &ht, int64_t start, int64_t L, int64_t r, int64_t out_off, int lane,
-                         uint64_t &acc_values) {
+                         uint64_t &acc_values, uint64_t *acc_claims = nullptr) {
     constexpr bool MINZ = (RM == RM_MINIMIZER || RM == RM_COUNT_MIN);
     const int span = MINZ ? a.window : (RM == RM_ENCODE ? 1 : a.k);
     const uint64_t kmask = (1ull << (2 * a.k)) - 1;
@@ -105,6 +107,17 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_flags,
                 out[p] = (int64_t)h;
             }
             if (npos > 0) acc_values += (uint64_t)((npos - lane + 31) / 32);
+        } else if constexpr (RM == RM_TABLE) {
+            // the k-mers of RM_HASH, inserted into the table instead of written out
+            const int npos = seg_len - span + 1;
+            uint32_t claimed = 0;
+            for (int p = lane; p < npos; p += 32) {
+                uint64_t h = stream_64(w_codes, (uint32_t)(off + p)) & kmask;
+                if (a.canon_xor) h = canonical_hash(h, a.k, a.canon_xor);
+                claimed += table_insert(a.table, h, 1ull, a.status);
+            }
+            if (npos > 0) acc_values += (uint64_t)((npos - lane + 31) / 32);
+            *acc_claims += claimed;
         } else if constexpr (RM == RM_MINIMIZER) {
             int64_t *out = reinterpret_cast<int64_t *>(a.out) + out_off + seg_start;
             const int w = a.window - a.k + 1;
@@ -140,8 +153,10 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_flags,
     }
 }
 
+// Table mode asks for 4 CTAs per SM (<= 64 registers): without a minimum, ptxas keeps the row loop's 64-bit
+// accumulators on the stack in the code-byte build.  0 = no minimum, the other modes' code is unchanged by it.
 template <int RM, int ENC, bool SMEM_HIST, bool DEFERRED>
-__global__ void __launch_bounds__(kRowThreads) rows_kernel(const RowArgs a) {
+__global__ void __launch_bounds__(kRowThreads, RM == RM_TABLE ? 4 : 0) rows_kernel(const RowArgs a) {
     extern __shared__ __align__(16) uint32_t smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint32_t *w_codes = smem + warp * kWarpWords;
@@ -161,7 +176,7 @@ __global__ void __launch_bounds__(kRowThreads) rows_kernel(const RowArgs a) {
     ht.canon_xor = a.canon_xor;
     __syncthreads();
 
-    uint64_t acc_values = 0, acc_bases = 0, acc_long = 0;
+    uint64_t acc_values = 0, acc_bases = 0, acc_long = 0, acc_claims = 0;
     size_t n_rows = a.n_rows;
     int64_t n_records = 0;
     bool cr = false;
@@ -188,7 +203,7 @@ __global__ void __launch_bounds__(kRowThreads) rows_kernel(const RowArgs a) {
         }
         if (L <= 0) continue;
         if (lane == 0) acc_bases += (uint64_t)L;
-        warp_row<RM, ENC, SMEM_HIST>(a, w_codes, w_flags, s_lut, ht, start, L, r, out_off, lane, acc_values);
+        warp_row<RM, ENC, SMEM_HIST>(a, w_codes, w_flags, s_lut, ht, start, L, r, out_off, lane, acc_values, &acc_claims);
     }
     if (COUNTING && SMEM_HIST) {
         __syncthreads();
@@ -205,6 +220,22 @@ __global__ void __launch_bounds__(kRowThreads) rows_kernel(const RowArgs a) {
         if (acc_bases) atomicAdd((unsigned long long *)&a.status[BNPK_ST_N_BASES], acc_bases);
         if (acc_long) atomicAdd((unsigned long long *)&a.status[BNPK_ST_N_LONG_ROWS], acc_long);
     }
+    if constexpr (RM == RM_TABLE) {
+        acc_claims = warp_sum_u64(acc_claims);
+        if (lane == 0 && acc_claims) atomicAdd(a.table.n_used, (unsigned long long)acc_claims);
+    }
+}
+
+// Growth: one thread per slot of the old table re-inserts its (key, count) into the new one with the same slot function.
+__global__ void __launch_bounds__(256) table_rehash_kernel(const int64_t *keys, const int64_t *counts, size_t capacity,
+                                                           const KmerTable t, int64_t *status) {
+    uint64_t claimed = 0;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < capacity; i += (size_t)gridDim.x * blockDim.x) {
+        const unsigned long long key = (unsigned long long)keys[i];
+        if (key != kTableEmpty) claimed += table_insert(t, key, (unsigned long long)counts[i], status);
+    }
+    claimed = warp_sum_u64(claimed);
+    if ((threadIdx.x & 31) == 0 && claimed) atomicAdd(t.n_used, (unsigned long long)claimed);
 }
 
 // Un-count the sequence line of a trailing incomplete entry: the fused pass counts every
@@ -478,6 +509,38 @@ int bnpk_rows_kmer_count_canonical(const uint8_t *base, size_t base_bytes, const
     cudaStream_t st = (cudaStream_t)stream;
     return use_smem_hist(n_bins, hist_mode) ? launch_rows_enc<RM_COUNT, true, false>(a, enc_mode, n_rows, st)
                                             : launch_rows_enc<RM_COUNT, false, false>(a, enc_mode, n_rows, st);
+}
+
+static bool is_pow2(size_t c) { return c && (c & (c - 1)) == 0; }
+
+int bnpk_rows_kmer_table_insert(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                                size_t n_rows, int enc_mode, const uint8_t *lut256, int k, int complement_xor,
+                                int64_t *keys, int64_t *counts, size_t capacity, int64_t *n_used,
+                                int64_t *status, void *stream) {
+    if (int rc = check_common(enc_mode, lut256, k, 0)) return rc;
+    if (complement_xor < 0 || complement_xor > 3) return set_err(BNPK_E_BADARG, "complement_xor must be 0, 1, 2 or 3");
+    if (!is_pow2(capacity)) return set_err(BNPK_E_BADARG, "table capacity must be a power of two");
+    if (n_rows == 0) return 0;
+    RowArgs a{};
+    a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
+    a.k = k; a.n_bins = 1; a.status = status;
+    a.canon_xor = complement_xor ? canon_pattern(complement_xor) : 0;
+    a.table.keys = (unsigned long long *)keys; a.table.counts = (unsigned long long *)counts;
+    a.table.mask = capacity - 1; a.table.n_used = (unsigned long long *)n_used;
+    return launch_rows_enc<RM_TABLE, false, false>(a, enc_mode, n_rows, (cudaStream_t)stream);
+}
+
+int bnpk_kmer_table_rehash(const int64_t *keys, const int64_t *counts, size_t capacity,
+                           int64_t *new_keys, int64_t *new_counts, size_t new_capacity, int64_t *n_used,
+                           int64_t *status, void *stream) {
+    if (!is_pow2(capacity) || !is_pow2(new_capacity)) return set_err(BNPK_E_BADARG, "table capacity must be a power of two");
+    KmerTable t;
+    t.keys = (unsigned long long *)new_keys; t.counts = (unsigned long long *)new_counts;
+    t.mask = new_capacity - 1; t.n_used = (unsigned long long *)n_used;
+    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((capacity + 255) / 256, (size_t)sm_count() * 8));
+    table_rehash_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(keys, counts, capacity, t, status);
+    BNPK_LAUNCHED("table_rehash_kernel");
+    return 0;
 }
 
 int bnpk_rows_reverse_complement(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,

@@ -157,6 +157,26 @@ Tensor rows_kmer_count(const Tensor &base, const Tensor &starts, const Tensor &l
     return status;
 }
 
+// exact k-mer table: insert every k-mer of the rows (mutates keys, counts, n_used).  Returns the status block.
+Tensor rows_kmer_table_insert(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t enc_mode,
+                              const c10::optional<Tensor> &lut, int64_t k, int64_t complement_xor, Tensor keys,
+                              Tensor counts, Tensor n_used) {
+    need_rows(base, starts, lens);
+    need(keys, torch::kInt64, "keys");
+    need(counts, torch::kInt64, "counts");
+    need(n_used, torch::kInt64, "n_used");
+    TORCH_CHECK(keys.numel() == counts.numel() && n_used.numel() == 1, "bnpk: keys/counts differ in length or n_used is not one word");
+    c10::cuda::CUDAGuard guard(base.device());
+    Tensor status = new_status(base);
+    check(bnpk_rows_kmer_table_insert(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
+                                      lens.data_ptr<int32_t>(), (size_t)lens.numel(), (int)enc_mode, lut ? u8(*lut) : nullptr,
+                                      (int)k, (int)complement_xor, keys.data_ptr<int64_t>(), counts.data_ptr<int64_t>(),
+                                      (size_t)keys.numel(), n_used.data_ptr<int64_t>(), status.data_ptr<int64_t>(),
+                                      cur_stream(base)),
+          "rows_kmer_table_insert");
+    return status;
+}
+
 Tensor rows_reverse_complement(const Tensor &base, const Tensor &starts, const Tensor &lens, const Tensor &lut,
                                const Tensor &offsets, int64_t total) {
     need_rows(base, starts, lens);
@@ -197,6 +217,8 @@ TORCH_LIBRARY(bnpk, m) {
           "int complement_xor, Tensor offsets, int total) -> (Tensor, Tensor)");
     m.def("rows_kmer_count(Tensor base, Tensor starts, Tensor lens, int enc_mode, Tensor? lut, int k, int window_size, "
           "int complement_xor, Tensor(a!) hist, int hist_mode=0) -> Tensor");
+    m.def("rows_kmer_table_insert(Tensor base, Tensor starts, Tensor lens, int enc_mode, Tensor? lut, int k, "
+          "int complement_xor, Tensor(a!) keys, Tensor(b!) counts, Tensor(c!) n_used) -> Tensor");
     m.def("rows_reverse_complement(Tensor base, Tensor starts, Tensor lens, Tensor lut, Tensor offsets, int total) -> Tensor");
     m.def("bincount(Tensor values, Tensor(a!) hist, int hist_mode=0) -> Tensor");
 }
@@ -208,6 +230,7 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("rows_encode", &rows_encode);
     m.impl("rows_kmer_hash", &rows_kmer_hash);
     m.impl("rows_kmer_count", &rows_kmer_count);
+    m.impl("rows_kmer_table_insert", &rows_kmer_table_insert);
     m.impl("rows_reverse_complement", &rows_reverse_complement);
     m.impl("bincount", &bincount);
 }

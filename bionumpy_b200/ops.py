@@ -250,6 +250,40 @@ def rows_kmer_count_canonical(base, starts, lens, enc_mode, k, complement_xor, n
     return hist, status
 
 
+def _table_args(keys, counts, n_used):
+    for t, name in ((keys, "keys"), (counts, "counts"), (n_used, "n_used")):
+        _need_cuda(t, name)
+        if t.dtype != torch.int64:
+            raise TypeError(f"{name} must be int64")
+    if counts.numel() != keys.numel() or n_used.numel() != 1:
+        raise ValueError("keys and counts must have the same length and n_used one element")
+    return ptr(keys), ptr(counts), keys.numel(), ptr(n_used)
+
+
+@_on_device
+def rows_kmer_table_insert(base, starts, lens, enc_mode, k, keys, counts, n_used, complement_xor=0, lut=None,
+                           status=None):
+    """EXTENSION: insert every k-mer of the rows (canonical ones when complement_xor != 0) into the exact table
+    (keys, counts: int64[C], C a power of two, free slot = key -1); n_used (int64[1]) grows by the slots claimed.
+    Returns the status tensor."""
+    if status is None:
+        status = nv.new_status(base.device)
+    check(lib().bnpk_rows_kmer_table_insert(*_rows_args(base, starts, lens), enc_mode, ptr(lut), k, complement_xor,
+                                            *_table_args(keys, counts, n_used), ptr(status), stream_ptr()))
+    return status
+
+
+@_on_device
+def kmer_table_rehash(keys, counts, new_keys, new_counts, n_used, status=None):
+    """Re-insert every (key, count) of a table into a cleared one (growth); n_used grows by the slots claimed there."""
+    if status is None:
+        status = nv.new_status(keys.device)
+    k_p, c_p, cap, _ = _table_args(keys, counts, n_used)
+    nk_p, nc_p, new_cap, u_p = _table_args(new_keys, new_counts, n_used)
+    check(lib().bnpk_kmer_table_rehash(k_p, c_p, cap, nk_p, nc_p, new_cap, u_p, ptr(status), stream_ptr()))
+    return status
+
+
 @_on_device
 def bincount(values, n_bins, hist=None, hist_mode=nv.HIST_AUTO, status=None):
     _need_cuda(values, "values")

@@ -76,6 +76,20 @@ def _split_long_rows(starts, lens, span, out_offsets=None, piece=LONG_ROW):
     return p_start.contiguous(), p_len.to(torch.int32).contiguous(), p_off
 
 
+def _check_bad_base(source: _Source, status, split=False):
+    """Raise the reference's EncodingError(offset) if the status block reports a byte outside the alphabet.  With
+    ``split``, the kernel ran on other rows than ``source``'s (pieces of long rows, batches), so the (row, position)
+    is recomputed on the source rows (error path)."""
+    bad = ops.read_status(status).bad_base()
+    if bad is not None and split:
+        _, status = ops.rows_kmer_count(source.base, source.starts, source.lens, source.enc_mode, 1, 4, 0, source.lut)
+        bad = ops.read_status(status).bad_base()
+    if bad is not None:
+        logging.error("Tried to change encoding of sequences to DNAEncoding, but failed. "
+                      "Make sure your sequences are valid DNA, only containing A, C, G, and T")
+        source.alphabet_encoding._raise_encoding_error(bad[0], bad[1], source.lens)
+
+
 class LazyKmerValues(EncodedRaggedArray):
     """EncodedRaggedArray of k-mer hashes / minimizers whose int64 data appear on first use."""
 
@@ -138,16 +152,7 @@ class LazyKmerValues(EncodedRaggedArray):
         return self._lazy is not None
 
     def _check(self, status, split=False):
-        bad = ops.read_status(status).bad_base()
-        if bad is not None and split:
-            # the (row, position) refers to a piece of a long row: recompute on the unsplit rows (error path)
-            s = self._source
-            _, status = ops.rows_kmer_count(s.base, s.starts, s.lens, s.enc_mode, 1, 4, 0, s.lut)
-            bad = ops.read_status(status).bad_base()
-        if bad is not None:
-            logging.error("Tried to change encoding of sequences to DNAEncoding, but failed. "
-                          "Make sure your sequences are valid DNA, only containing A, C, G, and T")
-            self._source.alphabet_encoding._raise_encoding_error(bad[0], bad[1], self._source.lens)
+        _check_bad_base(self._source, status, split)
 
     def fused_histogram(self, n_bins: int) -> torch.Tensor:
         """hist[b] = #{values == b (mod n_bins)} without writing the values (K3/K4 + K5 fused)."""

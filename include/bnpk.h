@@ -74,6 +74,8 @@ enum {
     BNPK_ST_LAST_ROW_INDEX = 11, /* internal: 1 + its entry index                          */
     BNPK_ST_OVERFLOW = 12,     /* != 0: the fused pass met more long/odd rows than its scratch holds;
                                   the counts are incomplete -- use bnpk_line_split + bnpk_rows_kmer_count */
+    BNPK_ST_TABLE_FULL = 13,   /* != 0: a k-mer table insert probed every slot without finding room; the table misses
+                                  k-mers.  Callers that keep the table at most half full never see it */
     BNPK_ST_WORDS = 16
 };
 
@@ -199,6 +201,27 @@ int bnpk_rows_kmer_hash_canonical(const uint8_t *base, size_t base_bytes, const 
 int bnpk_rows_kmer_count_canonical(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
                                    size_t n_rows, int enc_mode, const uint8_t *lut256, int k, int complement_xor,
                                    int64_t n_bins, int hist_mode, int64_t *hist, int64_t *status, void *stream);
+
+/* EXTENSION (no reference counterpart; what `jellyfish count` produces, benchmarks/rules/kmer_counting.smk:1-31): exact
+ *     counts of distinct k-mers, any k in 1..31, in an open-addressing hash table in device memory.
+ *     Table = keys int64[capacity] + counts int64[capacity], capacity a power of two; a free slot has key -1 and count 0
+ *     (clear a table by filling keys with -1 and counts with 0).  Key = the k-mer hash of bnpk_rows_kmer_hash (with
+ *     complement_xor 1..3: the canonical hash of bnpk_rows_kmer_hash_canonical; 0 = forward k-mers); its home slot is
+ *     splitmix64(key) mod capacity, collisions probe linearly.  The k-mers of every row are inserted (count + 1 each);
+ *     *n_used (device int64) is increased by the number of slots this call claimed.  The caller keeps the table at most
+ *     half full (n_used + positions of the call <= capacity / 2), so an insert always finds room; if it does not, the
+ *     k-mer is dropped and status[BNPK_ST_TABLE_FULL] is set.  Bad bases are reported as by bnpk_rows_kmer_hash, but the
+ *     row's k-mers are still inserted.  BNPK_E_BADARG for a capacity that is not a power of two, BNPK_E_K for k
+ *     outside 1..31. */
+int bnpk_rows_kmer_table_insert(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                                size_t n_rows, int enc_mode, const uint8_t *lut256, int k, int complement_xor,
+                                int64_t *keys, int64_t *counts, size_t capacity, int64_t *n_used,
+                                int64_t *status, void *stream);
+/*     Growth: every (key, count) of a table is inserted into a second (cleared, larger) table with the same slot function;
+ *     *n_used is increased by the slots claimed there.  Both capacities must be powers of two. */
+int bnpk_kmer_table_rehash(const int64_t *keys, const int64_t *counts, size_t capacity,
+                           int64_t *new_keys, int64_t *new_counts, size_t new_capacity, int64_t *n_used,
+                           int64_t *status, void *stream);
 
 /* K5  np.bincount(values % n_bins, minlength=n_bins) accumulated into hist
  *     (sequence/count_encoded.py:173-177; EncodedArray.__array_function__ encoded_array.py:459-460).
