@@ -64,7 +64,7 @@ int bnpk_pipeline_kmer_count_host_on(bnpk_pipeline *p, const uint8_t *chunk_host
                                      uint8_t header_char, int check_plus, int trim_cr, int enc_mode,
                                      const uint8_t *lut256_host, int k, int window_size, int64_t n_bins, int hist_mode,
                                      int64_t *hist, int64_t *status_host, void *stream) {
-    if (!p || !chunk_host || !status_host) return set_err(BNPK_E_BADARG, "null argument");
+    if (!p || (!chunk_host && n) || !status_host) return set_err(BNPK_E_BADARG, "null argument");
     if (n > p->capacity) return set_err(BNPK_E_BADARG, "chunk larger than the pipeline capacity");
     cudaStream_t cs = p->compute_stream;
     // the private streams do not synchronise with anybody: order the count after what the caller has queued

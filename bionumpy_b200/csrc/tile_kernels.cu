@@ -545,9 +545,13 @@ int chunk_kmer_count_impl(const uint8_t *chunk, size_t n, size_t slice_begin, si
     a.deferred_cap = deferred_capacity(n);
     a.deferred = (uint64_t *)workspace + ws_lookback_words((size_t)n_tiles_total);
     a.lut = lut256; a.k = k; a.window = window; a.n_bins = (uint64_t)n_bins; a.hist = (unsigned long long *)hist;
-    if (slice_begin == 0) {
+    if (slice_begin == 0)
         BNPK_CUDA(cudaMemsetAsync(workspace, 0, ws_lookback_words((size_t)n_tiles_total) * sizeof(uint64_t), st));
-        cr_detect_kernel<<<1, 32, 0, st>>>(chunk, std::min(n, slice_end), lpe, trim_cr, status);
+    // '\r' trimming is decided by the call that counts tile 0, from every byte resident by then (at least one tile
+    // and its halo): earlier calls count no tile, so no kernel reads the decision before it is taken.  Slices are
+    // consecutive, so this is the only call with tile_begin == 0 that counts anything.
+    if (a.tile_begin == 0 && a.tile_end > 0) {
+        cr_detect_kernel<<<1, 32, 0, st>>>(chunk, final_slice ? n : slice_end, lpe, trim_cr, status);
         BNPK_LAUNCHED("cr_detect_kernel");
     }
     BNPK_CUDA(cudaMemsetAsync(a.ws + kWsTicket, 0, sizeof(uint64_t), st));

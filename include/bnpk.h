@@ -135,6 +135,16 @@ int bnpk_line_split(const uint8_t *chunk, size_t n, int lines_per_entry, int fie
  *     hist is int64[n_bins] and is ACCUMULATED into (zero it yourself for a fresh count).
  *     Chunks may be fed in slices: call with the same workspace/status and consecutive
  *     [slice_begin, slice_end) byte ranges of one resident buffer; `final` marks the last.
+ *     Residency: a non-final call reads only chunk[0, slice_end), so the bytes from slice_end
+ *     on may still be in flight (the host pipeline copies slice s+1 while slice s is counted);
+ *     the final call may read all n bytes.  Empty slices and an empty final slice [n, n) are
+ *     allowed.  A call counts the 16 KiB tiles whose bytes and 2 KiB halo are resident, so
+ *     calls that end before byte 18432 (and are not final) count nothing.
+ *     '\r' trimming (trim_cr = -1) is decided by the call that counts the first tile, from all
+ *     bytes resident then: at least 18 KiB, or the whole chunk.  A sliced count can therefore
+ *     differ from a one-shot launch only if the first header line lacks '\r', a later one of
+ *     the first lines_per_entry headers ends in '\r', and those headers do not all lie in the
+ *     bytes resident at that call.
  * ------------------------------------------------------------------------------------- */
 int bnpk_chunk_kmer_count(const uint8_t *chunk, size_t n, size_t slice_begin, size_t slice_end,
                           int final_slice, int lines_per_entry, uint8_t header_char, int check_plus,
