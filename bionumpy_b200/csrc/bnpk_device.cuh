@@ -1,12 +1,12 @@
 // bnpk_device.cuh -- shared device helpers for the sm_90a k-mer hot path.
 //
-// Data model (see DESIGN.md):
-//   every 16-byte unit of the raw chunk is turned, in registers, into
-//     codes32 : 2 bits per byte  (byte j of the unit at bits 2j)  -> a contiguous 2-bit stream
-//     flags32 : low 16 bits = "byte is '\n'", high 16 bits = "byte is a valid base"
-//   and only those 8 bytes per unit are kept in shared memory.  A k-mer starting at byte b is
-//   the 2k-bit field at bit 2b of the packed stream (first base in the lowest bits), which is
-//   exactly the reference hash sum_j code[i+j]*4^j (sequence/kmers.py:105-126).
+// Every kernel that reads sequence bytes classifies them here, one 16-byte unit at a time (see DESIGN.md):
+//   newline_mask16 : bit i = "byte i is '\n'"
+//   encode_unit    : 2 bits per byte (byte j of the unit at bits 2j) -> a contiguous 2-bit stream, and which bytes are
+//                    outside the alphabet of the encoding
+//   first_bad_base : the same alphabets one byte at a time, for the rare rescan of a row that holds a bad byte
+// A k-mer starting at byte b is the 2k-bit field at bit 2b of the packed stream (first base in the lowest bits), which
+// is exactly the reference hash sum_j code[i+j]*4^j (sequence/kmers.py:105-126).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -115,60 +115,101 @@ __device__ __forceinline__ uint64_t lookback_exclusive(uint64_t *state, int64_t 
 }
 
 // ---------------------------------------------------------------------------------------------
-// byte -> code / flag transforms, four bytes at a time
+// byte classes of a 16-byte unit: the one statement of the alphabets, used by every kernel
 // ---------------------------------------------------------------------------------------------
-// gather bit 0 of each byte into a nibble (bits 0..3)
-__device__ __forceinline__ uint32_t bytes_lsb_to_nibble(uint32_t m01) {
-    return ((m01 & 0x01010101u) * 0x00204081u >> 21) & 0xFu;
+// Integer pipes of an SM sub-partition (tools/micro/pipe_bench.cu): LOP3/SHF/PRMT/IADD3 (ALU pipe) and IMAD /
+// IDP.4A (FMA pipe) each issue one warp instruction every two cycles, any mix of the two 0.65 per cycle; POPC one
+// every 8 cycles, ffs (BREV + FLO) one every 16.  This path is all integer work: instruction count sets the time.
+
+// PRMT without the selector clean-up __byte_perm adds (all selectors used here are in range)
+__device__ __forceinline__ uint32_t prmt(uint32_t lo, uint32_t hi, uint32_t sel) {
+    uint32_t d;
+    asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(lo), "r"(hi), "r"(sel));
+    return d;
 }
-// gather the low 2 bits of each byte into 8 bits
-__device__ __forceinline__ uint32_t bytes_2bit_to_byte(uint32_t x03) {
-    return (x03 * 0x01041040u) >> 24;
+// bit 7 of every byte that equals '\n' (bit 7 of the pattern is clear, so the last term can use w itself)
+__device__ __forceinline__ uint32_t newline_msb(uint32_t w) {
+    uint32_t x;                                                     // (w ^ 0x0A..) & 0x7F.. as ONE LOP3
+    asm("lop3.b32 %0, %1, 0x0A0A0A0A, 0x7F7F7F7F, 0x28;" : "=r"(x) : "r"(w));
+    const uint32_t s = x + 0x7F7F7F7Fu;
+    return ~(s | w) & 0x80808080u;
 }
 
-template <int ENC>
-__device__ __forceinline__ void encode_word(uint32_t w, const uint8_t *s_lut, uint32_t &code8, uint32_t &valid4) {
-    if constexpr (ENC == BNPK_ENC_ASCII_ACGT || ENC == BNPK_ENC_ASCII_ACTG) {
-        uint32_t x;
-        if constexpr (ENC == BNPK_ENC_ASCII_ACGT)
-            x = ((w >> 1) ^ (w >> 2)) & 0x03030303u;  // A0 C1 G2 T3
-        else
-            x = (w >> 1) & 0x03030303u;                // A0 C1 T2 G3
-        code8 = bytes_2bit_to_byte(x);
-        const uint32_t u = w | 0x20202020u;            // fold case (alphabet_encoding.py:24-28)
-        const uint32_t eq = __vcmpeq4(u, 0x61616161u) | __vcmpeq4(u, 0x63636363u) |
-                            __vcmpeq4(u, 0x67676767u) | __vcmpeq4(u, 0x74747474u);
-        valid4 = bytes_lsb_to_nibble(eq);
-    } else if constexpr (ENC == BNPK_ENC_CODES) {
-        code8 = bytes_2bit_to_byte(w & 0x03030303u);
-        valid4 = bytes_lsb_to_nibble(__vcmpeq4(w & 0xFCFCFCFCu, 0u));
-    } else {
-        uint32_t c = 0, v = 0;
+// exact '\n' flags of a 16-byte unit, bit i = byte i: the flag bytes are 0x80 or 0, one IDP.4A per word weighs
+// them into place (4 instructions per word, two of them on the FMA pipe)
+__device__ __forceinline__ uint32_t newline_mask16(const uint4 q) {
+    uint32_t lo = __dp4a(newline_msb(q.x), 0x08040201u, 0u);
+    lo = __dp4a(newline_msb(q.y), 0x80402010u, lo);                // 128 * (flags of bytes 0..7)
+    uint32_t hi = __dp4a(newline_msb(q.z), 0x08040201u, 0u);
+    hi = __dp4a(newline_msb(q.w), 0x80402010u, hi);                // 128 * (flags of bytes 8..15)
+    return (lo >> 7) | (hi << 1);
+}
+
+// 16-byte unit -> 32 bits of 2-bit codes; `bad` != 0 iff a byte of the unit (WHOLE) or a byte selected by seq16
+// (!WHOLE) is outside the alphabet (exact).  !WHOLE: `bad` is the 16-bit mask of those bytes, bit i = byte i.
+// ASCII alphabets: bits 1-2 of a letter are a Gray code of its index (A 00, C 01, G 11, T 10).  Per word: one LOP3
+// isolates them, one IMAD packs the four fields into the top byte, one IMAD lines them up as PRMT selector nibbles,
+// PRMT looks the expected lower-case letter up, LOP3 compares it with the case-folded input; per unit: three PRMT
+// gather the packed bytes and (ACGT only) two ops turn Gray into binary for all sixteen bases at once.
+template <int ENC, bool WHOLE>
+__device__ __forceinline__ uint32_t encode_unit(const uint4 q, uint32_t seq16, const uint8_t *s_lut, uint32_t &bad) {
+    const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+    if constexpr (ENC == BNPK_ENC_ASCII_ACGT || ENC == BNPK_ENC_ASCII_ACTG || ENC == BNPK_ENC_CODES) {
+        uint32_t dif[4], pk[4];
 #pragma unroll
-        for (int b = 0; b < 4; ++b) {
-            const uint32_t code = s_lut[(w >> (8 * b)) & 0xFFu];
-            c |= (code & 3u) << (2 * b);
-            v |= (code < 4u ? 1u : 0u) << b;
+        for (int j = 0; j < 4; ++j) {
+            if constexpr (ENC == BNPK_ENC_CODES) {
+                pk[j] = (w[j] & 0x03030303u) * 0x01041040u;
+                dif[j] = w[j] & 0xFCFCFCFCu;
+            } else {
+                const uint32_t g2 = w[j] & 0x06060606u;
+                pk[j] = g2 * 0x00820820u;                           // top byte = the four 2-bit fields
+                const uint32_t sel = prmt(g2 * 0x110u, 0u, 0x4431u);   // nibbles = 2 * field: 0 a, 2 c, 4 t, 6 g
+                dif[j] = prmt(0x00630061u, 0x00670074u, sel) ^ (w[j] | 0x20202020u);
+            }
         }
-        code8 = c;
-        valid4 = v;
+        uint32_t codes = prmt(prmt(pk[0], pk[1], 0x0073), prmt(pk[2], pk[3], 0x0073), 0x5410);
+        if constexpr (ENC == BNPK_ENC_ASCII_ACGT) codes ^= (codes >> 1) & 0x55555555u;
+        if constexpr (WHOLE) {
+            bad = dif[0] | dif[1] | dif[2] | dif[3];
+        } else {
+            // byte != 0 flags (bit 7 of every byte), weighed into a 16-bit mask like the newline flags
+            uint32_t nz[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) nz[j] = (((dif[j] & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | dif[j]) & 0x80808080u;
+            const uint32_t lo = __dp4a(nz[1], 0x80402010u, __dp4a(nz[0], 0x08040201u, 0u));
+            const uint32_t hi = __dp4a(nz[3], 0x80402010u, __dp4a(nz[2], 0x08040201u, 0u));
+            bad = ((lo >> 7) | (hi << 1)) & seq16;
+        }
+        return codes;
+    } else {
+        uint32_t codes = 0;
+        bad = 0;
+#pragma unroll
+        for (int b = 0; b < 16; ++b) {
+            const uint32_t code = s_lut[(w[b >> 2] >> (8 * (b & 3))) & 0xFFu];
+            codes |= (code & 3u) << (2 * b);
+            bad |= ((code >= 4u) ? 1u : 0u) << b;
+        }
+        if constexpr (!WHOLE) bad &= seq16;
+        return codes;
     }
 }
 
-// one 16-byte unit -> (codes32, flags32)
+// The same alphabets one byte at a time, for the rare rescan of a row some encode_unit flagged: the first byte of
+// bytes[p0, p1) outside the alphabet, as (entry << 32 | offset from the row's first byte b0) for the BAD_BASE status
+// word (a minimum); INT64_MAX if there is none.
 template <int ENC>
-__device__ __forceinline__ void encode_unit(const uint4 q, const uint8_t *s_lut, uint32_t &codes, uint32_t &flags) {
-    uint32_t c0, c1, c2, c3, v0, v1, v2, v3;
-    encode_word<ENC>(q.x, s_lut, c0, v0);
-    encode_word<ENC>(q.y, s_lut, c1, v1);
-    encode_word<ENC>(q.z, s_lut, c2, v2);
-    encode_word<ENC>(q.w, s_lut, c3, v3);
-    codes = c0 | (c1 << 8) | (c2 << 16) | (c3 << 24);
-    const uint32_t nl = bytes_lsb_to_nibble(__vcmpeq4(q.x, 0x0A0A0A0Au)) |
-                        (bytes_lsb_to_nibble(__vcmpeq4(q.y, 0x0A0A0A0Au)) << 4) |
-                        (bytes_lsb_to_nibble(__vcmpeq4(q.z, 0x0A0A0A0Au)) << 8) |
-                        (bytes_lsb_to_nibble(__vcmpeq4(q.w, 0x0A0A0A0Au)) << 12);
-    flags = nl | ((v0 | (v1 << 4) | (v2 << 8) | (v3 << 12)) << 16);
+__device__ __forceinline__ long long first_bad_base(const uint8_t *bytes, int p0, int p1, int b0, int64_t entry, const uint8_t *s_lut) {
+    for (int p = p0; p < p1; ++p) {
+        const uint32_t c = bytes[p];
+        bool okb;
+        if (ENC == BNPK_ENC_CODES) okb = c < 4;
+        else if (ENC == BNPK_ENC_LUT) okb = s_lut[c] < 4;
+        else { const uint32_t uu = c | 0x20u; okb = (uu == 'a' || uu == 'c' || uu == 'g' || uu == 't'); }
+        if (!okb) return (long long)((entry << 32) | (int64_t)(p - b0));
+    }
+    return INT64_MAX;
 }
 
 // load a 16-byte unit that may stick out of [0, n): out-of-range bytes read as 0
@@ -194,9 +235,7 @@ __device__ __forceinline__ int64_t warp_line_len(const uint8_t *base, size_t n, 
         const int64_t ub = u0 + 16 * (int64_t)lane;
         uint32_t m = 0;
         if (ub < (int64_t)n) {
-            const uint4 q = load_unit_guarded(base, n, ub);
-            m = bytes_lsb_to_nibble(__vcmpeq4(q.x, 0x0A0A0A0Au)) | (bytes_lsb_to_nibble(__vcmpeq4(q.y, 0x0A0A0A0Au)) << 4) |
-                (bytes_lsb_to_nibble(__vcmpeq4(q.z, 0x0A0A0A0Au)) << 8) | (bytes_lsb_to_nibble(__vcmpeq4(q.w, 0x0A0A0A0Au)) << 12);
+            m = newline_mask16(load_unit_guarded(base, n, ub));
             if (first && lane == 0) m &= 0xFFFFu << off;
         }
         const unsigned b = __ballot_sync(0xffffffffu, m != 0);
@@ -330,8 +369,9 @@ __device__ __forceinline__ void hist_add(const HistTarget &t, uint64_t value) {
         atomicAdd(t.global + b, t.delta);
 }
 
-// first invalid byte in [from, to) (tile-relative), -1 if all valid.  Warp-wide.
-__device__ __forceinline__ int find_invalid(const uint32_t *s_flags, int from, int to, int lane) {
+// first invalid byte in [from, to) (relative to unit 0), -1 if all valid; s_bad[u] = the invalid-byte mask encode_unit
+// gave unit u.  Warp-wide.
+__device__ __forceinline__ int find_invalid(const uint32_t *s_bad, int from, int to, int lane) {
     if (to <= from) return -1;
     int unit0 = from >> 4;
     const int last_unit = (to + 15) >> 4;
@@ -339,7 +379,7 @@ __device__ __forceinline__ int find_invalid(const uint32_t *s_flags, int from, i
         const int u = unit0 + lane;
         uint32_t bad = 0;
         if (u < last_unit) {
-            bad = (~(s_flags[u] >> 16)) & 0xFFFFu;
+            bad = s_bad[u];
             if (u == (from >> 4)) bad &= 0xFFFFu << (from & 15);
             if (u == ((to - 1) >> 4)) bad &= 0xFFFFu >> (15 - ((to - 1) & 15));
         }

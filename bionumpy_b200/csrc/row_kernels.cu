@@ -43,10 +43,11 @@ struct RowArgs {
 };
 
 template <int RM, int ENC, bool SMEM_HIST>
-__device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_flags, const uint8_t *s_lut,
+__device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_bad, const uint8_t *s_lut,
                          const HistTarget &ht, int64_t start, int64_t L, int64_t r, int64_t out_off, int lane,
                          uint64_t &acc_values, uint64_t *acc_claims = nullptr) {
     constexpr bool MINZ = (RM == RM_MINIMIZER || RM == RM_COUNT_MIN);
+    constexpr bool LUT_ENCODE = RM == RM_ENCODE && ENC == BNPK_ENC_LUT;   // writes the table values, finds its own bad bytes
     const int span = MINZ ? a.window : (RM == RM_ENCODE ? 1 : a.k);
     const uint64_t kmask = (1ull << (2 * a.k)) - 1;
     int64_t seg_start = 0;
@@ -57,17 +58,18 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_flags,
         const int64_t ua = g0 - off;
         const int seg_len = (int)min(L - seg_start, (int64_t)(kSegBytes - off));
         const int n_units = (off + seg_len + 15) >> 4;
-        for (int u = lane; u < n_units; u += 32) {
-            const uint4 q = load_unit_guarded(a.base, a.base_bytes, ua + 16 * (int64_t)u);
-            uint32_t c, f;
-            encode_unit<ENC>(q, s_lut, c, f);
-            w_codes[u] = c;
-            w_flags[u] = f;
+        if constexpr (!LUT_ENCODE) {
+            for (int u = lane; u < n_units; u += 32) {
+                const uint4 q = load_unit_guarded(a.base, a.base_bytes, ua + 16 * (int64_t)u);
+                uint32_t bad;
+                w_codes[u] = encode_unit<ENC, false>(q, 0xFFFFu, s_lut, bad);
+                w_bad[u] = bad;
+            }
+            if (lane < 4) w_codes[n_units + lane] = 0;
         }
-        if (lane < 4) w_codes[n_units + lane] = 0;
         __syncwarp();
-        if (!reported && !(RM == RM_ENCODE && ENC == BNPK_ENC_LUT)) {
-            const int bad = find_invalid(w_flags, off, off + seg_len, lane);
+        if (!reported && !LUT_ENCODE) {
+            const int bad = find_invalid(w_bad, off, off + seg_len, lane);
             if (bad >= 0) {
                 reported = true;
                 if (lane == 0)
@@ -153,14 +155,16 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_flags,
     }
 }
 
-// Table mode asks for 4 CTAs per SM (<= 64 registers): without a minimum, ptxas keeps the row loop's 64-bit
-// accumulators on the stack in the code-byte build.  0 = no minimum, the other modes' code is unchanged by it.
+// Table mode and the long-row minimizer count ask for 4 CTAs per SM (<= 64 registers): without a minimum, ptxas keeps
+// the row loop's 64-bit accumulators on the stack (table mode: the code-byte build; long rows: every build).  0 = no
+// minimum, the other modes' code is unchanged by it.
 template <int RM, int ENC, bool SMEM_HIST, bool DEFERRED>
-__global__ void __launch_bounds__(kRowThreads, RM == RM_TABLE ? 4 : 0) rows_kernel(const RowArgs a) {
+__global__ void __launch_bounds__(kRowThreads, (RM == RM_TABLE || (RM == RM_COUNT_MIN && DEFERRED)) ? 4 : 0)
+rows_kernel(const RowArgs a) {
     extern __shared__ __align__(16) uint32_t smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint32_t *w_codes = smem + warp * kWarpWords;
-    uint32_t *w_flags = w_codes + kSegUnits + 4;
+    uint32_t *w_bad = w_codes + kSegUnits + 4;
     uint8_t *s_lut = reinterpret_cast<uint8_t *>(smem + kRowWarps * kWarpWords);
     uint32_t *s_hist = reinterpret_cast<uint32_t *>(s_lut + 256);
     if (ENC == BNPK_ENC_LUT && tid < 256) s_lut[tid] = a.lut[tid];
@@ -203,7 +207,7 @@ __global__ void __launch_bounds__(kRowThreads, RM == RM_TABLE ? 4 : 0) rows_kern
         }
         if (L <= 0) continue;
         if (lane == 0) acc_bases += (uint64_t)L;
-        warp_row<RM, ENC, SMEM_HIST>(a, w_codes, w_flags, s_lut, ht, start, L, r, out_off, lane, acc_values, &acc_claims);
+        warp_row<RM, ENC, SMEM_HIST>(a, w_codes, w_bad, s_lut, ht, start, L, r, out_off, lane, acc_values, &acc_claims);
     }
     if (COUNTING && SMEM_HIST) {
         __syncthreads();
@@ -254,7 +258,7 @@ __global__ void uncount_kernel(const RowArgs a) {
     if (L < 0) return;
     if (a.status[BNPK_ST_CR] != 0 && L > 0 && a.base[start + L - 1] == '\r') L -= 1;
     uint32_t *w_codes = smem;
-    uint32_t *w_flags = w_codes + kSegUnits + 4;
+    uint32_t *w_bad = w_codes + kSegUnits + 4;
     uint8_t *s_lut = reinterpret_cast<uint8_t *>(smem + kWarpWords);
     if (ENC == BNPK_ENC_LUT)
         for (int i = lane; i < 256; i += 32) s_lut[i] = a.lut[i];
@@ -273,7 +277,7 @@ __global__ void uncount_kernel(const RowArgs a) {
     if (lane < BNPK_ST_WORDS) scratch_status[lane] = INT64_MAX;
     __syncwarp();
     b.status = scratch_status;
-    warp_row<MINZ ? RM_COUNT_MIN : RM_COUNT, ENC, false>(b, w_codes, w_flags, s_lut, ht, start, L, n_records, 0, lane, produced);
+    warp_row<MINZ ? RM_COUNT_MIN : RM_COUNT, ENC, false>(b, w_codes, w_bad, s_lut, ht, start, L, n_records, 0, lane, produced);
     produced = warp_sum_u64(produced);
     if (lane == 0) {
         atomicAdd((unsigned long long *)&a.status[BNPK_ST_N_VALUES], 0ull - produced);

@@ -1,7 +1,7 @@
 // tile_common.cuh -- pieces shared by the tile kernels (tile_kernels.cu: split + register-staged count;
 // tile_ws_kernel.cu: the warp-specialised counts; tile_tma_kernel.cu: the count into global tables): launch
-// arguments, exact byte tests, the 16-byte unit encoder, the rare-path helpers, the bulk-copy / mbarrier wrappers and
-// the two-level decoupled look-back over the tile newline counts.
+// arguments, the rare-path helpers, the bulk-copy / mbarrier wrappers, the newline list of a staged tile and the
+// two-level decoupled look-back over the tile newline counts.
 #pragma once
 #include "bnpk_host.h"
 
@@ -31,91 +31,7 @@ struct TileArgs {
     uint32_t *hist32;              // optional 32-bit scratch table in the workspace (large global tables), else null
 };
 
-// exact per-byte "== pattern byte" flags at bit 7 of every byte
-__device__ __forceinline__ uint32_t bytes_eq_msb(uint32_t w, uint32_t pattern) {
-    const uint32_t v = w ^ pattern;
-    return ~(((v & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | v) & 0x80808080u;
-}
-// bits 7,15,23,31 -> bits 0..3 (one IMAD.HI: the partial products land on distinct bits)
-__device__ __forceinline__ uint32_t msb_to_nibble(uint32_t z) { return __umulhi(z, 0x02040810u) & 0xFu; }
-
-// 16 flag bits (one per byte) of four words
-__device__ __forceinline__ uint32_t eq_mask16(const uint32_t *w, uint32_t pattern) {
-    const uint32_t n0 = msb_to_nibble(bytes_eq_msb(w[0], pattern)), n1 = msb_to_nibble(bytes_eq_msb(w[1], pattern));
-    const uint32_t n2 = msb_to_nibble(bytes_eq_msb(w[2], pattern)), n3 = msb_to_nibble(bytes_eq_msb(w[3], pattern));
-    return (n1 * 16u + n0) + (n3 * 16u + n2) * 256u;
-}
-__device__ __forceinline__ uint64_t eq_mask64(const uint32_t *raw, uint32_t pattern) {
-    const uint32_t lo = eq_mask16(raw, pattern) | (eq_mask16(raw + 4, pattern) << 16);
-    const uint32_t hi = eq_mask16(raw + 8, pattern) | (eq_mask16(raw + 12, pattern) << 16);
-    return ((uint64_t)hi << 32) | lo;
-}
-
-// One 16-byte unit of sequence bytes -> 32 bits of 2-bit codes; `bad` becomes non-zero iff a byte
-// selected by `seq16` is outside the alphabet (exact).
-template <int ENC>
-__device__ __forceinline__ uint32_t encode_unit_seq(const uint32_t *w, uint32_t seq16, const uint8_t *s_lut, uint32_t &bad) {
-    uint32_t codes = 0;
-    if constexpr (ENC == BNPK_ENC_ASCII_ACGT || ENC == BNPK_ENC_ASCII_ACTG) {
-        uint32_t dif[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            uint32_t x;
-            if constexpr (ENC == BNPK_ENC_ASCII_ACGT) x = ((w[j] >> 1) ^ (w[j] >> 2)) & 0x03030303u;
-            else x = (w[j] >> 1) & 0x03030303u;
-            codes |= bytes_2bit_to_byte(x) << (8 * j);
-            // re-decode the codes (PRMT as a 4-entry byte LUT) and compare with the case-folded input
-            const uint32_t y = x | (x >> 4);
-            const uint32_t sel = __byte_perm(y, 0u, 0x4420);       // nibbles = the four codes
-            const uint32_t letters = (ENC == BNPK_ENC_ASCII_ACGT) ? 0x74676361u : 0x67746361u;  // "acgt" / "actg"
-            dif[j] = __byte_perm(letters, 0u, sel) ^ (w[j] | 0x20202020u);
-        }
-        if (seq16 == 0xFFFFu) {
-            bad = dif[0] | dif[1] | dif[2] | dif[3];
-        } else {
-            bad = 0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const uint32_t nz = (((dif[j] & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | dif[j]) & 0x80808080u;  // byte != 0
-                bad |= msb_to_nibble(nz) & (seq16 >> (4 * j)) & 0xFu;
-            }
-        }
-    } else if constexpr (ENC == BNPK_ENC_CODES) {
-        bad = 0;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            codes |= bytes_2bit_to_byte(w[j] & 0x03030303u) << (8 * j);
-            const uint32_t hi = w[j] & 0xFCFCFCFCu;
-            const uint32_t nz = (((hi & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | hi) & 0x80808080u;
-            bad |= msb_to_nibble(nz) & (seq16 >> (4 * j)) & 0xFu;
-        }
-    } else {
-        bad = 0;
-#pragma unroll
-        for (int b = 0; b < 16; ++b) {
-            const uint32_t code = s_lut[(w[b >> 2] >> (8 * (b & 3))) & 0xFFu];
-            codes |= (code & 3u) << (2 * b);
-            bad |= ((code >= 4u) ? 1u : 0u) & (seq16 >> b);
-        }
-    }
-    return codes;
-}
-
-// Rare: the first byte of bytes[p0, p1) outside the alphabet, as (entry << 32 | offset from the row's first byte b0)
-// for the BAD_BASE status word (a minimum); INT64_MAX if there is none.  Called only when an encoder flagged a bad
-// byte in that range.
-template <int ENC>
-__device__ __forceinline__ long long first_bad_base(const uint8_t *bytes, int p0, int p1, int b0, int64_t entry, const uint8_t *s_lut) {
-    for (int p = p0; p < p1; ++p) {
-        const uint32_t c = bytes[p];
-        bool okb;
-        if (ENC == BNPK_ENC_CODES) okb = c < 4;
-        else if (ENC == BNPK_ENC_LUT) okb = s_lut[c] < 4;
-        else { const uint32_t uu = c | 0x20u; okb = (uu == 'a' || uu == 'c' || uu == 'g' || uu == 't'); }
-        if (!okb) return (long long)((entry << 32) | (int64_t)(p - b0));
-    }
-    return INT64_MAX;
-}
+// first bad byte of a row some encode_unit flagged -> the BAD_BASE status word
 template <int ENC>
 __device__ __forceinline__ void report_bad_base(const TileArgs &a, const uint8_t *bytes, int p0, int p1, int b0, int64_t entry,
                                                 const uint8_t *s_lut) {
@@ -166,22 +82,53 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
                  : "memory");
 }
 __device__ __forceinline__ uint4 lds128(const uint8_t *p) { return *reinterpret_cast<const uint4 *>(p); }
-// PRMT without the selector clean-up __byte_perm adds (all selectors used here are in range)
-__device__ __forceinline__ uint32_t prmt(uint32_t lo, uint32_t hi, uint32_t sel) {
-    uint32_t d;
-    asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(lo), "r"(hi), "r"(sel));
-    return d;
-}
 // one count into the CTA-private table (32-bit shared address)
 __device__ __forceinline__ void hist_inc(uint32_t addr) { asm volatile("red.shared.add.u32 [%0], 1;" ::"r"(addr) : "memory"); }
 // ptxas never predicates ATOMS (it branches around it), so a masked count adds 0 or 1 instead
 __device__ __forceinline__ void hist_add_val(uint32_t addr, uint32_t val) { asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(addr), "r"(val) : "memory"); }
-// bit 7 of every byte that equals '\n' (bit 7 of the pattern is clear, so the last term can use w itself)
-__device__ __forceinline__ uint32_t newline_msb(uint32_t w) {
-    uint32_t x;                                                     // (w ^ 0x0A..) & 0x7F.. as ONE LOP3
-    asm("lop3.b32 %0, %1, 0x0A0A0A0A, 0x7F7F7F7F, 0x28;" : "=r"(x) : "r"(w));
-    const uint32_t s = x + 0x7F7F7F7Fu;
-    return ~(s | w) & 0x80808080u;
+
+// ---- the sorted newline list of a tile (emit_positions: every tile kernel; ScanLane: the kernels that stage tiles in
+// shared-memory slots) ---------------------------------------------------------------------------------------------
+constexpr int kNlCap = 1024;                    // newline positions of one tile kept in shared memory
+constexpr uint32_t kNoCross = 0xFFFFFFFFu;      // no newline in the halo
+
+// Conflict-free read of a lane's 64 bytes (LDS.128 j fetches unit (j + lane/2) & 3) -> exact 64-bit newline mask.
+struct ScanLane {
+    uint32_t off[4], sel_lo, sel_hi;
+    __device__ __forceinline__ void init(int lane) {
+        const uint32_t rot = ((uint32_t)lane >> 1) & 3u;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) off[j] = 64u * (uint32_t)lane + 16u * (((uint32_t)j + rot) & 3u);
+        // halfword h of the byte-order mask comes from load (h - rot) & 3; PRMT byte pair of load jj in
+        // (A = m0|m1<<16, B = m2|m3<<16) is 0x10 + 0x22*jj
+        sel_lo = (0x10u + 0x22u * ((0u - rot) & 3u)) | ((0x10u + 0x22u * ((1u - rot) & 3u)) << 8);
+        sel_hi = (0x10u + 0x22u * ((2u - rot) & 3u)) | ((0x10u + 0x22u * ((3u - rot) & 3u)) << 8);
+    }
+    // p = base of the warp's 2 KiB piece
+    __device__ __forceinline__ uint64_t mask64(const uint8_t *p) const {
+        uint32_t m[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) m[j] = newline_mask16(lds128(p + off[j]));
+        const uint32_t A = m[1] * 65536u + m[0], B = m[3] * 65536u + m[2];
+        return ((uint64_t)prmt(A, B, sel_hi) << 32) | prmt(A, B, sel_lo);
+    }
+};
+
+// write the positions of the set bits of m (tile-relative base `pos`) at list[li - wb ...] when inside the window
+__device__ __forceinline__ void emit_positions(uint64_t m, uint32_t li, uint32_t pos, uint16_t *list, uint32_t wb) {
+    uint32_t lo = (uint32_t)m, hi = (uint32_t)(m >> 32);
+    while (lo) {
+        const int bit = __ffs((int)lo) - 1;
+        lo &= lo - 1;
+        if (li - wb < (uint32_t)kNlCap) list[li - wb] = (uint16_t)(pos + bit);
+        ++li;
+    }
+    while (hi) {
+        const int bit = __ffs((int)hi) - 1;
+        hi &= hi - 1;
+        if (li - wb < (uint32_t)kNlCap) list[li - wb] = (uint16_t)(pos + 32 + bit);
+        ++li;
+    }
 }
 
 // ---- two-level look-back state in the workspace ------------------------------------------------

@@ -47,7 +47,6 @@ constexpr int kCtaThreads = (kTileBytes + kHaloBytes) / 64;      // one thread p
 constexpr int kCtaWarps = kCtaThreads / 32;
 constexpr int kMainThreads = kTileBytes / 64;
 static_assert(kCtaThreads % 32 == 0 && kMainThreads % 32 == 0 && kCtaWarps <= 32, "tile geometry");
-constexpr int kNlCap = 1024;              // newline positions of one staged tile kept in shared memory
 constexpr int kNlStep = kNlCap - 8;       // window advance when a tile holds more (lines shorter than ~18 bytes)
 // shared-memory layout of the tile kernel behind the private histogram (n_bins words, count mode with SMEM_HIST only),
 // in 32-bit words
@@ -133,7 +132,9 @@ __global__ void __launch_bounds__(kCtaThreads, MODE == 0 ? 4 : 3) tile_kernel(co
         const int staged_len = staged_len_of(tile);
         nl = 0;
         if (my0 < staged_len) {
-            nl = eq_mask64(raw, 0x0A0A0A0Au);
+#pragma unroll
+            for (int u = 3; u >= 0; --u)
+                nl = (nl << 16) | newline_mask16(make_uint4(raw[4 * u], raw[4 * u + 1], raw[4 * u + 2], raw[4 * u + 3]));
             if (my0 + 64 > staged_len) nl &= (~0ull) >> (64 - (staged_len - my0));
         }
         const uint32_t cnt = (uint32_t)__popcll(nl);
@@ -208,16 +209,7 @@ __global__ void __launch_bounds__(kCtaThreads, MODE == 0 ? 4 : 3) tile_kernel(co
             // ---- 2. sorted list of the newline positions of this staged tile (window `round`) -------------
             if (round > 0) __syncthreads();
             const int win_lo = round * kNlStep;
-            {
-                uint64_t m = nlM;
-                int li = (int)exM - win_lo;
-                while (m) {
-                    const int bit = __ffsll((long long)m) - 1;
-                    m &= m - 1;
-                    if (li >= 0 && li < kNlCap) s_nlpos[li] = (uint16_t)(my0 + bit);
-                    ++li;
-                }
-            }
+            emit_positions(nlM, exM, (uint32_t)my0, s_nlpos, (uint32_t)win_lo);
             __syncthreads();                                         // S1: prefix, ticket, list (and the previous k-mer stage) done
             if (round == 0) {
                 line_base = s_line_base;
@@ -333,11 +325,10 @@ __global__ void __launch_bounds__(kCtaThreads, MODE == 0 ? 4 : 3) tile_kernel(co
                         const int u1 = (e - 1) >> 4;
                         for (int u = (b0 >> 4) + sub; u <= u1; u += nsub) {
                             const uint4 q = load_unit_guarded(a.chunk, a.n, (int64_t)byte0 + 16 * (int64_t)u);
-                            const uint32_t w[4] = {q.x, q.y, q.z, q.w};
                             const int lo = max(b0 - 16 * u, 0), hi = min(e - 16 * u, 16);
                             const uint32_t seq16 = (0xFFFFu >> (16 - hi)) & (0xFFFFu << lo);
                             uint32_t bad;
-                            s_codes[u] = encode_unit_seq<ENC>(w, seq16, s_lut, bad);
+                            s_codes[u] = encode_unit<ENC, false>(q, seq16, s_lut, bad);
                             if (bad) report_bad_base<ENC>(a, a.chunk + byte0, 16 * u + lo, 16 * u + hi, b0, r_first + slot, s_lut);
                         }
                     }

@@ -34,9 +34,7 @@ constexpr int kHalo = 512;
 constexpr int kSlot = kTileBytes + kHalo;
 constexpr int kSlots = 3;
 constexpr int kRowMax = 1024;                   // longer rows go to the deferred (one warp per segment) pass
-constexpr int kNlCap = 1024;                    // newline positions of one tile kept in shared memory
 constexpr int kNlStep = kNlCap - 8;
-constexpr uint32_t kNoCross = 0xFFFFFFFFu;
 static_assert(kGT == 256 && kGW == 8, "group geometry");
 
 // per-group control block (32-bit words)
@@ -54,59 +52,6 @@ constexpr int kOffLut = kOffBar + ((kGroups * kSlots * 8 + 15) & ~15);
 constexpr int kFixedBytes = kOffLut + 256;
 
 __device__ __forceinline__ void group_bar(int g) { asm volatile("bar.sync %0, %1;" ::"r"(g + 1), "n"(kGT) : "memory"); }
-
-// tools/micro/pipe_bench.cu measures the integer pipes: LOP3/SHF/PRMT/IADD3 (ALU pipe) and IMAD (FMA pipe) each issue one
-// warp instruction every two cycles per SM sub-partition, a 50:50 mix reaches 0.65/clk and IMAD.HI only 0.23/clk.
-// This path is all integer work, so instruction count -- not bytes -- is what the kernel time follows.
-
-// exact '\n' flags of a 16-byte unit, bit i = byte i.  Per word: the zero-byte test, one IMAD that lines the four
-// flags up in the top nibble of the product and one funnel shift that pushes them into the accumulator.  (The
-// warp-specialised kernel weighs the flags with IDP.4A instead; that variant has not been timed in this kernel.)
-__device__ __forceinline__ uint32_t newline_mask16_imad(const uint4 q) {
-    const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-    uint32_t acc = 0;
-#pragma unroll
-    for (int j = 3; j >= 0; --j) acc = __funnelshift_l(newline_msb(w[j]) * 0x00204081u, acc, 4);
-    return acc & 0xFFFFu;
-}
-
-// 16-byte unit -> 32 bits of 2-bit codes (+ exact validation of the bytes selected by seq16).  Same result
-// as encode_unit_seq; the ASCII alphabets gather the four packed bytes with byte permutes and gather the validation
-// flags with IMAD + funnel shift.  (The warp-specialised kernel's encoder packs Gray codes and weighs the flags with
-// IDP.4A; that variant has not been timed in this kernel.)
-template <int ENC>
-__device__ __forceinline__ uint32_t encode_unit_imad(const uint4 q, uint32_t seq16, const uint8_t *s_lut, uint32_t &bad) {
-    const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-    if constexpr (ENC == BNPK_ENC_ASCII_ACGT || ENC == BNPK_ENC_ASCII_ACTG) {
-        uint32_t dif[4], pk[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            uint32_t x;
-            if constexpr (ENC == BNPK_ENC_ASCII_ACGT) x = ((w[j] >> 1) ^ (w[j] >> 2)) & 0x03030303u;
-            else x = (w[j] >> 1) & 0x03030303u;
-            pk[j] = x * 0x01041040u;                               // top byte = the four codes, packed
-            const uint32_t y = x | (x >> 4);
-            const uint32_t sel = prmt(y, 0u, 0x4420);              // nibbles = the four codes
-            const uint32_t letters = (ENC == BNPK_ENC_ASCII_ACGT) ? 0x74676361u : 0x67746361u;  // "acgt" / "actg"
-            dif[j] = prmt(letters, 0u, sel) ^ (w[j] | 0x20202020u);
-        }
-        const uint32_t codes = prmt(prmt(pk[0], pk[1], 0x0073), prmt(pk[2], pk[3], 0x0073), 0x5410);
-        if (seq16 == 0xFFFFu) {
-            bad = dif[0] | dif[1] | dif[2] | dif[3];
-        } else {
-            uint32_t acc = 0;                                       // bit i = byte i of the unit differs (as in newline_mask16_imad)
-#pragma unroll
-            for (int j = 3; j >= 0; --j) {
-                const uint32_t nz = (((dif[j] & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | dif[j]) & 0x80808080u;  // byte != 0
-                acc = __funnelshift_l(nz * 0x00204081u, acc, 4);
-            }
-            bad = acc & seq16;
-        }
-        return codes;
-    } else {
-        return encode_unit_seq<ENC>(w, seq16, s_lut, bad);
-    }
-}
 
 // HIST: 0 = global int64 table, 2 = global u32 scratch table (the numbering of the other fused-count kernels)
 template <int ENC, int HIST>
@@ -141,18 +86,8 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
     const uint32_t want = (fl - 1u) & pm;
     const int32_t tile_end = (int32_t)a.tile_end;
 
-    // thread constants of the conflict-free front-end read: load j fetches unit (j + rot) & 3 of my 64 bytes
-    const uint32_t rot = ((uint32_t)lane >> 1) & 3u;
-    uint32_t f_off[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) f_off[j] = 64u * (uint32_t)gt + 16u * (((uint32_t)j + rot) & 3u);
-    // halfword h of the byte-order mask comes from load (h - rot) & 3
-    uint32_t sel_lo = 0, sel_hi = 0;
-    {
-        // PRMT byte pair of load jj in (A = m0|m1<<16, B = m2|m3<<16) is 0x10 + 0x22*jj
-        sel_lo = (0x10u + 0x22u * ((0u - rot) & 3u)) | ((0x10u + 0x22u * ((1u - rot) & 3u)) << 8);
-        sel_hi = (0x10u + 0x22u * ((2u - rot) & 3u)) | ((0x10u + 0x22u * ((3u - rot) & 3u)) << 8);
-    }
+    ScanLane sl;                                                    // front end: my 64 bytes of the warp's 2 KiB
+    sl.init(lane);
     const uint32_t sub = (uint32_t)lane & 3u;
     const int src1 = (lane & ~3) | (int)((sub + 1u) & 3u), src2 = (lane & ~3) | (int)((sub + 2u) & 3u),
               src3 = (lane & ~3) | (int)((sub + 3u) & 3u);
@@ -185,13 +120,7 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
             if (gt < (staged & 15)) g_slots[slot * kSlot + t0 + gt] = a.chunk[(size_t)tile * kTileBytes + t0 + gt];
             group_bar(g);
         }
-        uint32_t m[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            m[j] = newline_mask16_imad(lds128(sp + f_off[j]));
-        }
-        const uint32_t A = m[1] * 65536u + m[0], B = m[3] * 65536u + m[2];
-        nl = ((uint64_t)prmt(A, B, sel_hi) << 32) | prmt(A, B, sel_lo);
+        nl = sl.mask64(sp + 2048 * gw);
         const int lim = min(staged, kTileBytes) - 64 * gt;          // my bytes inside the tile proper
         if (lim < 64) nl = lim <= 0 ? 0ull : (nl & (~0ull >> (64 - lim)));
         const uint32_t cnt = (uint32_t)__popcll(nl);
@@ -205,7 +134,7 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
         if (lane == 31) g_ctl[kCtlWsum + 8 * slot + gw] = inc;
         if (gw == 0) {                                              // first newline of the halo: end of the crossing row
             const int valid = min(max(staged - kTileBytes - 16 * lane, 0), 16);
-            const uint32_t mm = newline_mask16_imad(lds128(sp + kTileBytes + 16 * lane)) & ((1u << valid) - 1u);
+            const uint32_t mm = newline_mask16(lds128(sp + kTileBytes + 16 * lane)) & ((1u << valid) - 1u);
             const unsigned b = __ballot_sync(0xffffffffu, mm != 0);
             const int srcl = b ? __ffs(b) - 1 : 0;
             const uint32_t pos = (uint32_t)(kTileBytes + 16 * lane + __ffs(mm) - 1);
@@ -260,16 +189,7 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
             my_excl = exM + __reduce_add_sync(0xffffffffu, lane < gw ? v : 0u);
         }
         uint16_t *list = g_list + mb * kNlCap;
-        {
-            uint64_t m = nlM;
-            uint32_t li = my_excl;
-            while (m) {
-                const int bit = __ffsll((long long)m) - 1;
-                m &= m - 1;
-                if (li < (uint32_t)kNlCap) list[li] = (uint16_t)(64 * gt + bit);
-                ++li;
-            }
-        }
+        emit_positions(nlM, my_excl, 64u * (uint32_t)gt, list, 0u);
         if (gt == 0) g_ctl[kCtlTk + mb] = (uint32_t)tF;
         group_bar(g);                                               // ---- the barrier ----
         // ---- c. publish P, refill the free slot, next ticket, P's look-back loads ------------------------
@@ -303,14 +223,7 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
             const int win_lo = round * kNlStep;
             if (round > 0) {                                        // rare: more than kNlCap lines in one tile
                 group_bar(g);
-                uint64_t m = nlM;
-                uint32_t li = my_excl - (uint32_t)win_lo;
-                while (m) {
-                    const int bit = __ffsll((long long)m) - 1;
-                    m &= m - 1;
-                    if (li < (uint32_t)kNlCap) list[li] = (uint16_t)(64 * gt + bit);
-                    ++li;
-                }
+                emit_positions(nlM, my_excl, 64u * (uint32_t)gt, list, (uint32_t)win_lo);
                 group_bar(g);
             }
             const int n_in_win = min((int)tile_nl - win_lo, kNlCap);
@@ -388,7 +301,7 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
                     const int lo = max(b0 - 16 * u, 0), hi = min(e - 16 * u, 16);
                     const uint32_t seq16 = (0xFFFFu >> (16 - hi)) & (0xFFFFu << lo);
                     uint32_t bad;
-                    const uint32_t codes = encode_unit_imad<ENC>(q, seq16, s_lut, bad);
+                    const uint32_t codes = encode_unit<ENC, false>(q, seq16, s_lut, bad);
                     if (bad) report_bad_base<ENC>(a, sp, 16 * u + lo, 16 * u + hi, b0, r_first + s, s_lut);
                     return codes;
                 };
