@@ -6,6 +6,7 @@
 //   K4 rows_minimizers  get_minimizers             sequence/minimizers.py:20-54
 //   K3/K4+K5 rows_kmer_count   count_kmers         sequence/kmers.py:129-145
 //   K3 + table rows_kmer_table_insert  exact distinct-k-mer counts (extension, like `jellyfish count`)
+//   K7 rows_pwm_scores / rows_pwm_max  get_motif_scores, PWM.calculate_scores  sequence/position_weight_matrix.py:83-100,166-196
 // plus the clean-up passes of the fused chunk count (long rows, trailing incomplete entry).
 #include <climits>
 #include "bnpk_host.h"
@@ -18,7 +19,11 @@ constexpr int kSegUnits = 128;               // 2 KiB staged per warp and segmen
 constexpr int kSegBytes = kSegUnits * 16;
 constexpr int kWarpWords = 2 * kSegUnits + 4;
 
-enum { RM_ENCODE = 0, RM_HASH = 1, RM_MINIMIZER = 2, RM_COUNT = 3, RM_COUNT_MIN = 4, RM_TABLE = 5 };
+enum { RM_ENCODE = 0, RM_HASH = 1, RM_MINIMIZER = 2, RM_COUNT = 3, RM_COUNT_MIN = 4, RM_TABLE = 5, RM_PWM = 6,
+       RM_PWM_MAX = 7 };
+constexpr int kPwmMaxLen = kSegBytes / 2;     // motif columns: the segment overlap limit of check_common
+constexpr int kPwmMaxCells = 8192;            // alphabet_size * motif_len doubles: 64 KiB of shared memory
+constexpr int kPwmInFlight = 4;               // positions per lane summed side by side (each one a chain of DADDs)
 
 struct RowArgs {
     const uint8_t *base;
@@ -40,15 +45,67 @@ struct RowArgs {
     int lpe;
     uint64_t canon_xor;          // != 0: canonical k-mers (hash / count / table modes without a minimizer window)
     KmerTable table;             // table mode
+    // motif modes: matrix[j * 4 + c] (motif_len = window), and whether the last window - 1 positions of a row are
+    // scored with the columns that fit
+    const double *pwm;
+    int tail;
 };
+
+// NaN-propagating maximum (np.max): once a NaN is in, it stays
+__device__ __forceinline__ double nan_max(double m, double v) { return (v > m || v != v) ? v : m; }
+
+// Motif scores of the positions of one staged segment that start in [0, npos): s = +0.0, then s += table[j][code]
+// for j = 0, 1, ... in order (PWM.calculate_scores, sequence/position_weight_matrix.py:96-99), each position with the
+// columns that fit before seg_len.  Codes come 16 at a time from the packed stream.  Writes out[p] (SCORES) or folds
+// the scores into `best`.  Returns the positions this lane scored.  Warp-wide.
+template <bool SCORES>
+__device__ __forceinline__ uint32_t pwm_segment(const uint32_t *w_codes, const double *s_pwm, int off, int seg_len,
+                                                int npos, int m, double *out, double &best, int lane) {
+    uint32_t produced = 0;
+    for (int p0 = lane; p0 < npos; p0 += 32 * kPwmInFlight) {
+        double s[kPwmInFlight];
+        int nc[kPwmInFlight];
+#pragma unroll
+        for (int q = 0; q < kPwmInFlight; ++q) {
+            const int p = p0 + 32 * q;
+            nc[q] = p < npos ? min(m, seg_len - p) : 0;
+            s[q] = 0.0;
+        }
+        for (int jb = 0; jb < nc[0]; jb += 16) {
+            uint32_t w[kPwmInFlight];
+#pragma unroll
+            for (int q = 0; q < kPwmInFlight; ++q)
+                w[q] = jb < nc[q] ? stream_lo32(w_codes, (uint32_t)(off + p0 + 32 * q + jb)) : 0u;
+            const int je = min(16, nc[0] - jb);
+            for (int jj = 0; jj < je; ++jj) {
+                const double *col = s_pwm + 4 * (jb + jj);
+#pragma unroll
+                for (int q = 0; q < kPwmInFlight; ++q)
+                    if (jb + jj < nc[q]) s[q] += col[(w[q] >> (2 * jj)) & 3u];
+            }
+        }
+#pragma unroll
+        for (int q = 0; q < kPwmInFlight; ++q) {
+            const int p = p0 + 32 * q;
+            if (p < npos) {
+                if constexpr (SCORES) out[p] = s[q];
+                else best = nan_max(best, s[q]);
+                ++produced;
+            }
+        }
+    }
+    return produced;
+}
 
 template <int RM, int ENC, bool SMEM_HIST>
 __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_bad, const uint8_t *s_lut,
                          const HistTarget &ht, int64_t start, int64_t L, int64_t r, int64_t out_off, int lane,
-                         uint64_t &acc_values, uint64_t *acc_claims = nullptr) {
+                         uint64_t &acc_values, uint64_t *acc_claims = nullptr, const double *s_pwm = nullptr) {
     constexpr bool MINZ = (RM == RM_MINIMIZER || RM == RM_COUNT_MIN);
+    constexpr bool PWM = (RM == RM_PWM || RM == RM_PWM_MAX);
     constexpr bool LUT_ENCODE = RM == RM_ENCODE && ENC == BNPK_ENC_LUT;   // writes the table values, finds its own bad bytes
-    const int span = MINZ ? a.window : (RM == RM_ENCODE ? 1 : a.k);
+    const int span = (MINZ || PWM) ? a.window : (RM == RM_ENCODE ? 1 : a.k);
+    double best = -INFINITY;                                              // RM_PWM_MAX: this lane's maximum
     const uint64_t kmask = (1ull << (2 * a.k)) - 1;
     int64_t seg_start = 0;
     bool reported = false;
@@ -145,6 +202,11 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_bad, c
                     ++acc_values;
                 }
             }
+        } else if constexpr (PWM) {
+            // with `tail`, the row's last segment also scores its last span - 1 positions with the columns that fit
+            const int npos = (a.tail && seg_start + seg_len >= L) ? seg_len : seg_len - span + 1;
+            acc_values += pwm_segment<RM == RM_PWM>(w_codes, s_pwm, off, seg_len, npos, span,
+                                                    reinterpret_cast<double *>(a.out) + out_off + seg_start, best, lane);
         } else {
             if (seg_len >= span)
                 acc_values += row_count<SMEM_HIST, MINZ>(w_codes, off, seg_len, a.k, a.window, ht, lane);
@@ -153,21 +215,27 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_bad, c
         if (seg_start + seg_len >= L) break;
         seg_start += seg_len - (span - 1);
     }
+    if constexpr (RM == RM_PWM_MAX) {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) best = nan_max(best, __shfl_xor_sync(0xffffffffu, best, o));
+        if (lane == 0) reinterpret_cast<double *>(a.out)[r] = best;
+    }
 }
 
-// Table mode and the long-row minimizer count ask for 4 CTAs per SM (<= 64 registers): without a minimum, ptxas keeps
-// the row loop's 64-bit accumulators on the stack (table mode: the code-byte build; long rows: every build).  0 = no
-// minimum, the other modes' code is unchanged by it.
+// The body of the row kernels: one warp per row, the block's rows strided over the grid.
 template <int RM, int ENC, bool SMEM_HIST, bool DEFERRED>
-__global__ void __launch_bounds__(kRowThreads, (RM == RM_TABLE || (RM == RM_COUNT_MIN && DEFERRED)) ? 4 : 0)
-rows_kernel(const RowArgs a) {
+__device__ __forceinline__ void rows_body(const RowArgs &a) {
     extern __shared__ __align__(16) uint32_t smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint32_t *w_codes = smem + warp * kWarpWords;
     uint32_t *w_bad = w_codes + kSegUnits + 4;
     uint8_t *s_lut = reinterpret_cast<uint8_t *>(smem + kRowWarps * kWarpWords);
     uint32_t *s_hist = reinterpret_cast<uint32_t *>(s_lut + 256);
+    double *s_pwm = reinterpret_cast<double *>(s_lut + 256);              // motif modes: the [window][4] table
     if (ENC == BNPK_ENC_LUT && tid < 256) s_lut[tid] = a.lut[tid];
+    constexpr bool PWM = (RM == RM_PWM || RM == RM_PWM_MAX);
+    if constexpr (PWM)
+        for (int i = tid; i < 4 * a.window; i += kRowThreads) s_pwm[i] = a.pwm[i];
     constexpr bool COUNTING = (RM == RM_COUNT || RM == RM_COUNT_MIN);
     if (COUNTING && SMEM_HIST)
         for (uint32_t b = tid; b < a.n_bins; b += kRowThreads) s_hist[b] = 0;
@@ -205,9 +273,14 @@ rows_kernel(const RowArgs a) {
             r = (int64_t)row;
             if (a.offsets) out_off = a.offsets[row];
         }
-        if (L <= 0) continue;
+        if (L <= 0) {
+            if constexpr (RM == RM_PWM_MAX)
+                if (lane == 0) reinterpret_cast<double *>(a.out)[r] = -INFINITY;   // no window
+            continue;
+        }
         if (lane == 0) acc_bases += (uint64_t)L;
-        warp_row<RM, ENC, SMEM_HIST>(a, w_codes, w_bad, s_lut, ht, start, L, r, out_off, lane, acc_values, &acc_claims);
+        warp_row<RM, ENC, SMEM_HIST>(a, w_codes, w_bad, s_lut, ht, start, L, r, out_off, lane, acc_values, &acc_claims,
+                                     s_pwm);
     }
     if (COUNTING && SMEM_HIST) {
         __syncthreads();
@@ -228,6 +301,21 @@ rows_kernel(const RowArgs a) {
         acc_claims = warp_sum_u64(acc_claims);
         if (lane == 0 && acc_claims) atomicAdd(a.table.n_used, (unsigned long long)acc_claims);
     }
+}
+
+// Table mode and the long-row minimizer count ask for 4 CTAs per SM (<= 64 registers): without a minimum, ptxas keeps
+// the row loop's 64-bit accumulators on the stack (table mode: the code-byte build; long rows: every build).  0 = no
+// minimum, the other modes' code is unchanged by it.
+template <int RM, int ENC, bool SMEM_HIST, bool DEFERRED>
+__global__ void __launch_bounds__(kRowThreads, (RM == RM_TABLE || (RM == RM_COUNT_MIN && DEFERRED)) ? 4 : 0)
+rows_kernel(const RowArgs a) {
+    rows_body<RM, ENC, SMEM_HIST, DEFERRED>(a);
+}
+
+// The motif modes (RM_PWM, RM_PWM_MAX), with 4 CTAs per SM for the same reason (the LUT build of the scores).
+template <int RM, int ENC>
+__global__ void __launch_bounds__(kRowThreads, 4) rows_pwm_kernel(const RowArgs a) {
+    rows_body<RM, ENC, false, false>(a);
 }
 
 // Growth: one thread per slot of the old table re-inserts its (key, count) into the new one with the same slot function.
@@ -320,6 +408,65 @@ __global__ void __launch_bounds__(256) rows_generic_hash_kernel(const uint8_t *b
     }
 }
 
+// Motif scores for alphabets that are not four letters ("ACE", "ACGTN", amino acids): the same sums, tail and maximum as
+// rows_kernel's motif modes, with codes from a 256-byte LUT in shared memory (255 = invalid; byte codes: c < A maps to
+// itself) and the [m][A] table behind it.  One warp per row, one lane per position.
+template <bool SCORES>
+__global__ void __launch_bounds__(256) rows_pwm_generic_kernel(const uint8_t *base, const int64_t *starts, const int32_t *lens,
+                                                               size_t n_rows, const uint8_t *lut, int alphabet_size,
+                                                               const double *matrix, int m, int tail, const int64_t *offsets,
+                                                               double *out, int64_t *status) {
+    extern __shared__ __align__(16) uint32_t smem[];
+    double *s_tab = reinterpret_cast<double *>(smem);
+    uint8_t *s_lut = reinterpret_cast<uint8_t *>(s_tab + alphabet_size * m);
+    const int tid = threadIdx.x, lane = tid & 31;
+    s_lut[tid] = lut ? lut[tid] : (tid < alphabet_size ? (uint8_t)tid : (uint8_t)255);
+    for (int i = tid; i < alphabet_size * m; i += 256) s_tab[i] = matrix[i];
+    __syncthreads();
+    uint64_t acc_values = 0, acc_bases = 0;
+    const size_t warp_global = ((size_t)blockIdx.x * blockDim.x + tid) >> 5;
+    const size_t n_warps = ((size_t)gridDim.x * blockDim.x) >> 5;
+    for (size_t r = warp_global; r < n_rows; r += n_warps) {
+        const uint8_t *row = base + starts[r];
+        const int64_t L = lens[r];
+        double best = -INFINITY;
+        if (L > 0) {
+            if (lane == 0) acc_bases += (uint64_t)L;
+            int64_t first_bad = INT64_MAX;                  // every byte is validated, as the reference encodes it all
+            for (int64_t i = lane; i < L; i += 32)
+                if (s_lut[row[i]] >= alphabet_size) { first_bad = i; break; }
+#pragma unroll
+            for (int o = 16; o; o >>= 1) first_bad = min(first_bad, __shfl_xor_sync(0xffffffffu, first_bad, o));
+            if (lane == 0 && first_bad != INT64_MAX)
+                atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)(((int64_t)r << 32) | first_bad));
+            const int64_t npos = tail ? L : L - m + 1;
+            double *o_row = SCORES ? out + offsets[r] : nullptr;
+            for (int64_t i = lane; i < npos; i += 32) {
+                const int nc = (int)min((int64_t)m, L - i);
+                double s = 0.0;
+                for (int j = 0; j < nc; ++j) {
+                    const uint32_t c = s_lut[row[i + j]];
+                    s += s_tab[j * alphabet_size + (c < (uint32_t)alphabet_size ? c : 0u)];
+                }
+                if constexpr (SCORES) o_row[i] = s;
+                else best = nan_max(best, s);
+                ++acc_values;
+            }
+        }
+        if constexpr (!SCORES) {
+#pragma unroll
+            for (int o = 16; o; o >>= 1) best = nan_max(best, __shfl_xor_sync(0xffffffffu, best, o));
+            if (lane == 0) out[r] = best;
+        }
+    }
+    acc_values = warp_sum_u64(acc_values);
+    acc_bases = warp_sum_u64(acc_bases);
+    if (lane == 0) {
+        if (acc_values) atomicAdd((unsigned long long *)&status[BNPK_ST_N_VALUES], acc_values);
+        if (acc_bases) atomicAdd((unsigned long long *)&status[BNPK_ST_N_BASES], acc_bases);
+    }
+}
+
 // get_reverse_complement (sequence/dna.py:36-65): out row r = lut[row r read backwards]; one warp per row,
 // coalesced writes.  The 256-byte lut is the reference's complement Lookup for the array's encoding.
 __global__ void __launch_bounds__(256) rows_reverse_complement_kernel(const uint8_t *base, const int64_t *starts, const int32_t *lens,
@@ -345,9 +492,12 @@ static size_t rows_smem_bytes(bool counting, bool smem_hist, uint64_t n_bins) {
 
 template <int RM, int ENC, bool SMEM_HIST, bool DEFERRED>
 static int launch_rows_t(const RowArgs &a, size_t est_rows, cudaStream_t st) {
-    auto kern = rows_kernel<RM, ENC, SMEM_HIST, DEFERRED>;
+    void (*kern)(const RowArgs);
+    if constexpr (RM == RM_PWM || RM == RM_PWM_MAX) kern = rows_pwm_kernel<RM, ENC>;
+    else kern = rows_kernel<RM, ENC, SMEM_HIST, DEFERRED>;
     constexpr bool COUNTING = (RM == RM_COUNT || RM == RM_COUNT_MIN);
-    const size_t smem = rows_smem_bytes(COUNTING, SMEM_HIST, a.n_bins);
+    size_t smem = rows_smem_bytes(COUNTING, SMEM_HIST, a.n_bins);
+    if constexpr (RM == RM_PWM || RM == RM_PWM_MAX) smem += (size_t)4 * a.window * sizeof(double);
     BNPK_DYN_SMEM(kern, 200 * 1024);
     int per_sm = 1;
     BNPK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kRowThreads, smem));
@@ -356,7 +506,7 @@ static int launch_rows_t(const RowArgs &a, size_t est_rows, cudaStream_t st) {
     const size_t cap = (size_t)sm_count() * per_sm;
     const unsigned grid = (unsigned)std::max<size_t>(1, std::min(want, cap));
     kern<<<grid, kRowThreads, smem, st>>>(a);
-    BNPK_LAUNCHED("rows_kernel");
+    BNPK_LAUNCHED((RM == RM_PWM || RM == RM_PWM_MAX) ? "rows_pwm_kernel" : "rows_kernel");
     return 0;
 }
 
@@ -406,6 +556,41 @@ int count_fixups_impl(const uint8_t *chunk, size_t n, int lpe, int enc_mode, con
                     : launch_rows_enc<RM_COUNT, false, true>(a, enc_mode, est, st);
     if (rc) return rc;
     return window ? launch_uncount<true>(a, enc_mode, st) : launch_uncount<false>(a, enc_mode, st);
+}
+
+static int check_pwm(int enc_mode, const uint8_t *lut256, int alphabet_size, const double *matrix, int motif_len) {
+    if (motif_len < 1 || motif_len > kPwmMaxLen) return set_err(BNPK_E_BADARG, "motif_len must be in 1..1024");
+    if (alphabet_size < 2 || alphabet_size > 255) return set_err(BNPK_E_BADARG, "alphabet_size must be in 2..255");
+    if (alphabet_size * motif_len > kPwmMaxCells) return set_err(BNPK_E_BADARG, "alphabet_size * motif_len above 8192");
+    if (enc_mode < 0 || enc_mode > 3) return set_err(BNPK_E_BADARG, "bad enc_mode");
+    if (alphabet_size != 4 && enc_mode != BNPK_ENC_LUT && enc_mode != BNPK_ENC_CODES)
+        return set_err(BNPK_E_BADARG, "alphabets that are not four letters take BNPK_ENC_LUT or BNPK_ENC_CODES");
+    if (enc_mode == BNPK_ENC_LUT && !lut256) return set_err(BNPK_E_BADARG, "lut256 required");
+    if (!matrix) return set_err(BNPK_E_BADARG, "matrix required");
+    return 0;
+}
+
+// Four-letter alphabets take rows_kernel's motif modes (2-bit codes, every enc_mode); the others the byte-LUT kernel.
+template <bool SCORES>
+static int launch_pwm(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
+                      int enc_mode, const uint8_t *lut256, int alphabet_size, const double *matrix, int motif_len,
+                      int tail, const int64_t *offsets, double *out, int64_t *status, cudaStream_t st) {
+    if (alphabet_size == 4) {
+        RowArgs a{};
+        a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
+        a.k = 1; a.window = motif_len; a.offsets = offsets; a.out = out; a.n_bins = 1; a.status = status;
+        a.pwm = matrix; a.tail = tail;
+        return launch_rows_enc<SCORES ? RM_PWM : RM_PWM_MAX, false, false>(a, enc_mode, n_rows, st);
+    }
+    auto kern = rows_pwm_generic_kernel<SCORES>;
+    const size_t smem = (size_t)alphabet_size * motif_len * sizeof(double) + 256;
+    BNPK_DYN_SMEM(kern, kPwmMaxCells * sizeof(double) + 256);
+    const size_t want = (n_rows + 7) / 8;
+    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 8));
+    kern<<<grid, 256, smem, st>>>(base, starts, lens, n_rows, enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size,
+                                  matrix, motif_len, tail, offsets, out, status);
+    BNPK_LAUNCHED("rows_pwm_generic_kernel");
+    return 0;
 }
 
 }  // namespace bnpk
@@ -557,6 +742,26 @@ int bnpk_rows_reverse_complement(const uint8_t *base, size_t base_bytes, const i
     rows_reverse_complement_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(base, starts, lens, n_rows, lut256, offsets, out);
     BNPK_LAUNCHED("rows_reverse_complement_kernel");
     return 0;
+}
+
+int bnpk_rows_pwm_scores(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                         size_t n_rows, int enc_mode, const uint8_t *lut256, int alphabet_size,
+                         const double *matrix, int motif_len, int tail,
+                         const int64_t *offsets, double *scores_out, int64_t *status, void *stream) {
+    if (int rc = check_pwm(enc_mode, lut256, alphabet_size, matrix, motif_len)) return rc;
+    if (tail != 0 && tail != 1) return set_err(BNPK_E_BADARG, "tail must be 0 or 1");
+    if (n_rows == 0) return 0;
+    return launch_pwm<true>(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, alphabet_size, matrix, motif_len,
+                            tail, offsets, scores_out, status, (cudaStream_t)stream);
+}
+
+int bnpk_rows_pwm_max(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                      size_t n_rows, int enc_mode, const uint8_t *lut256, int alphabet_size,
+                      const double *matrix, int motif_len, double *max_out, int64_t *status, void *stream) {
+    if (int rc = check_pwm(enc_mode, lut256, alphabet_size, matrix, motif_len)) return rc;
+    if (n_rows == 0) return 0;
+    return launch_pwm<false>(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, alphabet_size, matrix, motif_len,
+                             0, nullptr, max_out, status, (cudaStream_t)stream);
 }
 
 }  // extern "C"

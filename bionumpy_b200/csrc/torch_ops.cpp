@@ -190,6 +190,25 @@ Tensor rows_reverse_complement(const Tensor &base, const Tensor &starts, const T
     return out;
 }
 
+// K7: motif scores float64[total] of matrix [motif_len, alphabet_size] (float64, on the device)
+std::tuple<Tensor, Tensor> rows_pwm_scores(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t enc_mode,
+                                           const c10::optional<Tensor> &lut, const Tensor &matrix, bool tail,
+                                           const Tensor &offsets, int64_t total) {
+    need_rows(base, starts, lens);
+    need(matrix, torch::kFloat64, "matrix");
+    TORCH_CHECK(matrix.dim() == 2, "bnpk: matrix must be [motif_len, alphabet_size]");
+    c10::cuda::CUDAGuard guard(base.device());
+    Tensor out = torch::empty({total}, base.options().dtype(torch::kFloat64));
+    Tensor status = new_status(base);
+    check(bnpk_rows_pwm_scores(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
+                               lens.data_ptr<int32_t>(), (size_t)lens.numel(), (int)enc_mode, lut ? u8(*lut) : nullptr,
+                               (int)matrix.size(1), matrix.data_ptr<double>(), (int)matrix.size(0), tail,
+                               offsets.data_ptr<int64_t>(), out.data_ptr<double>(), status.data_ptr<int64_t>(),
+                               cur_stream(base)),
+          "rows_pwm_scores");
+    return {out, status};
+}
+
 // K5 (accumulates into hist)
 Tensor bincount(const Tensor &values, Tensor hist, int64_t hist_mode) {
     need(values, torch::kInt64, "values");
@@ -220,6 +239,8 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("rows_kmer_table_insert(Tensor base, Tensor starts, Tensor lens, int enc_mode, Tensor? lut, int k, "
           "int complement_xor, Tensor(a!) keys, Tensor(b!) counts, Tensor(c!) n_used) -> Tensor");
     m.def("rows_reverse_complement(Tensor base, Tensor starts, Tensor lens, Tensor lut, Tensor offsets, int total) -> Tensor");
+    m.def("rows_pwm_scores(Tensor base, Tensor starts, Tensor lens, int enc_mode, Tensor? lut, Tensor matrix, bool tail, "
+          "Tensor offsets, int total) -> (Tensor, Tensor)");
     m.def("bincount(Tensor values, Tensor(a!) hist, int hist_mode=0) -> Tensor");
 }
 
@@ -232,5 +253,6 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("rows_kmer_count", &rows_kmer_count);
     m.impl("rows_kmer_table_insert", &rows_kmer_table_insert);
     m.impl("rows_reverse_complement", &rows_reverse_complement);
+    m.impl("rows_pwm_scores", &rows_pwm_scores);
     m.impl("bincount", &bincount);
 }

@@ -5,3 +5,4 @@ from .files import bnp_open
 from .parser import CudaFileReader, NpDataclassReader
 from .multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
 from .indexed_fasta import IndexedFasta, read_index, create_index
+from .motifs import read_motif

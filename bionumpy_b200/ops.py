@@ -284,6 +284,45 @@ def kmer_table_rehash(keys, counts, new_keys, new_counts, n_used, status=None):
     return status
 
 
+def _pwm_args(matrix, alphabet_size, lut):
+    _need_cuda(matrix, "matrix")
+    if matrix.dtype != torch.float64 or matrix.dim() != 2 or matrix.shape[1] != alphabet_size:
+        raise TypeError("matrix must be float64 of shape [motif_len, alphabet_size]")
+    if lut is not None:
+        _need_cuda(lut, "lut")
+    return ptr(lut), alphabet_size, ptr(matrix), matrix.shape[0]
+
+
+@_on_device
+def rows_pwm_scores(base, starts, lens, enc_mode, matrix, lut=None, tail=False, offsets=None, status=None, total=None):
+    """K7: motif scores of every window of the rows (every position with ``tail``), float64, in column order.
+    ``matrix`` is [motif_len, alphabet_size] on the device.  Returns (scores, offsets, status)."""
+    alphabet_size = matrix.shape[-1] if matrix.dim() == 2 else 0
+    if offsets is None:
+        offsets = row_offsets(lens, 0 if tail else max(matrix.shape[0] - 1, 0))
+    if total is None:
+        total = int(offsets[-1].item())
+    out = torch.empty(total, dtype=torch.float64, device=base.device)
+    if status is None:
+        status = nv.new_status(base.device)
+    check(lib().bnpk_rows_pwm_scores(*_rows_args(base, starts, lens), enc_mode, *_pwm_args(matrix, alphabet_size, lut),
+                                     int(tail), ptr(offsets), ptr(out), ptr(status), stream_ptr()))
+    return out, offsets, status
+
+
+@_on_device
+def rows_pwm_max(base, starts, lens, enc_mode, matrix, lut=None, status=None):
+    """K7 fused with the row maximum: float64[R], NaN-propagating, -inf for a row without a window; the scores are
+    never written.  Returns (max, status)."""
+    alphabet_size = matrix.shape[-1] if matrix.dim() == 2 else 0
+    out = torch.empty(lens.numel(), dtype=torch.float64, device=base.device)
+    if status is None:
+        status = nv.new_status(base.device)
+    check(lib().bnpk_rows_pwm_max(*_rows_args(base, starts, lens), enc_mode, *_pwm_args(matrix, alphabet_size, lut),
+                                  ptr(out), ptr(status), stream_ptr()))
+    return out, status
+
+
 @_on_device
 def bincount(values, n_bins, hist=None, hist_mode=nv.HIST_AUTO, status=None):
     _need_cuda(values, "values")

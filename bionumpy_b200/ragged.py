@@ -16,6 +16,19 @@ def _as_index_tensor(x, device, dtype=torch.int64):
     return torch.as_tensor(np.asarray(x), dtype=dtype, device=device)
 
 
+def segment_max(values, rows, n_rows):
+    """out[r] = max of values[i] with rows[i] == r, NaN if one of them is NaN; the dtype's lowest value (-inf for
+    floats) where there is none."""
+    low = -float("inf") if values.is_floating_point() else torch.iinfo(values.dtype).min
+    out = torch.full((n_rows,), low, dtype=values.dtype, device=values.device)
+    out.scatter_reduce_(0, rows, values, "amax", include_self=True)
+    if values.is_floating_point():
+        nan = torch.zeros(n_rows, dtype=torch.int32, device=values.device)
+        nan.index_add_(0, rows, torch.isnan(values).to(torch.int32))
+        out = torch.where(nan > 0, torch.full_like(out, float("nan")), out)
+    return out
+
+
 class RaggedShape:
     """(starts, lens) of the rows.  Compared by lengths only, like npstructures.RaggedShape."""
 
@@ -201,7 +214,30 @@ class RaggedArray:
     def __ne__(self, other):
         return self._compare(other, torch.ne)
 
+    def __lt__(self, other):
+        return self._compare(other, torch.lt)
+
+    def __le__(self, other):
+        return self._compare(other, torch.le)
+
+    def __gt__(self, other):
+        return self._compare(other, torch.gt)
+
+    def __ge__(self, other):
+        return self._compare(other, torch.ge)
+
     __hash__ = None
+
+    def max(self, axis=None, **kwargs):
+        """np.max: a NaN makes the maximum NaN.  axis=-1: one value per row; an empty row gives the dtype's lowest
+        value (-inf for floats)."""
+        flat = self.ravel()
+        if axis is None:
+            return flat.max()
+        if axis in (-1, 1):
+            rows = torch.repeat_interleave(torch.arange(len(self), device=flat.device), self._lens.to(torch.int64))
+            return segment_max(flat, rows, len(self))
+        raise NotImplementedError(axis)
 
     def sum(self, axis=None, **kwargs):
         if axis is None:

@@ -5,3 +5,4 @@ from .count_encoded import count_encoded, count_hashed, EncodedCounts
 from .dna import complement, get_reverse_complement
 from .indexing import KmerIndex, KmerLookup
 from .bloom_filter import BloomFilter
+from .position_weight_matrix import get_motif_scores, PWM

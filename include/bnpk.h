@@ -233,6 +233,29 @@ int bnpk_kmer_table_rehash(const int64_t *keys, const int64_t *counts, size_t ca
                            int64_t *new_keys, int64_t *new_counts, size_t new_capacity, int64_t *n_used,
                            int64_t *status, void *stream);
 
+/* K7  motif scores of a position weight matrix: get_motif_scores / PWM.calculate_scores
+ *     (sequence/position_weight_matrix.py:83-100,166-196).  matrix[j * alphabet_size + c] (device float64) is the
+ *     score of code c at motif column j, the transpose of the reference's PWM._matrix[c, j]; motif_len = m.
+ *     out[offsets[r] + i] = ((+0.0 + matrix[0][code[r][i]]) + matrix[1][code[r][i+1]]) + ... summed in column order in
+ *     float64, which is the reference's sequence of adds, so the bits are the reference's.  tail = 0: the windows of
+ *     the row, max(L - m + 1, 0) values (offsets from shrink = m - 1; the reference's [..., :-m+1]); tail = 1: also the
+ *     last m - 1 positions with the columns that fit, L values (shrink = 0; calculate_scores on one flat row).
+ *     Text is read as by the other row entry points (enc_mode, lut256: AlphabetEncoding(pwm.alphabet)); for an
+ *     alphabet_size that is not 4 only BNPK_ENC_LUT (lut256: byte -> code, 255 = invalid) and BNPK_ENC_CODES (bytes
+ *     are codes, valid below alphabet_size) are accepted.  A byte outside the alphabet anywhere in a row, including its
+ *     last m - 1 bytes, is reported in status[BNPK_ST_BAD_BASE] (EncodingError, encodings/alphabet_encoding.py:34-46);
+ *     N_BASES += row lengths, N_VALUES += values scored.  BNPK_E_BADARG unless 1 <= motif_len <= 1024,
+ *     2 <= alphabet_size <= 255 and alphabet_size * motif_len <= 8192 (the table lives in shared memory). */
+int bnpk_rows_pwm_scores(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                         size_t n_rows, int enc_mode, const uint8_t *lut256, int alphabet_size,
+                         const double *matrix /* [m][alphabet_size] */, int motif_len, int tail,
+                         const int64_t *offsets, double *scores_out, int64_t *status, void *stream);
+/*     get_motif_scores(...).max(axis=-1) without writing the scores: max_out[r] = the largest score of row r's windows
+ *     (tail = 0), NaN if one of them is NaN (np.max), -inf for a row without a window.  Same arguments and status. */
+int bnpk_rows_pwm_max(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                      size_t n_rows, int enc_mode, const uint8_t *lut256, int alphabet_size,
+                      const double *matrix, int motif_len, double *max_out, int64_t *status, void *stream);
+
 /* K5  np.bincount(values % n_bins, minlength=n_bins) accumulated into hist
  *     (sequence/count_encoded.py:173-177; EncodedArray.__array_function__ encoded_array.py:459-460).
  *     Values must be non-negative; n_bins = len(alphabet) reproduces count_encoded exactly
