@@ -521,6 +521,16 @@ static int launch_rows_enc(const RowArgs &a, int enc_mode, size_t est_rows, cuda
     return set_err(BNPK_E_BADARG, "bad enc_mode");
 }
 
+// The kernels' view of a row entry point's rows (n_bins 1 for the modes that count nothing); the caller fills in its
+// mode's fields.
+static RowArgs row_args(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                        size_t n_rows, const uint8_t *lut256) {
+    RowArgs a{};
+    a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
+    a.n_bins = 1;
+    return a;
+}
+
 static int check_common(int enc_mode, const uint8_t *lut256, int k, int window) {
     if (k < 1 || k > 31) return set_err(BNPK_E_K, "k must be larger than 0 and smaller than 32");
     if (window != 0 && window < k) return set_err(BNPK_E_WINDOW, "kmer size must be smaller than window size");
@@ -576,9 +586,8 @@ static int launch_pwm(const uint8_t *base, size_t base_bytes, const int64_t *sta
                       int enc_mode, const uint8_t *lut256, int alphabet_size, const double *matrix, int motif_len,
                       int tail, const int64_t *offsets, double *out, int64_t *status, cudaStream_t st) {
     if (alphabet_size == 4) {
-        RowArgs a{};
-        a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
-        a.k = 1; a.window = motif_len; a.offsets = offsets; a.out = out; a.n_bins = 1; a.status = status;
+        RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
+        a.k = 1; a.window = motif_len; a.offsets = offsets; a.out = out; a.status = status;
         a.pwm = matrix; a.tail = tail;
         return launch_rows_enc<SCORES ? RM_PWM : RM_PWM_MAX, false, false>(a, enc_mode, n_rows, st);
     }
@@ -604,9 +613,8 @@ int bnpk_rows_encode(const uint8_t *base, size_t base_bytes, const int64_t *star
                      int64_t *status, void *stream) {
     if (int rc = check_common(enc_mode, lut256, 1, 0)) return rc;
     if (n_rows == 0) return 0;
-    RowArgs a{};
-    a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
-    a.k = 1; a.offsets = offsets; a.out = codes_out; a.n_bins = 1; a.status = status;
+    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
+    a.k = 1; a.offsets = offsets; a.out = codes_out; a.status = status;
     return launch_rows_enc<RM_ENCODE, false, false>(a, enc_mode, n_rows, (cudaStream_t)stream);
 }
 
@@ -615,9 +623,8 @@ int bnpk_rows_kmer_hash(const uint8_t *base, size_t base_bytes, const int64_t *s
                         int64_t *status, void *stream) {
     if (int rc = check_common(enc_mode, lut256, k, 0)) return rc;
     if (n_rows == 0) return 0;
-    RowArgs a{};
-    a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
-    a.k = k; a.offsets = offsets; a.out = hashes_out; a.n_bins = 1; a.status = status;
+    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
+    a.k = k; a.offsets = offsets; a.out = hashes_out; a.status = status;
     return launch_rows_enc<RM_HASH, false, false>(a, enc_mode, n_rows, (cudaStream_t)stream);
 }
 
@@ -641,9 +648,8 @@ int bnpk_rows_minimizers(const uint8_t *base, size_t base_bytes, const int64_t *
     if (window_size < 1) return set_err(BNPK_E_WINDOW, "window_size must be positive");
     if (int rc = check_common(enc_mode, lut256, k, window_size)) return rc;
     if (n_rows == 0) return 0;
-    RowArgs a{};
-    a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
-    a.k = k; a.window = window_size; a.offsets = offsets; a.out = mins_out; a.n_bins = 1; a.status = status;
+    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
+    a.k = k; a.window = window_size; a.offsets = offsets; a.out = mins_out; a.status = status;
     return launch_rows_enc<RM_MINIMIZER, false, false>(a, enc_mode, n_rows, (cudaStream_t)stream);
 }
 
@@ -654,8 +660,7 @@ int bnpk_rows_kmer_count(const uint8_t *base, size_t base_bytes, const int64_t *
     if (n_bins < 1) return set_err(BNPK_E_BINS, "n_bins must be positive");
     if (hist_mode == BNPK_HIST_SMEM && n_bins > kSmemMaxBins) return set_err(BNPK_E_BINS, "too many bins for the shared-memory histogram");
     if (n_rows == 0) return 0;
-    RowArgs a{};
-    a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
+    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
     a.k = k; a.window = window_size; a.n_bins = (uint64_t)n_bins; a.hist = (unsigned long long *)hist; a.status = status;
     const bool sm = use_smem_hist(n_bins, hist_mode);
     cudaStream_t st = (cudaStream_t)stream;
@@ -676,9 +681,8 @@ int bnpk_rows_kmer_hash_canonical(const uint8_t *base, size_t base_bytes, const 
     if (int rc = check_common(enc_mode, lut256, k, 0)) return rc;
     if (complement_xor < 1 || complement_xor > 3) return set_err(BNPK_E_BADARG, "complement_xor must be 1, 2 or 3");
     if (n_rows == 0) return 0;
-    RowArgs a{};
-    a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
-    a.k = k; a.offsets = offsets; a.out = hashes_out; a.n_bins = 1; a.status = status;
+    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
+    a.k = k; a.offsets = offsets; a.out = hashes_out; a.status = status;
     a.canon_xor = canon_pattern(complement_xor);
     return launch_rows_enc<RM_HASH, false, false>(a, enc_mode, n_rows, (cudaStream_t)stream);
 }
@@ -691,8 +695,7 @@ int bnpk_rows_kmer_count_canonical(const uint8_t *base, size_t base_bytes, const
     if (n_bins < 1) return set_err(BNPK_E_BINS, "n_bins must be positive");
     if (hist_mode == BNPK_HIST_SMEM && n_bins > kSmemMaxBins) return set_err(BNPK_E_BINS, "too many bins for the shared-memory histogram");
     if (n_rows == 0) return 0;
-    RowArgs a{};
-    a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
+    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
     a.k = k; a.n_bins = (uint64_t)n_bins; a.hist = (unsigned long long *)hist; a.status = status;
     a.canon_xor = canon_pattern(complement_xor);
     cudaStream_t st = (cudaStream_t)stream;
@@ -710,9 +713,8 @@ int bnpk_rows_kmer_table_insert(const uint8_t *base, size_t base_bytes, const in
     if (complement_xor < 0 || complement_xor > 3) return set_err(BNPK_E_BADARG, "complement_xor must be 0, 1, 2 or 3");
     if (!is_pow2(capacity)) return set_err(BNPK_E_BADARG, "table capacity must be a power of two");
     if (n_rows == 0) return 0;
-    RowArgs a{};
-    a.base = base; a.base_bytes = base_bytes; a.starts = starts; a.lens = lens; a.n_rows = n_rows; a.lut = lut256;
-    a.k = k; a.n_bins = 1; a.status = status;
+    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
+    a.k = k; a.status = status;
     a.canon_xor = complement_xor ? canon_pattern(complement_xor) : 0;
     a.table.keys = (unsigned long long *)keys; a.table.counts = (unsigned long long *)counts;
     a.table.mask = capacity - 1; a.table.n_used = (unsigned long long *)n_used;

@@ -47,33 +47,23 @@ class AlphabetEncoding(OneToOneEncoding):
         raise EncodingError(f"Error when encoding to {self.__class__.__name__}({''.join(self._raw_alphabet)}). "
                             f"Invalid character at flat offset {offset}", offset)
 
-    def _encode_rows(self, base, starts, lens):
+    def _encode_rows(self, rows):
         from .. import ops
-        mode = self.enc_mode
-        lut = self.device_lut(base.device) if mode == nv.ENC_LUT else None
-        codes, offsets, status = ops.rows_encode(base, starts, lens, mode, lut)
-        bad = ops.read_status(status).bad_base()
-        if bad is not None:
-            self._raise_encoding_error(bad[0], bad[1], lens)
+        codes, _, status = ops.rows_encode(rows.base, rows.starts, rows.lens, rows.enc_mode, rows.lut)
+        rows.raise_bad_base(status)
         return codes
 
     def _encode(self, byte_tensor):
         """Flat bytes -> codes (alphabet_encoding.py:34-46), as one row."""
-        if not byte_tensor.is_cuda:
-            raise nv.NativeLibraryError("encoding needs a CUDA tensor: bionumpy_b200 has no CPU fallback")
-        flat = byte_tensor.reshape(-1).contiguous()
-        if flat.dtype != torch.uint8:
-            flat = flat.to(torch.uint8)
-        starts = torch.zeros(1, dtype=torch.int64, device=flat.device)
-        lens = torch.full((1,), flat.numel(), dtype=torch.int32, device=flat.device)
-        return self._encode_rows(flat, starts, lens).reshape(byte_tensor.shape)
+        from ..rows import RowView
+        rows = RowView(EncodedArray(byte_tensor.reshape(-1), BaseEncoding), self)
+        return self._encode_rows(rows).reshape(byte_tensor.shape)
 
     def _encode_ragged(self, ragged):
         """Encode a (base, starts, lens) view straight from the raw chunk -- no gather pass."""
-        base = ragged._data.contiguous()
-        lens = ragged._lens.contiguous()
-        codes = self._encode_rows(base, ragged._starts.contiguous(), lens)
-        return EncodedRaggedArray(EncodedArray(codes, self), lens)
+        from ..rows import RowView
+        rows = RowView(ragged, self)
+        return EncodedRaggedArray(EncodedArray(self._encode_rows(rows), self), rows.lens)
 
     def _decode(self, encoded):
         alpha = torch.from_numpy(self._alphabet).to(encoded.device)

@@ -128,21 +128,18 @@ class CudaOneLineBuffer:
     def can_fuse_count(self) -> bool:
         return True
 
-    def fused_kmer_histogram(self, k, window_size, n_bins, enc_mode, lut):
+    def fused_kmer_histogram(self, k, window_size, n_bins, rows):
+        """``rows``: the RowView of this buffer's sequence field, as the k-mer functions read it."""
         hist, status = ops.chunk_kmer_count(self._data, k, n_bins, None, window_size, self.n_lines_per_entry,
-                                            ord(self.HEADER), False, 1 if self._cr else 0, enc_mode, lut)
+                                            ord(self.HEADER), False, 1 if self._cr else 0, rows.enc_mode, rows.lut)
         st = ops.read_status(status)
         if st.overflow:
             # pathological line structure (more odd rows than the fused pass keeps scratch for):
             # take the general two-kernel route over the row-offset vector instead
-            seq = self.get_field_by_number(1)
-            hist, status = ops.rows_kmer_count(seq._data, seq._starts.contiguous(), seq._lens.contiguous(), enc_mode,
-                                               k, n_bins, window_size, lut)
+            hist, status = ops.rows_kmer_count(rows.base, rows.starts, rows.lens, rows.enc_mode, k, n_bins, window_size,
+                                               rows.lut)
             st = ops.read_status(status)
-        bad = st.bad_base(self._n_records)
-        if bad is not None:
-            from ..encodings.alphabet_encoding import DNAEncoding
-            DNAEncoding._raise_encoding_error(bad[0], bad[1], self.get_field_by_number(1)._lens)
+        rows.raise_bad_base(st)
         return hist
 
 

@@ -136,6 +136,16 @@ def row_offsets(lens, shrink=0):
     return out
 
 
+def _ragged_out(lens, shrink, offsets, total, dtype):
+    """The flat output of a row op and its row offsets: max(lens - shrink, 0) values per row unless ``offsets``
+    (int64[R+1]) are given, ``total`` values (default offsets[-1])."""
+    if offsets is None:
+        offsets = row_offsets(lens, shrink)
+    if total is None:
+        total = int(offsets[-1].item())
+    return torch.empty(total, dtype=dtype, device=lens.device), offsets
+
+
 def _rows_args(base, starts, lens):
     _need_cuda(base, "base")
     _need_cuda(starts, "starts")
@@ -146,11 +156,8 @@ def _rows_args(base, starts, lens):
 
 
 @_on_device
-def rows_encode(base, starts, lens, enc_mode, lut=None, offsets=None, status=None):
-    if offsets is None:
-        offsets = row_offsets(lens, 0)
-    total = int(offsets[-1].item())
-    out = torch.empty(total, dtype=torch.uint8, device=base.device)
+def rows_encode(base, starts, lens, enc_mode, lut=None, offsets=None, status=None, total=None):
+    out, offsets = _ragged_out(lens, 0, offsets, total, torch.uint8)
     if status is None:
         status = nv.new_status(base.device)
     check(lib().bnpk_rows_encode(*_rows_args(base, starts, lens), enc_mode, ptr(lut), ptr(offsets), ptr(out),
@@ -160,11 +167,7 @@ def rows_encode(base, starts, lens, enc_mode, lut=None, offsets=None, status=Non
 
 @_on_device
 def rows_kmer_hash(base, starts, lens, enc_mode, k, lut=None, offsets=None, status=None, total=None):
-    if offsets is None:
-        offsets = row_offsets(lens, k - 1)
-    if total is None:
-        total = int(offsets[-1].item())
-    out = torch.empty(total, dtype=torch.int64, device=base.device)
+    out, offsets = _ragged_out(lens, k - 1, offsets, total, torch.int64)
     if status is None:
         status = nv.new_status(base.device)
     check(lib().bnpk_rows_kmer_hash(*_rows_args(base, starts, lens), enc_mode, ptr(lut), k, ptr(offsets), ptr(out),
@@ -173,12 +176,9 @@ def rows_kmer_hash(base, starts, lens, enc_mode, k, lut=None, offsets=None, stat
 
 
 @_on_device
-def rows_generic_hash(base, starts, lens, alphabet_size, k, lut=None, offsets=None, status=None):
+def rows_generic_hash(base, starts, lens, alphabet_size, k, lut=None, offsets=None, status=None, total=None):
     """sum_j code[i+j] * alphabet_size^j for alphabets that are not four letters (K3')."""
-    if offsets is None:
-        offsets = row_offsets(lens, k - 1)
-    total = int(offsets[-1].item())
-    out = torch.empty(total, dtype=torch.int64, device=base.device)
+    out, offsets = _ragged_out(lens, k - 1, offsets, total, torch.int64)
     if status is None:
         status = nv.new_status(base.device)
     check(lib().bnpk_rows_generic_hash(*_rows_args(base, starts, lens), ptr(lut), alphabet_size, k, ptr(offsets),
@@ -188,11 +188,7 @@ def rows_generic_hash(base, starts, lens, alphabet_size, k, lut=None, offsets=No
 
 @_on_device
 def rows_minimizers(base, starts, lens, enc_mode, k, window_size, lut=None, offsets=None, status=None, total=None):
-    if offsets is None:
-        offsets = row_offsets(lens, window_size - 1)
-    if total is None:
-        total = int(offsets[-1].item())
-    out = torch.empty(total, dtype=torch.int64, device=base.device)
+    out, offsets = _ragged_out(lens, window_size - 1, offsets, total, torch.int64)
     if status is None:
         status = nv.new_status(base.device)
     check(lib().bnpk_rows_minimizers(*_rows_args(base, starts, lens), enc_mode, ptr(lut), k, window_size,
@@ -213,24 +209,18 @@ def rows_kmer_count(base, starts, lens, enc_mode, k, n_bins, window_size=0, lut=
 
 
 @_on_device
-@_on_device
-def rows_reverse_complement(base, starts, lens, lut, offsets=None):
+def rows_reverse_complement(base, starts, lens, lut, offsets=None, total=None):
     """get_reverse_complement on a ragged view: out row r = lut[row r backwards] (uint8, contiguous rows)."""
-    if offsets is None:
-        offsets = row_offsets(lens, 0)
-    total = int(offsets[-1].item())
-    out = torch.empty(total, dtype=torch.uint8, device=base.device)
+    out, offsets = _ragged_out(lens, 0, offsets, total, torch.uint8)
     check(lib().bnpk_rows_reverse_complement(*_rows_args(base, starts, lens), ptr(lut), ptr(offsets), ptr(out), stream_ptr()))
     return out, offsets
 
 
 @_on_device
-def rows_kmer_hash_canonical(base, starts, lens, enc_mode, k, complement_xor, lut=None, offsets=None, status=None):
+def rows_kmer_hash_canonical(base, starts, lens, enc_mode, k, complement_xor, lut=None, offsets=None, status=None,
+                             total=None):
     """EXTENSION: min(h, hash of the reverse complement) for every k-mer (K3 with a second strand)."""
-    if offsets is None:
-        offsets = row_offsets(lens, k - 1)
-    total = int(offsets[-1].item())
-    out = torch.empty(total, dtype=torch.int64, device=base.device)
+    out, offsets = _ragged_out(lens, k - 1, offsets, total, torch.int64)
     if status is None:
         status = nv.new_status(base.device)
     check(lib().bnpk_rows_kmer_hash_canonical(*_rows_args(base, starts, lens), enc_mode, ptr(lut), k, complement_xor,
@@ -298,11 +288,7 @@ def rows_pwm_scores(base, starts, lens, enc_mode, matrix, lut=None, tail=False, 
     """K7: motif scores of every window of the rows (every position with ``tail``), float64, in column order.
     ``matrix`` is [motif_len, alphabet_size] on the device.  Returns (scores, offsets, status)."""
     alphabet_size = matrix.shape[-1] if matrix.dim() == 2 else 0
-    if offsets is None:
-        offsets = row_offsets(lens, 0 if tail else max(matrix.shape[0] - 1, 0))
-    if total is None:
-        total = int(offsets[-1].item())
-    out = torch.empty(total, dtype=torch.float64, device=base.device)
+    out, offsets = _ragged_out(lens, 0 if tail else max(matrix.shape[0] - 1, 0), offsets, total, torch.float64)
     if status is None:
         status = nv.new_status(base.device)
     check(lib().bnpk_rows_pwm_scores(*_rows_args(base, starts, lens), enc_mode, *_pwm_args(matrix, alphabet_size, lut),

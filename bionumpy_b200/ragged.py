@@ -258,3 +258,32 @@ class RaggedArray:
     def __repr__(self):
         rows = self.tolist()
         return f"ragged_array({rows})"
+
+
+class LazyRaggedArray(RaggedArray):
+    """A contiguous RaggedArray with max(lens - shrink, 0) values per row (the windows of rows of ``lens`` bases) whose
+    flat data ``_compute()`` makes on first use."""
+
+    def __init__(self, lens, shrink):
+        self._lens = torch.clamp(lens - shrink, min=0).to(torch.int32)
+        ends = torch.cumsum(self._lens.to(torch.int64), 0)
+        self._starts = ends - self._lens
+        self._contiguous = True
+        self._lazy = None
+
+    def _compute(self):
+        raise NotImplementedError
+
+    # RaggedArray keeps its flat data in ``_data``; here it is computed on demand
+    @property
+    def _data(self):
+        if self._lazy is None:
+            self._lazy = self._compute()
+        return self._lazy
+
+    @_data.setter
+    def _data(self, v):
+        self._lazy = v
+
+    def is_materialised(self):
+        return self._lazy is not None

@@ -13,6 +13,7 @@ from .. import _native as nv
 from .. import ops
 from ..encoded_array import EncodedArray, EncodedRaggedArray, as_encoded_array
 from ..encodings.alphabet_encoding import AlphabetEncoding
+from ..rows import RowView
 from ..streams import streamable
 
 _complements = {"A": "T", "G": "C", "C": "G", "T": "A", "N": "N"}
@@ -67,19 +68,12 @@ def get_reverse_complement(sequence):
     sequence = as_encoded_array(sequence)
     if isinstance(sequence, EncodedArray):
         assert sequence.ndim == 1, "only 1-D EncodedArray and EncodedRaggedArray are supported"
-        data = sequence.raw().contiguous()
-        starts = torch.zeros(1, dtype=torch.int64, device=data.device)
-        lens = torch.full((1,), data.numel(), dtype=torch.int32, device=data.device)
-    else:
-        data, starts, lens = sequence._data.contiguous(), sequence._starts.contiguous(), sequence._lens.contiguous()
-    if not data.is_cuda:
-        raise nv.NativeLibraryError("get_reverse_complement needs CUDA tensors: bionumpy_b200 has no CPU fallback")
-    if data.dtype != torch.uint8:
-        data = data.to(torch.uint8)
-    out, _ = ops.rows_reverse_complement(data, starts, lens, _device_table(sequence.encoding, data.device))
-    if isinstance(sequence, EncodedArray):
+    rows = RowView(sequence)
+    lut = _device_table(sequence.encoding, rows.base.device)
+    out, _ = ops.rows_reverse_complement(rows.base, rows.starts, rows.lens, lut)
+    if rows.flat:
         return EncodedArray(out, sequence.encoding)
-    return EncodedRaggedArray(EncodedArray(out, sequence.encoding), lens)
+    return EncodedRaggedArray(EncodedArray(out, sequence.encoding), rows.lens)
 
 
 def complement_xor_of(alphabet_encoding) -> int:

@@ -25,7 +25,8 @@ from .. import ops
 from ..encoded_array import EncodedArray, EncodedRaggedArray
 from ..encodings.exceptions import EncodingError
 from ..streams import _is_stream
-from .kmers import LONG_ROW, _check_bad_base, _source_of, _split_long_rows
+from ..rows import LONG_ROW
+from .kmers import _source_of, rescan_kmers
 
 MAX_LOAD = 0.5            # keys per slot the table may reach; every insert launch stays within it
 MIN_BATCH = 1 << 20       # k-mer positions: grow rather than launch on less free room than this
@@ -222,27 +223,27 @@ class KmerCounter:
             self._insert(src)
         return self
 
-    def _insert(self, src):
+    def _insert(self, rows):
         k = self.k
-        starts, lens = src.starts, src.lens
-        offsets = ops.row_offsets(lens, k - 1)
-        total, longest = torch.stack([offsets[-1], lens.max().to(torch.int64)]).tolist()
+        offsets = ops.row_offsets(rows.lens, k - 1)
+        total, longest = torch.stack([offsets[-1], rows.lens.max().to(torch.int64)]).tolist()
+        pieces = rows
         if longest > LONG_ROW + k - 1:
             # chromosome-length rows: pieces of LONG_ROW positions, one warp each (same positions, same total)
-            starts, lens, _ = _split_long_rows(starts, lens, k)
-            offsets = ops.row_offsets(lens, k - 1)
+            pieces = rows.split(k)[0]
+            offsets = ops.row_offsets(pieces.lens, k - 1)
         n_used_t = self._state[nv.ST_WORDS:]
         row, done = 0, 0
-        while row < lens.numel():
+        while row < pieces.lens.numel():
             slots, end, end_pos = plan_insert(offsets, row, done, total, self._n_used, self._slots, MIN_BATCH)
             if slots != self._slots:
                 self._grow(slots)
-            ops.rows_kmer_table_insert(src.base, starts[row:end], lens[row:end], src.enc_mode, k, self._keys,
-                                       self._counts, n_used_t, self._cxor, src.lut, status=self._status())
+            ops.rows_kmer_table_insert(rows.base, pieces.starts[row:end], pieces.lens[row:end], rows.enc_mode, k,
+                                       self._keys, self._counts, n_used_t, self._cxor, rows.lut, status=self._status())
             words = self._read_state()
             if words[nv.ST_BAD_BASE] != nv.INT64_MAX:
                 try:
-                    _check_bad_base(src, self._state[:nv.ST_WORDS], split=True)
+                    rows.raise_bad_base(self._state[:nv.ST_WORDS], rescan_kmers)
                 except EncodingError as e:
                     self._error = e
                     raise

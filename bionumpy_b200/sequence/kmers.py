@@ -9,154 +9,83 @@ import logging
 
 import torch
 
-from .. import _native as nv
 from .. import config, ops
-from ..encoded_array import EncodedArray, EncodedRaggedArray, BaseEncoding
+from ..encoded_array import EncodedArray, EncodedRaggedArray
 from ..encodings.alphabet_encoding import AlphabetEncoding, DNAEncoding
 from ..encodings.exceptions import EncodingError
 from ..encodings.kmer_encodings import KmerEncoding
+from ..ragged import LazyRaggedArray
+from ..rows import LONG_ROW, RowView, _split_long_rows  # noqa: F401 (the split is also imported from here)
 from ..streams import streamable
 from .count_encoded import count_encoded, count_hashed, EncodedCounts
 
 logger = logging.getLogger(__name__)
 
 
-class _Source:
-    """The ragged byte view a lazy value array is computed from."""
-
-    def __init__(self, base, starts, lens, enc_mode, lut, alphabet_encoding, chunk_buffer=None):
-        self.base, self.starts, self.lens = base, starts, lens
-        self.enc_mode, self.lut, self.alphabet_encoding = enc_mode, lut, alphabet_encoding
-        self.chunk_buffer = chunk_buffer     # set when the view is an untouched field of a file buffer
-
-
-def _source_of(sequence) -> _Source:
+def _source_of(sequence) -> RowView:
+    """The rows k-mers are taken from: text is read as DNAEncoding (kmers.py:70-72), encoded arrays need an
+    AlphabetEncoding."""
     if isinstance(sequence, EncodedArray):
         assert sequence.ndim == 1, "only 1-D EncodedArray and EncodedRaggedArray are supported"
-        data = sequence.raw().contiguous()
-        starts = torch.zeros(1, dtype=torch.int64, device=data.device)
-        lens = torch.full((1,), data.numel(), dtype=torch.int32, device=data.device)
-    else:
-        data = sequence._data.contiguous()
-        starts, lens = sequence._starts.contiguous(), sequence._lens.contiguous()
-    if not data.is_cuda:
-        raise nv.NativeLibraryError("k-mer kernels need CUDA tensors: bionumpy_b200 has no CPU fallback")
-    if data.dtype != torch.uint8:
-        data = data.to(torch.uint8)
-    enc = sequence.encoding
-    if enc.is_base_encoding():
-        target = DNAEncoding                                    # kmers.py:70-72
-        return _Source(data, starts, lens, target.enc_mode, None, target,
-                       getattr(sequence, "_chunk_buffer", None))
-    assert isinstance(enc, AlphabetEncoding), \
+    rows = RowView(sequence, DNAEncoding)
+    assert isinstance(rows.alphabet_encoding, AlphabetEncoding), \
         "Sequence needs to be encoded with an AlphabetEncoding, e.g. DNAEncoding. " \
         "Change encoding of your sequences by using e.g. bnp.change_encoding(sequences, bnp.DNAEncoding)"
-    return _Source(data, starts, lens, nv.ENC_CODES, None, enc)
+    return rows
 
 
-LONG_ROW = 1 << 14          # rows longer than this are cut into overlapping pieces, one warp each
+def rescan_kmers(rows: RowView):
+    """The status of counting the rows' 1-mers: it reads every byte, so it places a bad base that a launch on pieces
+    or batches of the rows reported (error path)."""
+    return ops.rows_kmer_count(rows.base, rows.starts, rows.lens, rows.enc_mode, 1, 4, 0, rows.lut)[1]
 
 
-def _split_long_rows(starts, lens, span, out_offsets=None, piece=LONG_ROW):
-    """Rows longer than ``piece`` positions become pieces [i*piece, (i+1)*piece + span - 1): every k-mer /
-    window start belongs to exactly one piece, so counts and (with ``out_offsets``) materialised values are
-    unchanged while long rows (chromosomes) spread over many warps.  Index arithmetic only (torch);
-    returns (starts, lens, out_offsets) of the pieces."""
-    L = lens.to(torch.int64)
-    if L.numel() == 0 or int(L.max().item()) <= piece + span - 1:
-        return starts, lens, out_offsets
-    n_pos = torch.clamp(L - (span - 1), min=0)                       # window starts per row
-    n_pieces = torch.clamp((n_pos + piece - 1) // piece, min=1)
-    row = torch.repeat_interleave(torch.arange(L.numel(), device=L.device), n_pieces)
-    first = torch.cumsum(n_pieces, 0) - n_pieces
-    idx = torch.arange(row.numel(), device=L.device) - first[row]    # piece index inside its row
-    p_start = starts[row] + idx * piece
-    p_len = torch.minimum(L[row] - idx * piece, torch.full_like(idx, piece + span - 1))
-    p_off = None if out_offsets is None else out_offsets[:-1][row] + idx * piece
-    return p_start.contiguous(), p_len.to(torch.int32).contiguous(), p_off
-
-
-def _check_bad_base(source: _Source, status, split=False):
-    """Raise the reference's EncodingError(offset) if the status block reports a byte outside the alphabet.  With
-    ``split``, the kernel ran on other rows than ``source``'s (pieces of long rows, batches), so the (row, position)
-    is recomputed on the source rows (error path)."""
-    bad = ops.read_status(status).bad_base()
-    if bad is not None and split:
-        _, status = ops.rows_kmer_count(source.base, source.starts, source.lens, source.enc_mode, 1, 4, 0, source.lut)
-        bad = ops.read_status(status).bad_base()
-    if bad is not None:
-        logging.error("Tried to change encoding of sequences to DNAEncoding, but failed. "
-                      "Make sure your sequences are valid DNA, only containing A, C, G, and T")
-        source.alphabet_encoding._raise_encoding_error(bad[0], bad[1], source.lens)
-
-
-class LazyKmerValues(EncodedRaggedArray):
+class LazyKmerValues(LazyRaggedArray, EncodedRaggedArray):
     """EncodedRaggedArray of k-mer hashes / minimizers whose int64 data appear on first use."""
 
-    def __init__(self, source: _Source, k: int, window_size: int, flat_input: bool = False, canonical: bool = False):
-        self._source, self._k, self._window = source, k, window_size
+    def __init__(self, rows: RowView, k: int, window_size: int, canonical: bool = False):
+        self._rows, self._k, self._window = rows, k, window_size
         self._canonical = canonical
         if canonical:
             from .dna import complement_xor_of
             assert window_size == 0, "canonical minimizers are not implemented"
-            self._cxor = complement_xor_of(source.alphabet_encoding)
-        shrink = (window_size if window_size else k) - 1
-        self._lens = torch.clamp(source.lens - shrink, min=0).to(torch.int32)
-        ends = torch.cumsum(self._lens.to(torch.int64), 0)
-        self._starts = ends - self._lens
-        self._contiguous = True
-        self._encoding = KmerEncoding(source.alphabet_encoding, k)
-        self._lazy = None
-        self._flat_input = flat_input
+            self._cxor = complement_xor_of(rows.alphabet_encoding)
+        super().__init__(rows.lens, (window_size if window_size else k) - 1)
+        self._encoding = KmerEncoding(rows.alphabet_encoding, k)
 
-    # RaggedArray keeps its flat data in ``_data``; here it is computed on demand
-    @property
-    def _data(self):
-        if self._lazy is None:
-            s = self._source
-            shrink = (self._window if self._window else self._k) - 1
-            if s.alphabet_encoding.alphabet_size != 4:
-                # the reference's generic dot-product path (kmers.py:87): plain k-mers only
-                if self._window:
-                    raise NotImplementedError("minimizers are only implemented for 4-letter alphabets")
-                vals, _, status = ops.rows_generic_hash(s.base, s.starts, s.lens, s.alphabet_encoding.alphabet_size,
-                                                        self._k, None)
-                self._lazy = vals
-                return self._lazy
-            offsets = ops.row_offsets(s.lens, shrink)
-            p_starts, p_lens, p_off = _split_long_rows(s.starts, s.lens, shrink + 1, offsets)
-            if p_off is not None and p_off is not offsets:
-                total = int(offsets[-1].item())
-                p_off = torch.cat([p_off, offsets[-1:]]).contiguous()   # kernels read offsets[row] only
-            else:
-                total, p_off = None, offsets
+    def _compute(self):
+        s = self._rows
+        if s.alphabet_encoding.alphabet_size != 4:
+            # the reference's generic dot-product path (kmers.py:87): plain k-mers only
             if self._window:
-                vals, _, status = ops.rows_minimizers(s.base, p_starts, p_lens, s.enc_mode, self._k, self._window,
-                                                      s.lut, p_off, total=total)
-            elif self._canonical:
-                vals, _, status = ops.rows_kmer_hash_canonical(s.base, s.starts, s.lens, s.enc_mode, self._k, self._cxor,
-                                                               s.lut, offsets)
-                p_starts = s.starts
-            else:
-                vals, _, status = ops.rows_kmer_hash(s.base, p_starts, p_lens, s.enc_mode, self._k, s.lut, p_off,
-                                                     total=total)
-            self._check(status, split=p_starts is not s.starts)
-            self._lazy = vals
-        return self._lazy
-
-    @_data.setter
-    def _data(self, v):
-        self._lazy = v
-
-    def is_materialised(self):
-        return self._lazy is not None
+                raise NotImplementedError("minimizers are only implemented for 4-letter alphabets")
+            vals, _, status = ops.rows_generic_hash(s.base, s.starts, s.lens, s.alphabet_encoding.alphabet_size, self._k, None)
+            return vals
+        span = self._window if self._window else self._k
+        p, offsets, total, piece_row = s.split(span, ops.row_offsets(s.lens, span - 1))
+        if self._window:
+            vals, _, status = ops.rows_minimizers(s.base, p.starts, p.lens, s.enc_mode, self._k, self._window, s.lut,
+                                                  offsets, total=total)
+        elif self._canonical:
+            vals, _, status = ops.rows_kmer_hash_canonical(s.base, p.starts, p.lens, s.enc_mode, self._k, self._cxor,
+                                                           s.lut, offsets, total=total)
+        else:
+            vals, _, status = ops.rows_kmer_hash(s.base, p.starts, p.lens, s.enc_mode, self._k, s.lut, offsets,
+                                                 total=total)
+        self._check(status, split=piece_row is not None)
+        return vals
 
     def _check(self, status, split=False):
-        _check_bad_base(self._source, status, split)
+        try:
+            self._rows.raise_bad_base(status, rescan_kmers if split else None)
+        except EncodingError:
+            logging.error("Tried to change encoding of sequences to DNAEncoding, but failed. "
+                          "Make sure your sequences are valid DNA, only containing A, C, G, and T")
+            raise
 
     def fused_histogram(self, n_bins: int) -> torch.Tensor:
         """hist[b] = #{values == b (mod n_bins)} without writing the values (K3/K4 + K5 fused)."""
-        s = self._source
+        s = self._rows
         if s.alphabet_encoding.alphabet_size != 4:
             hist, _ = ops.bincount(self._data.contiguous(), n_bins)
             return hist
@@ -166,11 +95,10 @@ class LazyKmerValues(EncodedRaggedArray):
             return hist
         buf = s.chunk_buffer
         if buf is not None and buf.can_fuse_count():
-            return buf.fused_kmer_histogram(self._k, self._window, n_bins, s.enc_mode, s.lut)
-        span = self._window if self._window else self._k
-        p_starts, p_lens, _ = _split_long_rows(s.starts, s.lens, span)
-        hist, status = ops.rows_kmer_count(s.base, p_starts, p_lens, s.enc_mode, self._k, n_bins, self._window, s.lut)
-        self._check(status, split=p_starts is not s.starts)
+            return buf.fused_kmer_histogram(self._k, self._window, n_bins, s)
+        p, _, _, piece_row = s.split(self._window if self._window else self._k)
+        hist, status = ops.rows_kmer_count(s.base, p.starts, p.lens, s.enc_mode, self._k, n_bins, self._window, s.lut)
+        self._check(status, split=piece_row is not None)
         return hist
 
 
@@ -179,8 +107,7 @@ def get_kmers(sequence, k: int, canonical: bool = False):
     AlphabetEncoding with four letters; k in 1..31.  EXTENSION: ``canonical=True`` gives min(hash, hash of the
     reverse complement) for every k-mer (sequence/dna.py)."""
     assert 0 < k < 32, "k must be larger than 0 and smaller than 32"
-    src = _source_of(sequence)
-    out = LazyKmerValues(src, k, 0, canonical=canonical)
+    out = LazyKmerValues(_source_of(sequence), k, 0, canonical=canonical)
     if not config.LAZY:
         out._data
     if isinstance(sequence, EncodedArray):

@@ -12,8 +12,7 @@ def get_minimizers(sequence, k: int, window_size: int):
         "Sequence needs to be encoded with an AlphabetEncoding, e.g. DNAEncoding"
     assert k <= window_size, "kmer size must be smaller than window size"
     assert 0 < k < 32, "k must be larger than 0 and smaller than 32"
-    src = _source_of(sequence)
-    out = LazyKmerValues(src, k, window_size)
+    out = LazyKmerValues(_source_of(sequence), k, window_size)
     if not config.LAZY:
         out._data
     if isinstance(sequence, EncodedArray):

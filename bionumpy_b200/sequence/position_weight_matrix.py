@@ -13,12 +13,11 @@ from typing import Dict
 import numpy as np
 import torch
 
-from .. import _native as nv
 from .. import config, ops
 from ..encoded_array import EncodedArray, EncodedRaggedArray, as_encoded_array
 from ..encodings.alphabet_encoding import AlphabetEncoding
-from ..ragged import RaggedArray, segment_max
-from .kmers import LONG_ROW, _split_long_rows
+from ..ragged import LazyRaggedArray, segment_max
+from ..rows import RowView
 
 MAX_MOTIF_LEN = 1024          # the row kernels' segment overlap
 MAX_TABLE_CELLS = 8192        # alphabet_size * motif length doubles: 64 KiB of shared memory
@@ -28,14 +27,6 @@ def _pwm_from_counts(count_matrix):
     """position_weight_matrix.py:26-28."""
     with_pseudo = count_matrix + 1
     return np.log(with_pseudo / with_pseudo.sum(axis=0, keepdims=True))
-
-
-class _Rows:
-    """The ragged byte view a motif is scored on, and how the kernels read it."""
-
-    def __init__(self, base, starts, lens, enc_mode, lut, encoding, flat):
-        self.base, self.starts, self.lens = base, starts, lens
-        self.enc_mode, self.lut, self.encoding, self.flat = enc_mode, lut, encoding, flat
 
 
 class PWM:
@@ -97,7 +88,7 @@ class PWM:
             self._dev_matrix[key] = torch.from_numpy(t).to(device)
         return self._dev_matrix[key]
 
-    def _rows(self, sequence) -> _Rows:
+    def _rows(self, sequence) -> RowView:
         """as_valid_encoded_array (position_weight_matrix.py:45-55) as a kernel input: text is read with
         AlphabetEncoding(alphabet); an AlphabetEncoding array is read as codes when its alphabet starts with this one
         and every code is below len(alphabet)."""
@@ -106,28 +97,10 @@ class PWM:
             sequence = as_encoded_array(sequence)
         if not isinstance(sequence, (EncodedArray, EncodedRaggedArray)):
             raise TypeError(f"cannot score {type(sequence)}")
+        rows = RowView(sequence, self._encoding)
         enc = sequence.encoding
-        if isinstance(sequence, EncodedArray):
-            data = sequence.raw().reshape(-1) if sequence.ndim == 1 else sequence.raw().contiguous()
-            if sequence.ndim == 1:
-                starts = torch.zeros(1, dtype=torch.int64, device=data.device)
-                lens = torch.full((1,), data.numel(), dtype=torch.int32, device=data.device)
-            else:
-                n, w = data.shape
-                starts = torch.arange(n, dtype=torch.int64, device=data.device) * w
-                lens = torch.full((n,), w, dtype=torch.int32, device=data.device)
-            data, flat = data.reshape(-1).contiguous(), sequence.ndim == 1
-        else:
-            data, starts, lens, flat = sequence._data.contiguous(), sequence._starts.contiguous(), \
-                sequence._lens.contiguous(), False
-        if not data.is_cuda:
-            raise nv.NativeLibraryError("motif scores need CUDA tensors: bionumpy_b200 has no CPU fallback")
-        if data.dtype != torch.uint8:
-            data = data.to(torch.uint8)
         if enc.is_base_encoding():
-            mode = self._encoding.enc_mode
-            lut = self._encoding.device_lut(data.device) if mode == nv.ENC_LUT else None
-            return _Rows(data, starts, lens, mode, lut, self._encoding, flat)
+            return rows
         if isinstance(enc, AlphabetEncoding):
             alphabet = list(enc.get_alphabet())
             s_alphabet = list(self._alphabet)
@@ -135,52 +108,36 @@ class PWM:
             top = int(codes.max().item()) if codes.numel() else 0
             if not alphabet[:len(self._alphabet)] == s_alphabet or top >= len(self._alphabet):
                 raise Exception(f'Could not calculate pwm for alphabet {s_alphabet} on {alphabet} encoded array')
-            return _Rows(data, starts, lens, nv.ENC_CODES, None, self._encoding, flat)
+            return rows
         as_encoded_array(sequence, self._encoding)          # raises the reference's EncodingException
         raise TypeError(f"cannot score an array encoded with {enc}")
 
-    def _check(self, rows: _Rows, status, split=False):
-        """EncodingError(offset) if a byte is outside the alphabet.  With ``split`` the kernel ran on pieces of the
-        rows, so the (row, position) is found again on the rows themselves (error path)."""
-        bad = ops.read_status(status).bad_base()
-        if bad is not None and split:
-            _, status = ops.rows_pwm_max(rows.base, rows.starts, rows.lens, rows.enc_mode,
-                                         self.device_matrix(rows.base.device), rows.lut)
-            bad = ops.read_status(status).bad_base()
-        if bad is not None:
-            rows.encoding._raise_encoding_error(bad[0], bad[1], rows.lens)
+    def _rescan(self, rows: RowView):
+        """The status of the fused maximum on the rows themselves: it places a bad base that a launch on pieces of
+        the rows reported (error path)."""
+        return ops.rows_pwm_max(rows.base, rows.starts, rows.lens, rows.enc_mode, self.device_matrix(rows.base.device),
+                                rows.lut)[1]
 
-    def _window_scores(self, rows: _Rows):
-        """The scores of every window of every row, flat float64, and the row offsets (shrink m - 1).  Long rows are
-        cut into overlapping pieces, one warp each."""
+    def _window_scores(self, rows: RowView):
+        """The scores of every window of every row, flat float64.  Long rows are cut into overlapping pieces, one warp
+        each."""
         m = self.window_size
         mat = self.device_matrix(rows.base.device)
-        offsets = ops.row_offsets(rows.lens, m - 1)
-        p_starts, p_lens, p_off = _split_long_rows(rows.starts, rows.lens, m, offsets)
-        if p_off is not None and p_off is not offsets:
-            total = int(offsets[-1].item())
-            p_off = torch.cat([p_off, offsets[-1:]]).contiguous()     # the kernel reads offsets[row] only
-        else:
-            total, p_off = None, offsets
-        scores, _, status = ops.rows_pwm_scores(rows.base, p_starts, p_lens, rows.enc_mode, mat, rows.lut,
-                                                offsets=p_off, total=total)
-        self._check(rows, status, split=p_starts is not rows.starts)
-        return scores, offsets
+        p, offsets, total, piece_row = rows.split(m, ops.row_offsets(rows.lens, m - 1))
+        scores, _, status = ops.rows_pwm_scores(rows.base, p.starts, p.lens, rows.enc_mode, mat, rows.lut,
+                                                offsets=offsets, total=total)
+        rows.raise_bad_base(status, self._rescan if piece_row is not None else None)
+        return scores
 
-    def _row_max(self, rows: _Rows):
+    def _row_max(self, rows: RowView):
         """max(axis=-1) of the window scores of every row without writing them: NaN-propagating, -inf for a row
         without a window.  The pieces of a long row are combined on the device."""
-        m = self.window_size
         mat = self.device_matrix(rows.base.device)
-        p_starts, p_lens, _ = _split_long_rows(rows.starts, rows.lens, m)
-        split = p_starts is not rows.starts
-        best, status = ops.rows_pwm_max(rows.base, p_starts, p_lens, rows.enc_mode, mat, rows.lut)
-        self._check(rows, status, split=split)
-        if split:
-            L = rows.lens.to(torch.int64)
-            n_pieces = torch.clamp((torch.clamp(L - (m - 1), min=0) + LONG_ROW - 1) // LONG_ROW, min=1)
-            piece_row = torch.repeat_interleave(torch.arange(L.numel(), device=L.device), n_pieces)
-            best = segment_max(best, piece_row, L.numel())
+        p, _, _, piece_row = rows.split(self.window_size)
+        best, status = ops.rows_pwm_max(rows.base, p.starts, p.lens, rows.enc_mode, mat, rows.lut)
+        rows.raise_bad_base(status, self._rescan if piece_row is not None else None)
+        if piece_row is not None:
+            best = segment_max(best, piece_row, rows.lens.numel())
         return best
 
     # -- scoring ------------------------------------------------------------------------------
@@ -191,7 +148,7 @@ class PWM:
         rows = self._rows(sequence)
         if bool((rows.lens != self.window_size).any().item()):
             raise AssertionError(f"sequence length must be the motif length {self.window_size}")
-        scores, _ = self._window_scores(rows)
+        scores = self._window_scores(rows)
         return scores[0].item() if rows.flat else scores
 
     def calculate_scores(self, sequence) -> torch.Tensor:
@@ -203,7 +160,7 @@ class PWM:
             sequence = sequence.ravel()
         rows = self._rows(sequence)
         m = self.window_size
-        scores, _ = self._window_scores(rows)          # validates every byte, the last m - 1 included
+        scores = self._window_scores(rows)             # validates every byte, the last m - 1 included
         L = int(rows.lens[0].item())
         tail_start = max(L - (m - 1), 0)
         if tail_start == L:
@@ -215,33 +172,19 @@ class PWM:
         return torch.cat([scores[:tail_start], tail])
 
 
-class LazyMotifScores(RaggedArray):
+class LazyMotifScores(LazyRaggedArray):
     """float64 RaggedArray of the window scores of every row, computed on first use; ``max(axis=-1)`` before that runs
     the fused maximum instead."""
 
-    def __init__(self, pwm: PWM, rows: _Rows):
+    def __init__(self, pwm: PWM, rows: RowView):
         self._pwm, self._rows = pwm, rows
-        self._lens = torch.clamp(rows.lens - (pwm.window_size - 1), min=0).to(torch.int32)
-        ends = torch.cumsum(self._lens.to(torch.int64), 0)
-        self._starts = ends - self._lens
-        self._contiguous = True
-        self._lazy = None
+        super().__init__(rows.lens, pwm.window_size - 1)
 
-    @property
-    def _data(self):
-        if self._lazy is None:
-            self._lazy, _ = self._pwm._window_scores(self._rows)
-        return self._lazy
-
-    @_data.setter
-    def _data(self, v):
-        self._lazy = v
-
-    def is_materialised(self):
-        return self._lazy is not None
+    def _compute(self):
+        return self._pwm._window_scores(self._rows)
 
     def max(self, axis=None, **kwargs):
-        if axis in (-1, 1) and self._lazy is None:
+        if axis in (-1, 1) and not self.is_materialised():
             return self._pwm._row_max(self._rows)
         return super().max(axis=axis, **kwargs)
 
@@ -277,8 +220,7 @@ def get_motif_scores(sequence, pwm: PWM):
     """
     rows = pwm._rows(sequence)
     if rows.flat:
-        scores, _ = pwm._window_scores(rows)
-        return scores
+        return pwm._window_scores(rows)
     out = LazyMotifScores(pwm, rows)
     if not config.LAZY:
         out._data

@@ -600,8 +600,8 @@ def test_split_long_rows_puts_every_window_start_in_one_piece(piece, span):
 @gpu
 @pytest.mark.parametrize("k,window", [(21, 0), (31, 0), (15, 40)])
 def test_api_on_rows_cut_into_pieces(k, window):
-    """get_kmers / get_minimizers, count_kmers_hashed and count_kmers_exact on rows around the piece length; a bad
-    byte that only the second piece of a row holds raises EncodingError with the oracle's offset."""
+    """get_kmers (plain and canonical) / get_minimizers, count_kmers_hashed and count_kmers_exact on rows around the
+    piece length; a bad byte that only the second piece of a row holds raises EncodingError with the oracle's offset."""
     import bionumpy_b200 as bnp
     from bionumpy_b200.sequence.kmers import LONG_ROW
     span = window or k
@@ -627,6 +627,8 @@ def test_api_on_rows_cut_into_pieces(k, window):
     assert np.array_equal(bnp.count_kmers_hashed(text, k, B, window_size=window).cpu().numpy(),
                           o.count_bucketed_flat(want, B))
     if not window:
+        want_c, _ = o.canonical_kmers(codes, L, k)
+        assert np.array_equal(bnp.get_kmers(text, k, canonical=True).raw().ravel().cpu().numpy(), want_c)
         u, c = np.unique(want, return_counts=True)
         got_t = bnp.count_kmers_exact(text, k)
         assert np.array_equal(got_t.kmers.cpu().numpy(), u) and np.array_equal(got_t.counts.cpu().numpy(), c)
@@ -644,7 +646,8 @@ def test_api_on_rows_cut_into_pieces(k, window):
     if window:
         calls.append(lambda: bnp.get_minimizers(as_codes(bad_codes), k, window).raw())
     else:
-        calls += [lambda: bnp.get_kmers(bad_text, k).raw(), lambda: bnp.count_kmers_exact(bad_text, k),
+        calls += [lambda: bnp.get_kmers(bad_text, k).raw(), lambda: bnp.get_kmers(bad_text, k, canonical=True).raw(),
+                  lambda: bnp.count_kmers_exact(bad_text, k),
                   lambda: bnp.count_kmers_hashed(as_codes(bad_codes), k, B)]
     for call in calls:
         with pytest.raises(bnp.EncodingError) as got_err:
