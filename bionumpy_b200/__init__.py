@@ -17,7 +17,7 @@ from .encodings import (AlphabetEncoding, DNAEncoding, ACTGEncoding, ACGTEncodin
                         AminoAcidEncoding, RNAENcoding)
 from . import encodings, sequence, io, streams
 from .sequence import (get_kmers, get_minimizers, count_encoded, count_kmers, count_hashed, count_kmers_hashed,
-                       EncodedCounts, complement, get_reverse_complement, get_motif_scores)
+                       EncodedCounts, complement, get_reverse_complement, get_motif_scores, match_string)
 from .streams import streamable, bincount, BnpStream
 from .io import bnp_open, FormatException, IndexedFasta
 from .sequence import KmerIndex, KmerLookup, BloomFilter

@@ -54,6 +54,8 @@ SIGNATURES = {
     "bnpk_kmer_table_rehash": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
     "bnpk_rows_pwm_scores": (_i, [_vp, _sz, _vp, _vp, _sz, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "bnpk_rows_pwm_max": (_i, [_vp, _sz, _vp, _vp, _sz, _i, _vp, _i, _vp, _i, _vp, _vp, _vp]),
+    "bnpk_rows_match": (_i, [_vp, _sz, _vp, _vp, _sz, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "bnpk_rows_match_count": (_i, [_vp, _sz, _vp, _vp, _sz, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "bnpk_bincount": (_i, [_vp, _sz, _i64, _i, _vp, _vp, _vp]),
     "bnpk_bincount_rows": (_i, [_vp, _vp, _sz, _i64, _vp, _vp, _vp]),
     "bnpk_pipeline_create": (_i, [ctypes.POINTER(_vp), _sz, _sz]),

@@ -7,6 +7,7 @@
 //   K3/K4+K5 rows_kmer_count   count_kmers         sequence/kmers.py:129-145
 //   K3 + table rows_kmer_table_insert  exact distinct-k-mer counts (extension, like `jellyfish count`)
 //   K7 rows_pwm_scores / rows_pwm_max  get_motif_scores, PWM.calculate_scores  sequence/position_weight_matrix.py:83-100,166-196
+//   K8 rows_match / rows_match_count   match_string, StringMatcher, RegexMatcher  sequence/string_matcher.py
 // plus the clean-up passes of the fused chunk count (long rows, trailing incomplete entry).
 #include <climits>
 #include "bnpk_host.h"
@@ -20,10 +21,24 @@ constexpr int kSegBytes = kSegUnits * 16;
 constexpr int kWarpWords = 2 * kSegUnits + 4;
 
 enum { RM_ENCODE = 0, RM_HASH = 1, RM_MINIMIZER = 2, RM_COUNT = 3, RM_COUNT_MIN = 4, RM_TABLE = 5, RM_PWM = 6,
-       RM_PWM_MAX = 7 };
+       RM_PWM_MAX = 7, RM_MATCH = 8, RM_MATCH_COUNT = 9 };
 constexpr int kPwmMaxLen = kSegBytes / 2;     // motif columns: the segment overlap limit of check_common
 constexpr int kPwmMaxCells = 8192;            // alphabet_size * motif_len doubles: 64 KiB of shared memory
 constexpr int kPwmInFlight = 4;               // positions per lane summed side by side (each one a chain of DADDs)
+constexpr int kMatchMaxLen = kSegBytes / 2;   // columns of one sub-pattern: the segment overlap, as check_common
+constexpr int kMatchMaxSubs = 64;             // sub-patterns of one expanded pattern
+constexpr int kMatchMaxWords = 8192;          // symbol-set words of all columns: 32 KiB of shared memory
+
+// A pattern expanded into sub-patterns (one per combination of gap lengths), the match of a position being the OR of
+// theirs.  Column c of the concatenated sub-patterns is the symbol set sets[c * words_per_col ...]: bit s of the
+// words is set when code s (a byte, for raw bytes) matches there.
+struct MatchArgs {
+    const uint32_t *sets;
+    int n_sub, span, words_per_col, n_words, same;
+    int len[kMatchMaxSubs];
+};
+// The match modes' shared memory behind the LUT: [kMatchMaxSubs] lengths, [kMatchMaxSubs] first columns, then the sets.
+constexpr int kMatchSmemHead = 2 * kMatchMaxSubs * 4;
 
 struct RowArgs {
     const uint8_t *base;
@@ -97,15 +112,60 @@ __device__ __forceinline__ uint32_t pwm_segment(const uint32_t *w_codes, const d
     return produced;
 }
 
+// Whether each of 16 2-bit codes (code i at bits 2i, 2i+1 of y) is in the 4-letter set s (bit c = code c), as bit 2i of
+// the result: the set's truth table over the word's two bit planes.  Odd bits are don't-care.
+__device__ __forceinline__ uint32_t codes_in_set(uint32_t y, uint32_t s) {
+    const uint32_t lo = y, hi = y >> 1;
+    const uint32_t s0 = 0u - (s & 1u), s1 = 0u - ((s >> 1) & 1u), s2 = 0u - ((s >> 2) & 1u), s3 = 0u - (s >> 3);
+    return (~hi & ((~lo & s0) | (lo & s1))) | (hi & ((~lo & s2) | (lo & s3)));
+}
+
+// Matches at the positions of one staged segment that start in [0, npos), 16 starts per lane at a time: bit 2i of a
+// sub-pattern's word is start p0 + i, ANDed over the sub-pattern's columns (codes p0 + j .. p0 + j + 15 come from the
+// packed stream in one funnel shift) and ORed over the sub-patterns.  A start only counts for a sub-pattern that fits
+// before seg_len; '.' columns (all four codes) are skipped, and a sub-pattern whose 16 starts have all failed stops.
+// Writes out[p] = 0/1 (OUT) and adds the matches to `hits`.  Returns the positions this lane tested.  Warp-wide.
+template <bool OUT>
+__device__ __forceinline__ uint32_t match_segment(const uint32_t *w_codes, const int *s_match, int n_sub, int off,
+                                                  int seg_len, int npos, uint8_t *out, uint64_t &hits, int lane) {
+    const uint32_t *s_sets = reinterpret_cast<const uint32_t *>(s_match + 2 * kMatchMaxSubs);
+    uint32_t produced = 0;
+    for (int p0 = 16 * lane; p0 < npos; p0 += 16 * 32) {
+        const int nv = min(16, npos - p0);
+        uint32_t any = 0;
+        for (int k = 0; k < n_sub; ++k) {
+            const int m = s_match[k];
+            const int fit = min(nv, seg_len - m + 1 - p0);           // starts of the block where sub-pattern k fits
+            if (fit <= 0) continue;
+            uint32_t acc = 0x55555555u >> (32 - 2 * fit);
+            const uint32_t *set = s_sets + s_match[kMatchMaxSubs + k];
+            for (int j = 0; j < m && acc; ++j) {
+                const uint32_t s = set[j];
+                if (s == 0xFu) continue;
+                acc &= codes_in_set(stream_lo32(w_codes, (uint32_t)(off + p0 + j)), s);
+            }
+            any |= acc;
+        }
+        if constexpr (OUT)
+            for (int i = 0; i < nv; ++i) out[p0 + i] = (uint8_t)((any >> (2 * i)) & 1u);
+        hits += (uint64_t)__popc(any);
+        produced += (uint32_t)nv;
+    }
+    return produced;
+}
+
 template <int RM, int ENC, bool SMEM_HIST>
 __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_bad, const uint8_t *s_lut,
                          const HistTarget &ht, int64_t start, int64_t L, int64_t r, int64_t out_off, int lane,
-                         uint64_t &acc_values, uint64_t *acc_claims = nullptr, const double *s_pwm = nullptr) {
+                         uint64_t &acc_values, uint64_t *acc_claims = nullptr, const double *s_pwm = nullptr,
+                         const MatchArgs *ma = nullptr, const int *s_match = nullptr) {
     constexpr bool MINZ = (RM == RM_MINIMIZER || RM == RM_COUNT_MIN);
     constexpr bool PWM = (RM == RM_PWM || RM == RM_PWM_MAX);
+    constexpr bool MATCH = (RM == RM_MATCH || RM == RM_MATCH_COUNT);
     constexpr bool LUT_ENCODE = RM == RM_ENCODE && ENC == BNPK_ENC_LUT;   // writes the table values, finds its own bad bytes
-    const int span = (MINZ || PWM) ? a.window : (RM == RM_ENCODE ? 1 : a.k);
+    const int span = (MINZ || PWM || MATCH) ? a.window : (RM == RM_ENCODE ? 1 : a.k);
     double best = -INFINITY;                                              // RM_PWM_MAX: this lane's maximum
+    uint64_t hits = 0;                                                    // RM_MATCH_COUNT: this lane's matches
     const uint64_t kmask = (1ull << (2 * a.k)) - 1;
     int64_t seg_start = 0;
     bool reported = false;
@@ -207,6 +267,12 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_bad, c
             const int npos = (a.tail && seg_start + seg_len >= L) ? seg_len : seg_len - span + 1;
             acc_values += pwm_segment<RM == RM_PWM>(w_codes, s_pwm, off, seg_len, npos, span,
                                                     reinterpret_cast<double *>(a.out) + out_off + seg_start, best, lane);
+        } else if constexpr (MATCH) {
+            // "same": the row's last segment also tests its last span - 1 positions, with the sub-patterns that fit
+            const int npos = (ma->same && seg_start + seg_len >= L) ? seg_len : seg_len - span + 1;
+            acc_values += match_segment<RM == RM_MATCH>(w_codes, s_match, ma->n_sub, off, seg_len, npos,
+                                                        reinterpret_cast<uint8_t *>(a.out) + out_off + seg_start, hits,
+                                                        lane);
         } else {
             if (seg_len >= span)
                 acc_values += row_count<SMEM_HIST, MINZ>(w_codes, off, seg_len, a.k, a.window, ht, lane);
@@ -220,11 +286,15 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_bad, c
         for (int o = 16; o; o >>= 1) best = nan_max(best, __shfl_xor_sync(0xffffffffu, best, o));
         if (lane == 0) reinterpret_cast<double *>(a.out)[r] = best;
     }
+    if constexpr (RM == RM_MATCH_COUNT) {
+        hits = warp_sum_u64(hits);
+        if (lane == 0) reinterpret_cast<int64_t *>(a.out)[r] = (int64_t)hits;
+    }
 }
 
 // The body of the row kernels: one warp per row, the block's rows strided over the grid.
 template <int RM, int ENC, bool SMEM_HIST, bool DEFERRED>
-__device__ __forceinline__ void rows_body(const RowArgs &a) {
+__device__ __forceinline__ void rows_body(const RowArgs &a, const MatchArgs *ma = nullptr) {
     extern __shared__ __align__(16) uint32_t smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint32_t *w_codes = smem + warp * kWarpWords;
@@ -236,6 +306,18 @@ __device__ __forceinline__ void rows_body(const RowArgs &a) {
     constexpr bool PWM = (RM == RM_PWM || RM == RM_PWM_MAX);
     if constexpr (PWM)
         for (int i = tid; i < 4 * a.window; i += kRowThreads) s_pwm[i] = a.pwm[i];
+    constexpr bool MATCH = (RM == RM_MATCH || RM == RM_MATCH_COUNT);
+    int *s_match = reinterpret_cast<int *>(s_lut + 256);                   // match modes: kMatchSmemHead, then the sets
+    if constexpr (MATCH) {
+        if (tid == 0) {
+            int col = 0;
+#pragma unroll
+            for (int k = 0; k < kMatchMaxSubs; ++k)
+                if (k < ma->n_sub) { s_match[k] = ma->len[k]; s_match[kMatchMaxSubs + k] = col; col += ma->len[k]; }
+        }
+        uint32_t *s_sets = reinterpret_cast<uint32_t *>(s_match + 2 * kMatchMaxSubs);
+        for (int i = tid; i < ma->n_words; i += kRowThreads) s_sets[i] = ma->sets[i];
+    }
     constexpr bool COUNTING = (RM == RM_COUNT || RM == RM_COUNT_MIN);
     if (COUNTING && SMEM_HIST)
         for (uint32_t b = tid; b < a.n_bins; b += kRowThreads) s_hist[b] = 0;
@@ -276,11 +358,13 @@ __device__ __forceinline__ void rows_body(const RowArgs &a) {
         if (L <= 0) {
             if constexpr (RM == RM_PWM_MAX)
                 if (lane == 0) reinterpret_cast<double *>(a.out)[r] = -INFINITY;   // no window
+            if constexpr (RM == RM_MATCH_COUNT)
+                if (lane == 0) reinterpret_cast<int64_t *>(a.out)[r] = 0;
             continue;
         }
         if (lane == 0) acc_bases += (uint64_t)L;
         warp_row<RM, ENC, SMEM_HIST>(a, w_codes, w_bad, s_lut, ht, start, L, r, out_off, lane, acc_values, &acc_claims,
-                                     s_pwm);
+                                     s_pwm, ma, s_match);
     }
     if (COUNTING && SMEM_HIST) {
         __syncthreads();
@@ -316,6 +400,13 @@ rows_kernel(const RowArgs a) {
 template <int RM, int ENC>
 __global__ void __launch_bounds__(kRowThreads, 4) rows_pwm_kernel(const RowArgs a) {
     rows_body<RM, ENC, false, false>(a);
+}
+
+// The match modes (RM_MATCH, RM_MATCH_COUNT) of four-letter alphabets.  2 CTAs per SM (<= 128 registers): at 4, ptxas
+// keeps a 64-bit accumulator of the count on the stack.
+template <int RM, int ENC>
+__global__ void __launch_bounds__(kRowThreads, 2) rows_match_kernel(const RowArgs a, const __grid_constant__ MatchArgs m) {
+    rows_body<RM, ENC, false, false>(a, &m);
 }
 
 // Growth: one thread per slot of the old table re-inserts its (key, count) into the new one with the same slot function.
@@ -467,6 +558,83 @@ __global__ void __launch_bounds__(256) rows_pwm_generic_kernel(const uint8_t *ba
     }
 }
 
+// Matches for alphabets that are not four letters (amino acids, "ACGTN") and raw bytes (alphabet_size 256): the same
+// positions, sub-patterns and "same" tail as rows_match_kernel, with codes from a 256-byte LUT in shared memory
+// (255 = invalid; byte codes: c < A maps to itself; raw bytes: every byte is its own code) and the column sets behind
+// the sub-pattern table.  One warp per row, one lane per position; a sub-pattern stops at its first failed column.
+// Writes out[offsets[r] + i] = 0/1 (OUT) or out[r] = the row's matches (int64).
+template <bool OUT>
+__global__ void __launch_bounds__(256) rows_match_generic_kernel(const uint8_t *base, const int64_t *starts,
+                                                                 const int32_t *lens, size_t n_rows, const uint8_t *lut,
+                                                                 int alphabet_size, const __grid_constant__ MatchArgs m,
+                                                                 const int64_t *offsets, void *out, int64_t *status) {
+    extern __shared__ __align__(16) uint32_t smem[];
+    int *s_len = reinterpret_cast<int *>(smem);
+    int *s_col = s_len + kMatchMaxSubs;
+    uint32_t *s_sets = reinterpret_cast<uint32_t *>(s_col + kMatchMaxSubs);
+    uint8_t *s_lut = reinterpret_cast<uint8_t *>(s_sets + m.n_words);
+    const int tid = threadIdx.x, lane = tid & 31;
+    const uint32_t A = (uint32_t)alphabet_size, wpc = (uint32_t)m.words_per_col;
+    s_lut[tid] = lut ? lut[tid] : ((uint32_t)tid < A ? (uint8_t)tid : (uint8_t)255);
+    if (tid == 0) {
+        int col = 0;
+#pragma unroll
+        for (int k = 0; k < kMatchMaxSubs; ++k)
+            if (k < m.n_sub) { s_len[k] = m.len[k]; s_col[k] = col; col += m.len[k]; }
+    }
+    for (int i = tid; i < m.n_words; i += 256) s_sets[i] = m.sets[i];
+    __syncthreads();
+    uint64_t acc_values = 0, acc_bases = 0;
+    const size_t warp_global = ((size_t)blockIdx.x * blockDim.x + tid) >> 5;
+    const size_t n_warps = ((size_t)gridDim.x * blockDim.x) >> 5;
+    for (size_t r = warp_global; r < n_rows; r += n_warps) {
+        const uint8_t *row = base + starts[r];
+        const int64_t L = lens[r];
+        uint64_t hits = 0;
+        if (L > 0) {
+            if (lane == 0) acc_bases += (uint64_t)L;
+            if (A < 256) {                                  // every byte is validated, as the reference encodes it all
+                int64_t first_bad = INT64_MAX;
+                for (int64_t i = lane; i < L; i += 32)
+                    if (s_lut[row[i]] >= A) { first_bad = i; break; }
+#pragma unroll
+                for (int o = 16; o; o >>= 1) first_bad = min(first_bad, __shfl_xor_sync(0xffffffffu, first_bad, o));
+                if (lane == 0 && first_bad != INT64_MAX)
+                    atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)(((int64_t)r << 32) | first_bad));
+            }
+            const int64_t npos = m.same ? L : L - m.span + 1;
+            uint8_t *o_row = OUT ? reinterpret_cast<uint8_t *>(out) + offsets[r] : nullptr;
+            for (int64_t i = lane; i < npos; i += 32) {
+                bool hit = false;
+                for (int k = 0; k < m.n_sub && !hit; ++k) {
+                    const int mk = s_len[k];
+                    if (i + mk > L) continue;
+                    const uint32_t *set = s_sets + (size_t)s_col[k] * wpc;
+                    bool ok = true;
+                    for (int j = 0; j < mk && ok; ++j) {
+                        const uint32_t c = s_lut[row[i + j]];
+                        ok = c < A && ((set[j * wpc + (c >> 5)] >> (c & 31u)) & 1u);
+                    }
+                    hit = ok;
+                }
+                if constexpr (OUT) o_row[i] = (uint8_t)hit;
+                hits += hit;
+                ++acc_values;
+            }
+        }
+        if constexpr (!OUT) {
+            hits = warp_sum_u64(hits);
+            if (lane == 0) reinterpret_cast<int64_t *>(out)[r] = (int64_t)hits;
+        }
+    }
+    acc_values = warp_sum_u64(acc_values);
+    acc_bases = warp_sum_u64(acc_bases);
+    if (lane == 0) {
+        if (acc_values) atomicAdd((unsigned long long *)&status[BNPK_ST_N_VALUES], acc_values);
+        if (acc_bases) atomicAdd((unsigned long long *)&status[BNPK_ST_N_BASES], acc_bases);
+    }
+}
+
 // get_reverse_complement (sequence/dna.py:36-65): out row r = lut[row r read backwards]; one warp per row,
 // coalesced writes.  The 256-byte lut is the reference's complement Lookup for the array's encoding.
 __global__ void __launch_bounds__(256) rows_reverse_complement_kernel(const uint8_t *base, const int64_t *starts, const int32_t *lens,
@@ -599,6 +767,72 @@ static int launch_pwm(const uint8_t *base, size_t base_bytes, const int64_t *sta
     kern<<<grid, 256, smem, st>>>(base, starts, lens, n_rows, enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size,
                                   matrix, motif_len, tail, offsets, out, status);
     BNPK_LAUNCHED("rows_pwm_generic_kernel");
+    return 0;
+}
+
+// The limits of bnpk_rows_match*, and the kernels' view of the pattern in `m`.
+static int check_match(int enc_mode, const uint8_t *lut256, int alphabet_size, const uint32_t *sets,
+                       const int32_t *sub_lens, int n_sub, int same, MatchArgs &m) {
+    if (enc_mode < 0 || enc_mode > 3) return set_err(BNPK_E_BADARG, "bad enc_mode");
+    if (alphabet_size < 2 || alphabet_size > 256) return set_err(BNPK_E_BADARG, "alphabet_size must be in 2..256");
+    if (alphabet_size != 4 && enc_mode != BNPK_ENC_LUT && enc_mode != BNPK_ENC_CODES)
+        return set_err(BNPK_E_BADARG, "alphabets that are not four letters take BNPK_ENC_LUT or BNPK_ENC_CODES");
+    if (alphabet_size == 256 && enc_mode != BNPK_ENC_CODES)
+        return set_err(BNPK_E_BADARG, "raw bytes (alphabet_size 256) take BNPK_ENC_CODES");
+    if (enc_mode == BNPK_ENC_LUT && !lut256) return set_err(BNPK_E_BADARG, "lut256 required");
+    if (!sets || !sub_lens) return set_err(BNPK_E_BADARG, "sets and sub_lens required");
+    if (n_sub < 1 || n_sub > kMatchMaxSubs) return set_err(BNPK_E_BADARG, "n_sub must be in 1..64");
+    if (same != 0 && same != 1) return set_err(BNPK_E_BADARG, "same must be 0 or 1");
+    m = MatchArgs{};
+    m.sets = sets; m.n_sub = n_sub; m.same = same; m.words_per_col = (alphabet_size + 31) / 32;
+    int cols = 0;
+    for (int k = 0; k < n_sub; ++k) {
+        if (sub_lens[k] < 1 || sub_lens[k] > kMatchMaxLen) return set_err(BNPK_E_BADARG, "sub-pattern lengths must be in 1..1024");
+        m.len[k] = sub_lens[k];
+        m.span = std::max(m.span, (int)sub_lens[k]);
+        cols += sub_lens[k];
+    }
+    if ((int64_t)cols * m.words_per_col > kMatchMaxWords)
+        return set_err(BNPK_E_BADARG, "symbol sets above 8192 words (columns * ceil(alphabet_size / 32))");
+    m.n_words = cols * m.words_per_col;
+    return 0;
+}
+
+// Four-letter alphabets take rows_match_kernel (2-bit codes, every enc_mode); the others and raw bytes the LUT kernel.
+template <bool OUT>
+static int launch_match(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                        size_t n_rows, int enc_mode, const uint8_t *lut256, int alphabet_size, const MatchArgs &m,
+                        const int64_t *offsets, void *out, int64_t *status, cudaStream_t st) {
+    constexpr int RM = OUT ? RM_MATCH : RM_MATCH_COUNT;
+    if (alphabet_size == 4) {
+        RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
+        a.k = 1; a.window = m.span; a.offsets = offsets; a.out = out; a.status = status;
+        void (*kern)(const RowArgs, const MatchArgs);
+        switch (enc_mode) {
+            case BNPK_ENC_ASCII_ACGT: kern = rows_match_kernel<RM, BNPK_ENC_ASCII_ACGT>; break;
+            case BNPK_ENC_ASCII_ACTG: kern = rows_match_kernel<RM, BNPK_ENC_ASCII_ACTG>; break;
+            case BNPK_ENC_CODES: kern = rows_match_kernel<RM, BNPK_ENC_CODES>; break;
+            default: kern = rows_match_kernel<RM, BNPK_ENC_LUT>; break;
+        }
+        const size_t smem = rows_smem_bytes(false, false, 0) + kMatchSmemHead + (size_t)m.n_words * 4;
+        BNPK_DYN_SMEM(kern, rows_smem_bytes(false, false, 0) + kMatchSmemHead + kMatchMaxWords * 4);
+        int per_sm = 1;
+        BNPK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kRowThreads, smem));
+        if (per_sm < 1) return set_err(BNPK_E_BINS, "rows kernel does not fit shared memory");
+        const size_t want = (n_rows + kRowWarps - 1) / kRowWarps;
+        const unsigned grid = (unsigned)std::max<size_t>(1, std::min(want, (size_t)sm_count() * per_sm));
+        kern<<<grid, kRowThreads, smem, st>>>(a, m);
+        BNPK_LAUNCHED("rows_match_kernel");
+        return 0;
+    }
+    auto kern = rows_match_generic_kernel<OUT>;
+    const size_t smem = kMatchSmemHead + (size_t)m.n_words * 4 + 256;
+    BNPK_DYN_SMEM(kern, kMatchSmemHead + kMatchMaxWords * 4 + 256);
+    const size_t want = (n_rows + 7) / 8;
+    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 8));
+    kern<<<grid, 256, smem, st>>>(base, starts, lens, n_rows, enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size,
+                                  m, offsets, out, status);
+    BNPK_LAUNCHED("rows_match_generic_kernel");
     return 0;
 }
 
@@ -764,6 +998,28 @@ int bnpk_rows_pwm_max(const uint8_t *base, size_t base_bytes, const int64_t *sta
     if (n_rows == 0) return 0;
     return launch_pwm<false>(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, alphabet_size, matrix, motif_len,
                              0, nullptr, max_out, status, (cudaStream_t)stream);
+}
+
+int bnpk_rows_match(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
+                    int enc_mode, const uint8_t *lut256, int alphabet_size, const uint32_t *sets,
+                    const int32_t *sub_lens, int n_sub, int same, const int64_t *offsets, uint8_t *match_out,
+                    int64_t *status, void *stream) {
+    MatchArgs m;
+    if (int rc = check_match(enc_mode, lut256, alphabet_size, sets, sub_lens, n_sub, same, m)) return rc;
+    if (n_rows == 0) return 0;
+    return launch_match<true>(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, alphabet_size, m, offsets,
+                              match_out, status, (cudaStream_t)stream);
+}
+
+int bnpk_rows_match_count(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                          size_t n_rows, int enc_mode, const uint8_t *lut256, int alphabet_size, const uint32_t *sets,
+                          const int32_t *sub_lens, int n_sub, int same, int64_t *count_out, int64_t *status,
+                          void *stream) {
+    MatchArgs m;
+    if (int rc = check_match(enc_mode, lut256, alphabet_size, sets, sub_lens, n_sub, same, m)) return rc;
+    if (n_rows == 0) return 0;
+    return launch_match<false>(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, alphabet_size, m, nullptr,
+                               count_out, status, (cudaStream_t)stream);
 }
 
 }  // extern "C"

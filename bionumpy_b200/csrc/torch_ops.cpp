@@ -209,6 +209,25 @@ std::tuple<Tensor, Tensor> rows_pwm_scores(const Tensor &base, const Tensor &sta
     return {out, status};
 }
 
+// K8: matches uint8[total] (1 = some sub-pattern matches there) of the column sets `sets` (int32 words, on the device)
+std::tuple<Tensor, Tensor> rows_match(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t enc_mode,
+                                      const c10::optional<Tensor> &lut, int64_t alphabet_size, const Tensor &sets,
+                                      c10::IntArrayRef sub_lens, bool same, const Tensor &offsets, int64_t total) {
+    need_rows(base, starts, lens);
+    need(sets, torch::kInt32, "sets");
+    std::vector<int32_t> sl(sub_lens.begin(), sub_lens.end());
+    c10::cuda::CUDAGuard guard(base.device());
+    Tensor out = torch::empty({total}, base.options().dtype(torch::kUInt8));
+    Tensor status = new_status(base);
+    check(bnpk_rows_match(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
+                          lens.data_ptr<int32_t>(), (size_t)lens.numel(), (int)enc_mode, lut ? u8(*lut) : nullptr,
+                          (int)alphabet_size, reinterpret_cast<const uint32_t *>(sets.data_ptr<int32_t>()), sl.data(),
+                          (int)sl.size(), same, offsets.data_ptr<int64_t>(), out.data_ptr<uint8_t>(),
+                          status.data_ptr<int64_t>(), cur_stream(base)),
+          "rows_match");
+    return {out, status};
+}
+
 // K5 (accumulates into hist)
 Tensor bincount(const Tensor &values, Tensor hist, int64_t hist_mode) {
     need(values, torch::kInt64, "values");
@@ -241,6 +260,8 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("rows_reverse_complement(Tensor base, Tensor starts, Tensor lens, Tensor lut, Tensor offsets, int total) -> Tensor");
     m.def("rows_pwm_scores(Tensor base, Tensor starts, Tensor lens, int enc_mode, Tensor? lut, Tensor matrix, bool tail, "
           "Tensor offsets, int total) -> (Tensor, Tensor)");
+    m.def("rows_match(Tensor base, Tensor starts, Tensor lens, int enc_mode, Tensor? lut, int alphabet_size, Tensor sets, "
+          "int[] sub_lens, bool same, Tensor offsets, int total) -> (Tensor, Tensor)");
     m.def("bincount(Tensor values, Tensor(a!) hist, int hist_mode=0) -> Tensor");
 }
 
@@ -254,5 +275,6 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("rows_kmer_table_insert", &rows_kmer_table_insert);
     m.impl("rows_reverse_complement", &rows_reverse_complement);
     m.impl("rows_pwm_scores", &rows_pwm_scores);
+    m.impl("rows_match", &rows_match);
     m.impl("bincount", &bincount);
 }

@@ -1,6 +1,8 @@
 """Record containers for the chunk objects the readers yield: the field names of
 bionumpy/datatypes/__init__.py:39-47 (SequenceEntry: name, sequence; SequenceEntryWithQuality:
 + quality), materialised lazily from the file buffer (bnpdataclass/lazybnpdataclass.py:117-125)."""
+import numpy as np
+import torch
 
 
 class _Entries:
@@ -20,6 +22,15 @@ class _Entries:
         if name not in self._values:
             self._values[name] = self._buffer.get_field_by_number(self._fields.index(name))
         return self._values[name]
+
+    def __getitem__(self, idx):
+        """The selected entries (a bool mask, an index tensor/array/list or a slice): each field a view of the same
+        bytes with the selected rows, no copy (``reads[np.sum(match_string(reads.sequence, "ACT"), axis=1) > 0]``)."""
+        if isinstance(idx, (int, np.integer)):
+            raise TypeError("select entries with a mask, an index array or a slice")
+        if isinstance(idx, (list, np.ndarray)):
+            idx = torch.as_tensor(np.asarray(idx))
+        return self.__class__(*[getattr(self, f)[idx] for f in self._fields])
 
     def __len__(self):
         if self._buffer is not None:

@@ -309,6 +309,45 @@ def rows_pwm_max(base, starts, lens, enc_mode, matrix, lut=None, status=None):
     return out, status
 
 
+def _match_args(alphabet_size, sets, sub_lens, lut):
+    """sets: int32 (uint32 words) on the device; sub_lens: a host sequence of ints."""
+    _need_cuda(sets, "sets")
+    if sets.dtype != torch.int32:
+        raise TypeError("sets must be int32 words")
+    if lut is not None:
+        _need_cuda(lut, "lut")
+    lens = (ctypes.c_int32 * len(sub_lens))(*[int(x) for x in sub_lens])
+    return ptr(lut), alphabet_size, ptr(sets), ctypes.cast(lens, ctypes.c_void_p), len(sub_lens)
+
+
+@_on_device
+def rows_match(base, starts, lens, enc_mode, alphabet_size, sets, sub_lens, same=False, lut=None, offsets=None,
+               status=None, total=None, out=None):
+    """K8: 1 where some sub-pattern matches at a position and fits in its row, else 0 (uint8): the windows of the
+    longest sub-pattern, or every position with ``same``.  ``out`` (uint8[total]) is written in place when given.
+    Returns (matches, offsets, status)."""
+    span = max(int(x) for x in sub_lens) if len(sub_lens) else 1
+    if out is None:
+        out, offsets = _ragged_out(lens, 0 if same else span - 1, offsets, total, torch.uint8)
+    if status is None:
+        status = nv.new_status(base.device)
+    check(lib().bnpk_rows_match(*_rows_args(base, starts, lens), enc_mode, *_match_args(alphabet_size, sets, sub_lens, lut),
+                                int(same), ptr(offsets), ptr(out), ptr(status), stream_ptr()))
+    return out, offsets, status
+
+
+@_on_device
+def rows_match_count(base, starts, lens, enc_mode, alphabet_size, sets, sub_lens, same=False, lut=None, status=None):
+    """K8 fused with the row sum: int64[R] matches per row; the matches are never written.  Returns (counts, status)."""
+    out = torch.empty(lens.numel(), dtype=torch.int64, device=base.device)
+    if status is None:
+        status = nv.new_status(base.device)
+    check(lib().bnpk_rows_match_count(*_rows_args(base, starts, lens), enc_mode,
+                                      *_match_args(alphabet_size, sets, sub_lens, lut), int(same), ptr(out),
+                                      ptr(status), stream_ptr()))
+    return out, status
+
+
 @_on_device
 def bincount(values, n_bins, hist=None, hist_mode=nv.HIST_AUTO, status=None):
     _need_cuda(values, "values")

@@ -29,6 +29,12 @@ def segment_max(values, rows, n_rows):
     return out
 
 
+def segment_sum(values, rows, n_rows):
+    """out[r] = the sum of values[i] with rows[i] == r, int64."""
+    out = torch.zeros(n_rows, dtype=torch.int64, device=values.device)
+    return out.index_add_(0, rows, values.to(torch.int64))
+
+
 class RaggedShape:
     """(starts, lens) of the rows.  Compared by lengths only, like npstructures.RaggedShape."""
 
@@ -248,6 +254,28 @@ class RaggedArray:
             rows = torch.repeat_interleave(torch.arange(len(self), device=flat.device), lens64)
             out = torch.zeros(len(self), dtype=torch.int64, device=flat.device)
             return out.index_add_(0, rows, flat.to(torch.int64))
+        raise NotImplementedError(axis)
+
+    def _row_index(self):
+        return torch.repeat_interleave(torch.arange(len(self), device=self._data.device), self._lens.to(torch.int64))
+
+    def any(self, axis=None, **kwargs):
+        """np.any: axis=-1 gives one bool per row, False for an empty row."""
+        flat = self.ravel()
+        if axis is None:
+            return (flat != 0).any()
+        if axis in (-1, 1):
+            return segment_sum(flat != 0, self._row_index(), len(self)) > 0
+        raise NotImplementedError(axis)
+
+    def mean(self, axis=None, **kwargs):
+        """np.mean in float64: axis=-1 gives one value per row, NaN for an empty row."""
+        flat = self.ravel().to(torch.float64)
+        if axis is None:
+            return flat.mean()
+        if axis in (-1, 1):
+            out = torch.zeros(len(self), dtype=torch.float64, device=flat.device)
+            return out.index_add_(0, self._row_index(), flat) / self._lens.to(torch.float64)
         raise NotImplementedError(axis)
 
     def __array__(self, dtype=None, copy=None):

@@ -6,3 +6,4 @@ from .dna import complement, get_reverse_complement
 from .indexing import KmerIndex, KmerLookup
 from .bloom_filter import BloomFilter
 from .position_weight_matrix import get_motif_scores, PWM
+from .string_matcher import match_string, StringMatcher, FixedLenRegexMatcher, RegexMatcher

@@ -256,6 +256,31 @@ int bnpk_rows_pwm_max(const uint8_t *base, size_t base_bytes, const int64_t *sta
                       size_t n_rows, int enc_mode, const uint8_t *lut256, int alphabet_size,
                       const double *matrix, int motif_len, double *max_out, int64_t *status, void *stream);
 
+/* K8  string and pattern matches: match_string, StringMatcher, FixedLenRegexMatcher, RegexMatcher
+ *     (sequence/string_matcher.py).  A pattern is n_sub sub-patterns (one per combination of gap lengths; 1..64) of
+ *     sub_lens[k] columns each (host int32; 1..1024).  Their columns, concatenated in order, are symbol sets in
+ *     `sets` (device): column c is the words sets[c * W .. c * W + W - 1], W = ceil(alphabet_size / 32), and code s
+ *     matches there iff bit s % 32 of word s / 32 is set.  match_out[offsets[r] + p] = 1 iff some sub-pattern matches
+ *     at position p of row r and fits inside the row, else 0.  same = 0: the positions of the longest sub-pattern's
+ *     windows, max(L - span + 1, 0) per row (span = the longest sub-pattern; offsets from shrink = span - 1);
+ *     same = 1: every position, L per row (shrink = 0).
+ *     Text is read as by the other row entry points (enc_mode, lut256); an alphabet_size that is not 4 takes
+ *     BNPK_ENC_LUT (lut256: byte -> code, 255 = invalid) or BNPK_ENC_CODES (bytes are codes, valid below
+ *     alphabet_size), and alphabet_size 256 means raw bytes: BNPK_ENC_CODES, every byte valid and its own code.
+ *     A byte outside the alphabet anywhere in a row is reported in status[BNPK_ST_BAD_BASE]; N_BASES += row lengths,
+ *     N_VALUES += positions tested.  BNPK_E_BADARG unless 2 <= alphabet_size <= 256, the sub-pattern limits above
+ *     hold and the sets fit 8192 words (32 KiB of shared memory: total columns * W <= 8192). */
+int bnpk_rows_match(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
+                    int enc_mode, const uint8_t *lut256, int alphabet_size, const uint32_t *sets,
+                    const int32_t *sub_lens, int n_sub, int same, const int64_t *offsets, uint8_t *match_out,
+                    int64_t *status, void *stream);
+/*     The matches of every row counted without writing them: count_out[r] (int64) = the number of ones row r's
+ *     match_out would hold.  Same arguments and status. */
+int bnpk_rows_match_count(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                          size_t n_rows, int enc_mode, const uint8_t *lut256, int alphabet_size, const uint32_t *sets,
+                          const int32_t *sub_lens, int n_sub, int same, int64_t *count_out, int64_t *status,
+                          void *stream);
+
 /* K5  np.bincount(values % n_bins, minlength=n_bins) accumulated into hist
  *     (sequence/count_encoded.py:173-177; EncodedArray.__array_function__ encoded_array.py:459-460).
  *     Values must be non-negative; n_bins = len(alphabet) reproduces count_encoded exactly
