@@ -279,13 +279,20 @@ __global__ void __launch_bounds__(256) fasta_gather_kernel(const uint8_t *file, 
 
 // ------------------------------------------------------------------------------------------
 // Bloom filter over k-mer hashes (sequence/bloom_filter.py:15-42): bit j of the filter is the byte mask[j];
-// hash function i is v ^ offsets[i], reduced mod the mask size.
+// hash function i is v ^ offsets[i], reduced mod the mask size as NumPy's int64 `%` does (a floor modulo: a negative
+// v ^ offsets[i] lands in [0, mask_size) like a positive one, on the slot NumPy picks).
 // ------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint64_t bloom_slot(int64_t x, uint64_t mask_size) {
+    const int64_t m = (int64_t)mask_size;
+    int64_t r = x % m;
+    if (r < 0) r += m;
+    return (uint64_t)r;
+}
 __global__ void __launch_bounds__(256) bloom_insert_kernel(const int64_t *values, size_t n, const int64_t *offsets, int n_hash,
                                                            uint8_t *mask, uint64_t mask_size) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const int64_t v = values[i];
-        for (int h = 0; h < n_hash; ++h) mask[(uint64_t)(v ^ offsets[h]) % mask_size] = 1;
+        for (int h = 0; h < n_hash; ++h) mask[bloom_slot(v ^ offsets[h], mask_size)] = 1;
     }
 }
 __global__ void __launch_bounds__(256) bloom_query_kernel(const int64_t *values, size_t n, const int64_t *offsets, int n_hash,
@@ -293,7 +300,7 @@ __global__ void __launch_bounds__(256) bloom_query_kernel(const int64_t *values,
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const int64_t v = values[i];
         uint8_t all = 1;
-        for (int h = 0; h < n_hash; ++h) all &= mask[(uint64_t)(v ^ offsets[h]) % mask_size];
+        for (int h = 0; h < n_hash; ++h) all &= mask[bloom_slot(v ^ offsets[h], mask_size)];
         out[i] = all;
     }
 }

@@ -340,24 +340,40 @@ def _normalise(name):
     return name.replace("(int)", "").replace("(bool)1", "true").replace("(bool)0", "false")
 
 
+PROFILE_ATTEMPTS = 5
+
+
 @gpu
 def test_each_case_reaches_its_kernel():
-    """Pins the route table: a change to the eligibility tests must not silently move a case to another kernel."""
+    """Pins the route table: a change to the eligibility tests must not silently move a case to another kernel.
+
+    Late in a long test process the CUDA profiler can lose the records of a session's first kernels (the fills, the
+    status init and the count kernel) while it keeps the later ones of the same call (the deferred-row and finalize
+    kernels).  A call's route is fixed by the call alone, so a session that lacks a kernel of the route is repeated, up
+    to PROFILE_ATTEMPTS sessions per case.  Every session must show no count kernel outside the route, and one of them
+    must show every kernel of the route."""
     from torch.profiler import profile, ProfilerActivity
     inp = get_input("ragged")
     src = device_input("ragged")
+    any_kernel = False
     for route_name, route in ROUTES.items():
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            count_sliced(src, schedule("one_shot", src.numel()), route, inp)
-            torch.cuda.synchronize()
-        names = {_normalise(e.key) for e in prof.key_averages()}
-        if not any("bnpk::" in n for n in names):
-            pytest.skip("the profiler recorded no CUDA kernels")
-        launched = {c for c in COUNT_KERNELS if any(c in n for n in names)}
-        for kern in route.kernels:
-            assert any(kern in n for n in names), (route_name, kern, sorted(names))
         want = {c for c in COUNT_KERNELS if any(c in kern for kern in route.kernels)}
-        assert launched == want, (route_name, sorted(names))
+        sessions = []
+        for _ in range(PROFILE_ATTEMPTS):
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                count_sliced(src, schedule("one_shot", src.numel()), route, inp)
+                torch.cuda.synchronize()
+            names = {_normalise(e.key) for e in prof.key_averages()}
+            any_kernel |= any("bnpk::" in n for n in names)
+            launched = {c for c in COUNT_KERNELS if any(c in n for n in names)}
+            assert launched <= want, (route_name, sorted(names))
+            sessions.append(sorted(names))
+            if all(any(kern in n for n in names) for kern in route.kernels):
+                break
+        else:
+            if not any_kernel:
+                pytest.skip("the profiler recorded no CUDA kernels")
+            raise AssertionError((route_name, route.kernels, sessions))
 
 
 # ---- the host pipeline --------------------------------------------------------------------------------------------------
