@@ -86,6 +86,20 @@ __device__ __forceinline__ uint4 lds128(const uint8_t *p) { return *reinterpret_
 __device__ __forceinline__ void hist_inc(uint32_t addr) { asm volatile("red.shared.add.u32 [%0], 1;" ::"r"(addr) : "memory"); }
 // ptxas never predicates ATOMS (it branches around it), so a masked count adds 0 or 1 instead
 __device__ __forceinline__ void hist_add_val(uint32_t addr, uint32_t val) { asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(addr), "r"(val) : "memory"); }
+// The 16 k-mers of one block of a lane's row into the CTA-private table (table bins a power of two).  K-mer t is the
+// field at bit 2t of (cur, nxt), the row's 2-bit codes from the block's first base on; shifted two bits less,
+// (window & mask) is its byte offset.  FULL (the block is full in every row of the warp): the offset is
+// (window & mask) | dummy, one LOP3 -- mask 0 and dummy = the spare word behind the table for a lane without a row.
+// Otherwise k-mers t >= left (left = the lane's k-mers that start in this block) count into the spare word `dummy`:
+// a select per k-mer, no branch.
+template <bool FULL>
+__device__ __forceinline__ void count_block16(uint32_t hist_sa, uint32_t cur, uint32_t nxt, uint32_t mask, uint32_t dummy, int left) {
+#pragma unroll
+    for (int t = 0; t < 16; ++t) {
+        const uint32_t win = t == 0 ? cur << 2 : __funnelshift_r(cur, nxt, 2 * t - 2);
+        hist_inc(hist_sa + (FULL ? (win & mask) | dummy : t < left ? win & mask : dummy));
+    }
+}
 
 // ---- the sorted newline list of a tile (emit_positions: every tile kernel; ScanLane: the kernels that stage tiles in
 // shared-memory slots) ---------------------------------------------------------------------------------------------
