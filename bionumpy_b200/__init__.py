@@ -24,7 +24,9 @@ from .sequence import KmerIndex, KmerLookup, BloomFilter
 from .sequence import count_kmers_exact, KmerCounter, KmerCounts
 from .io.buffers import CudaFastQBuffer, CudaTwoLineFastaBuffer, FastQBuffer, TwoLineFastaBuffer
 from .io.multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
-from .datatypes import SequenceEntry, SequenceEntryWithQuality
+from .datatypes import SequenceEntry, SequenceEntryWithQuality, replace
+from .io.files import count_entries
+from .io.write import NpBufferedWriter
 
 open = bnp_open
 

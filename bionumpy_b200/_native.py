@@ -20,6 +20,7 @@ E_BADARG, E_K, E_WINDOW, E_WORKSPACE, E_BINS = -1, -2, -3, -4, -5
  ST_N_BASES, ST_N_VALUES, ST_N_LONG_ROWS, ST_CR, ST_LAST_ROW_START, ST_LAST_ROW_INDEX, ST_OVERFLOW,
  ST_TABLE_FULL) = range(14)
 ST_WORDS = 16
+FMT_FASTQ, FMT_FASTA, FMT_FASTA_WRAPPED = 0, 1, 2
 INT64_MAX = (1 << 63) - 1
 SMEM_MAX_BINS = 32768
 
@@ -68,7 +69,14 @@ SIGNATURES = {
     "bnpk_bloom_insert": (_i, [_vp, _sz, _vp, _i, _vp, _sz, _vp]),
     "bnpk_bloom_query": (_i, [_vp, _sz, _vp, _i, _vp, _sz, _vp, _vp]),
     "bnpk_synth_fastq": (_i, [_vp, _u64, _u64, _u64, _vp]),
+    "bnpk_format_offsets": (_i, [_i, _i, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "bnpk_format_records": (_i, [_i, _i, _sz, _vp, _vp, _i64, _i64, _vp, _vp]),
 }
+
+
+class Field(ctypes.Structure):
+    """bnpk_field: a ragged view (base, starts, lens) and an optional device LUT applied on the way out."""
+    _fields_ = [("base", _vp), ("base_bytes", _sz), ("starts", _vp), ("lens", _vp), ("lut256", _vp)]
 
 
 class NativeLibraryError(RuntimeError):

@@ -240,6 +240,51 @@ Tensor bincount(const Tensor &values, Tensor hist, int64_t hist_mode) {
     return status;
 }
 
+// Writers: fields = [name base, starts, lens, sequence base, starts, lens(, quality base, starts, lens)], luts = one
+// optional 256-byte table per field.  format_offsets returns (offsets int64[E+1], status); format_records writes bytes
+// [out_begin, out_end) of the text (the caller reads offsets[-1] for the total: no sync here).
+std::vector<bnpk_field> make_fields(const std::vector<Tensor> &fields, const std::vector<c10::optional<Tensor>> &luts) {
+    TORCH_CHECK(fields.size() == 6 || fields.size() == 9, "bnpk: fields are (base, starts, lens) of 2 or 3 fields");
+    TORCH_CHECK(luts.size() * 3 == fields.size(), "bnpk: one lut (or None) per field");
+    std::vector<bnpk_field> out(3, bnpk_field{nullptr, 0, nullptr, nullptr, nullptr});
+    for (size_t f = 0; f < luts.size(); ++f) {
+        need_rows(fields[3 * f], fields[3 * f + 1], fields[3 * f + 2]);
+        TORCH_CHECK(fields[3 * f + 2].numel() == fields[2].numel(), "bnpk: fields differ in entry count");
+        out[f] = bnpk_field{u8(fields[3 * f]), (size_t)fields[3 * f].numel(), fields[3 * f + 1].data_ptr<int64_t>(),
+                            fields[3 * f + 2].data_ptr<int32_t>(), luts[f] ? u8(*luts[f]) : nullptr};
+    }
+    return out;
+}
+
+std::tuple<Tensor, Tensor> format_offsets(int64_t format, int64_t line_width, const std::vector<Tensor> &fields,
+                                          const std::vector<c10::optional<Tensor>> &luts) {
+    std::vector<bnpk_field> f = make_fields(fields, luts);
+    c10::cuda::CUDAGuard guard(fields[0].device());
+    const int64_t n = fields[2].numel();
+    Tensor offsets = torch::empty({n + 1}, fields[0].options().dtype(torch::kInt64));
+    Tensor status = new_status(fields[0]);
+    Tensor ws = new_workspace(fields[0], (size_t)std::max<int64_t>(n, 1));
+    check(bnpk_format_offsets((int)format, (int)line_width, (size_t)n, f.data(), offsets.data_ptr<int64_t>(),
+                              status.data_ptr<int64_t>(), ws.data_ptr<uint8_t>(), (size_t)ws.numel(), cur_stream(fields[0])),
+          "format_offsets");
+    return {offsets, status};
+}
+
+Tensor format_records(int64_t format, int64_t line_width, const std::vector<Tensor> &fields,
+                      const std::vector<c10::optional<Tensor>> &luts, const Tensor &offsets, int64_t out_begin,
+                      int64_t out_end) {
+    std::vector<bnpk_field> f = make_fields(fields, luts);
+    need(offsets, torch::kInt64, "offsets");
+    TORCH_CHECK(out_end >= out_begin, "bnpk: out_end < out_begin");
+    c10::cuda::CUDAGuard guard(fields[0].device());
+    Tensor out = torch::empty({out_end - out_begin}, fields[0].options().dtype(torch::kUInt8));
+    check(bnpk_format_records((int)format, (int)line_width, (size_t)fields[2].numel(), f.data(),
+                              offsets.data_ptr<int64_t>(), out_begin, out_end, out.numel() ? out.data_ptr<uint8_t>() : nullptr,
+                              cur_stream(fields[0])),
+          "format_records");
+    return out;
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bnpk, m) {
@@ -263,6 +308,9 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("rows_match(Tensor base, Tensor starts, Tensor lens, int enc_mode, Tensor? lut, int alphabet_size, Tensor sets, "
           "int[] sub_lens, bool same, Tensor offsets, int total) -> (Tensor, Tensor)");
     m.def("bincount(Tensor values, Tensor(a!) hist, int hist_mode=0) -> Tensor");
+    m.def("format_offsets(int format, int line_width, Tensor[] fields, Tensor?[] luts) -> (Tensor, Tensor)");
+    m.def("format_records(int format, int line_width, Tensor[] fields, Tensor?[] luts, Tensor offsets, int out_begin, "
+          "int out_end) -> Tensor");
 }
 
 TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
@@ -277,4 +325,6 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("rows_pwm_scores", &rows_pwm_scores);
     m.impl("rows_match", &rows_match);
     m.impl("bincount", &bincount);
+    m.impl("format_offsets", &format_offsets);
+    m.impl("format_records", &format_records);
 }

@@ -5,12 +5,27 @@ import numpy as np
 import torch
 
 
+def _from_strings(field, value):
+    """Lists of Python strings, as the reference's dataclasses take them: names and sequences become text
+    (as_encoded_array), quality strings byte - 33 (QualityEncoding, encodings/__init__.py:26)."""
+    if not isinstance(value, list) or not all(isinstance(v, str) for v in value):
+        return value
+    if field == "quality":
+        from .ragged import RaggedArray
+        from . import config
+        flat = np.frombuffer("".join(value).encode("ascii"), dtype=np.uint8) - np.uint8(33)
+        data = torch.from_numpy(flat.copy()).to(config.default_device())
+        return RaggedArray(data, [len(v) for v in value])
+    from .encoded_array import as_encoded_array
+    return as_encoded_array(value)
+
+
 class _Entries:
     _fields = ()
 
     def __init__(self, *values, buffer=None):
         self._buffer = buffer
-        self._values = dict(zip(self._fields, values))
+        self._values = {f: _from_strings(f, v) for f, v in zip(self._fields, values)}
 
     @classmethod
     def lazy(cls, buffer):
@@ -41,6 +56,15 @@ class _Entries:
 
     def __repr__(self):
         return f"{self.__class__.__name__} with {len(self)} entries"
+
+
+def replace(entries, **fields):
+    """dataclasses.replace for record chunks (bnpdataclass.py): the same record class, the named fields replaced and the
+    others carried over."""
+    unknown = set(fields) - set(entries._fields)
+    if unknown:
+        raise TypeError(f"{type(entries).__name__} has no field(s) {sorted(unknown)}")
+    return type(entries)(*[fields[f] if f in fields else getattr(entries, f) for f in entries._fields])
 
 
 class SequenceEntry(_Entries):

@@ -124,6 +124,24 @@ class CudaOneLineBuffer:
     def get_data(self):
         return self.dataclass.lazy(self)
 
+    # ---- writing (OneLineBuffer.from_data / join_fields, io/one_line_buffer.py:100-134) ----------------------------
+    _write_format_id = nv.FMT_FASTA
+
+    @classmethod
+    def _write_format(cls):
+        return cls._write_format_id, 1
+
+    @classmethod
+    def from_data(cls, entries):
+        """The records as this format's text: a device EncodedArray (csrc/write_kernels.cu)."""
+        from .write import format_entries
+        return format_entries(entries, *cls._write_format())
+
+    @classmethod
+    def join_fields(cls, fields):
+        from .write import join_fields
+        return join_fields(fields, *cls._write_format())
+
     # ---- fused count on the raw bytes (K6) ------------------------------------------------------
     def can_fuse_count(self) -> bool:
         return True
@@ -156,6 +174,7 @@ class CudaFastQBuffer(CudaOneLineBuffer):
     _check_plus = True
     dataclass = SequenceEntryWithQuality
     _field_lines = (0, 1, 3)       # name, sequence, quality (fastq_buffer.py:21-30)
+    _write_format_id = nv.FMT_FASTQ
 
     def get_field_by_number(self, i: int, t=None):
         if i == 2 and 2 not in self._fields:

@@ -1,6 +1,6 @@
-"""bnp.open for the sequence formats of the hot path (mirror of bionumpy/io/files.py:28-182):
-suffix -> buffer type, ``.gz`` detection, reader construction.  ``buffer_type=`` injects any class
-honouring the FileBuffer protocol, exactly as in the reference (files.py:52-68)."""
+"""bnp.open for the sequence formats of the hot path (mirror of bionumpy/io/files.py:28-227):
+suffix -> buffer type, ``.gz`` detection, reader or writer construction, count_entries.  ``buffer_type=`` injects any
+class honouring the FileBuffer protocol, exactly as in the reference (files.py:52-68)."""
 import gzip
 import os
 
@@ -11,6 +11,8 @@ buffer_types = {
     ".fq": CudaFastQBuffer,
     ".fastq": CudaFastQBuffer,
 }
+
+WRITE_MODES = {"w": "wb", "wb": "wb", "write": "wb", "a": "ab", "ab": "ab", "append": "ab"}
 
 
 def _multiline():
@@ -27,17 +29,30 @@ def _buffer_type_for(suffix):
                        f"(supported: .fq .fastq .fa .fasta and their .gz forms); pass buffer_type=")
 
 
-def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
-    """files.py:85-182 (reading only: writers are outside the k-mer hot path)."""
-    if mode not in (None, "r", "rb"):
-        raise NotImplementedError("only reading is on the CUDA k-mer path")
-    path = str(filename)
+def _suffix(path):
     base, suffix = os.path.splitext(path)
     is_gzip = suffix == ".gz"
     if is_gzip:
         suffix = os.path.splitext(base)[1]
+    return suffix, is_gzip
+
+
+def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
+    """files.py:85-182.  Reading ("r", "rb") gives an NpDataclassReader; writing ("w", "wb", "write") or appending
+    ("a", "ab", "append") gives an NpBufferedWriter, which writes ``.gz`` files as BGZF."""
+    if mode not in (None, "r", "rb") and mode not in WRITE_MODES:
+        raise NotImplementedError(f"mode {mode!r}: use r/rb to read, w/wb/write or a/ab/append to write")
+    path = str(filename)
+    suffix, is_gzip = _suffix(path)
     if buffer_type is None:
         buffer_type = _buffer_type_for(suffix)
+    if mode in WRITE_MODES:
+        from .write import NpBufferedWriter
+        raw = open(path, WRITE_MODES[mode])
+        if is_gzip:
+            from .bgzf import BgzfWriter
+            raw = BgzfWriter(raw)
+        return NpBufferedWriter(raw, buffer_type)
     from . import ingest
     raw = open(path, "rb")
     reader = ingest.open_reader(path, raw, buffer_type, is_gzip)        # pinned, prefetching ingest (FASTQ / 2-line FASTA)
@@ -47,3 +62,9 @@ def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
             raw = gzip.open(path, "rb")
         reader = CudaFileReader(raw, buffer_type)
     return NpDataclassReader(reader, lazy)
+
+
+def count_entries(filename, buffer_type=None) -> int:
+    """files.py:185-227: the number of entries in the file, the sum of its chunks' count_entries()."""
+    with bnp_open(filename, buffer_type=buffer_type) as f:
+        return sum(buff.count_entries() for buff in f._reader.read_chunks(min_chunk_size=5000000))

@@ -134,5 +134,22 @@ class CudaMultiLineFastaBuffer:
     def get_data(self):
         return self.dataclass.lazy(self)
 
+    # ---- writing (MultiLineFastaBuffer.from_data, io/multiline_buffer.py:67-86) --------------------------------------
+    @classmethod
+    def _write_format(cls):
+        return nv.FMT_FASTA_WRAPPED, int(cls.n_characters_per_line)
+
+    @classmethod
+    def from_data(cls, entries):
+        """The records as FASTA with n_characters_per_line bases per line: a device EncodedArray.  An entry with an
+        empty sequence is its header line alone."""
+        from .write import format_entries
+        return format_entries(entries, *cls._write_format())
+
+    @classmethod
+    def join_fields(cls, fields):
+        from .write import join_fields
+        return join_fields(fields, *cls._write_format())
+
 
 MultiLineFastaBuffer = CudaMultiLineFastaBuffer

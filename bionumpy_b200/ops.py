@@ -411,3 +411,65 @@ class HostPipeline:
             self.close()
         except Exception:
             pass
+
+
+def _format_fields(fields):
+    """A host bnpk_field[3] of (name, sequence, quality); each a (base uint8, starts int64, lens int32, lut uint8[256]
+    or None) of CUDA tensors, or None.  Returns (array, number of entries, device)."""
+    arr = (nv.Field * 3)()
+    n, dev = None, None
+    for i, f in enumerate(fields):
+        if f is None:
+            continue
+        base, starts, lens, lut = f
+        _need_cuda(base, "base")
+        _need_cuda(starts, "starts")
+        _need_cuda(lens, "lens")
+        if base.dtype != torch.uint8 or starts.dtype != torch.int64 or lens.dtype != torch.int32:
+            raise TypeError("base must be uint8, starts int64, lens int32")
+        if lut is not None:
+            _need_cuda(lut, "lut")
+            if lut.dtype != torch.uint8 or lut.numel() != 256:
+                raise TypeError("lut must be 256 uint8")
+        if n is None:
+            n, dev = lens.numel(), base.device
+        if lens.numel() != n or starts.numel() != n:
+            raise ValueError("every field needs one row per entry")
+        if any(t.device != dev for t in (base, starts, lens) + ((lut,) if lut is not None else ())):
+            raise ValueError("the fields are on different devices")
+        arr[i] = nv.Field(base.data_ptr() or None, base.numel(), starts.data_ptr() or None, lens.data_ptr() or None,
+                          lut.data_ptr() if lut is not None else None)
+    return arr, n or 0, dev
+
+
+def format_offsets(fmt, line_width, fields, status=None):
+    """int64[E+1] output offsets of the records (name, sequence, quality fields) in format ``fmt`` (nv.FMT_*) and the
+    status tensor; with a sequence LUT, a sequence byte the LUT maps to 0 is reported in status[ST_BAD_BASE]."""
+    arr, n, dev = _format_fields(fields)
+    if dev is None:
+        raise ValueError("format_offsets needs the name and sequence fields")
+    with torch.cuda.device(dev):
+        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        if status is None:
+            status = nv.new_status(dev)
+        ws = nv.workspace(max(n, 1), dev)
+        check(lib().bnpk_format_offsets(fmt, line_width, n, ctypes.cast(arr, ctypes.c_void_p), ptr(offsets),
+                                        ptr(status), ptr(ws), ws.numel(), stream_ptr()))
+    return offsets, status
+
+
+@_on_device
+def format_records(fmt, line_width, fields, offsets, out_begin=0, out_end=None, out=None):
+    """Bytes [out_begin, out_end) of the formatted records (default: all of them, offsets[-1] read back) into ``out``
+    (uint8, at least out_end - out_begin bytes; allocated when None).  Returns ``out``."""
+    _need_cuda(offsets, "offsets")
+    arr, n, _ = _format_fields(fields)
+    if out_end is None:
+        out_end = int(offsets[-1].item())
+    if out is None:
+        out = torch.empty(max(out_end - out_begin, 0), dtype=torch.uint8, device=offsets.device)
+    elif out.numel() < out_end - out_begin:
+        raise ValueError("out is smaller than the range")
+    check(lib().bnpk_format_records(fmt, line_width, n, ctypes.cast(arr, ctypes.c_void_p), ptr(offsets), out_begin,
+                                    out_end, ptr(out) if out.numel() else None, stream_ptr()))
+    return out

@@ -29,6 +29,18 @@ def segment_max(values, rows, n_rows):
     return out
 
 
+def segment_min(values, rows, n_rows):
+    """out[r] = min of values[i] with rows[i] == r, NaN if one of them is NaN; the dtype's highest value (+inf for
+    floats) where there is none."""
+    return -segment_max(-values, rows, n_rows) if values.is_floating_point() else \
+        _segment_min_int(values, rows, n_rows)
+
+
+def _segment_min_int(values, rows, n_rows):
+    out = torch.full((n_rows,), torch.iinfo(values.dtype).max, dtype=values.dtype, device=values.device)
+    return out.scatter_reduce_(0, rows, values, "amin", include_self=True)
+
+
 def segment_sum(values, rows, n_rows):
     """out[r] = the sum of values[i] with rows[i] == r, int64."""
     out = torch.zeros(n_rows, dtype=torch.int64, device=values.device)
@@ -243,6 +255,17 @@ class RaggedArray:
         if axis in (-1, 1):
             rows = torch.repeat_interleave(torch.arange(len(self), device=flat.device), self._lens.to(torch.int64))
             return segment_max(flat, rows, len(self))
+        raise NotImplementedError(axis)
+
+    def min(self, axis=None, **kwargs):
+        """np.min, the mirror of ``max``: axis=-1 gives one value per row; an empty row gives the dtype's highest value
+        (+inf for floats)."""
+        flat = self.ravel()
+        if axis is None:
+            return flat.min()
+        if axis in (-1, 1):
+            rows = torch.repeat_interleave(torch.arange(len(self), device=flat.device), self._lens.to(torch.int64))
+            return segment_min(flat, rows, len(self))
         raise NotImplementedError(axis)
 
     def sum(self, axis=None, **kwargs):

@@ -325,6 +325,48 @@ int bnpk_bloom_query(const int64_t *values, size_t n, const int64_t *offsets, in
                      uint8_t *out, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Writers: records -> file text (FastQBuffer.from_data / join_fields io/fastq_buffer.py:47-61,
+ * OneLineBuffer.join_fields io/one_line_buffer.py:119-134, MultiLineFastaBuffer.from_data
+ * io/multiline_buffer.py:67-86).  Entry e with name, sequence and quality lengths Ln, Ls, Lq is
+ *   BNPK_FMT_FASTQ          '@' name '\n' seq '\n' '+' '\n' qual '\n'            Ln + Ls + Lq + 6 bytes
+ *   BNPK_FMT_FASTA          '>' name '\n' seq '\n'                               Ln + Ls + 3
+ *   BNPK_FMT_FASTA_WRAPPED  '>' name '\n', then ceil(Ls / W) lines of W = line_width bases (the last one
+ *                           shorter), each ending in '\n'; an empty sequence gives no line
+ *                                                                                Ln + 2 + Ls + ceil(Ls / W)
+ * `fields` is a HOST array of three bnpk_field: name, sequence, quality (the quality is read by the
+ * FASTQ format only).  A field is the ragged view every row kernel takes, rows (base, starts[E],
+ * lens[E]); a byte outside [base, base + base_bytes) is written as lut256[0] (never read); lut256 (device, 256 bytes) NULL = copy the bytes, else each byte b is written as
+ * lut256[b] (an AlphabetEncoding's codes -> letters; qualities: (v + 33) & 255).
+ * Neither entry point traps on bad data.  BNPK_E_BADARG before any device work for an unknown format,
+ * line_width < 1 on the wrapped format, a missing name/sequence field (or quality field for FASTQ)
+ * when n_entries > 0, and, for bnpk_format_records, out_begin < 0, out_end < out_begin or a NULL out
+ * with a non-empty range.
+ * ------------------------------------------------------------------------------------- */
+#define BNPK_FMT_FASTQ         0
+#define BNPK_FMT_FASTA         1
+#define BNPK_FMT_FASTA_WRAPPED 2
+
+typedef struct bnpk_field {
+    const uint8_t *base;
+    size_t base_bytes;
+    const int64_t *starts;     /* int64[E] */
+    const int32_t *lens;       /* int32[E] (negative = 0) */
+    const uint8_t *lut256;     /* NULL or a device 256-byte table */
+} bnpk_field;
+
+/* out_offsets int64[E+1]: the exclusive prefix sum of the entry sizes, out_offsets[E] = the text's size (int64: a
+ * wrapped chromosome with a long name can exceed int32).  When the sequence field has a LUT, also reads every sequence
+ * byte once: the first byte b with lut256[b] == 0 is reported as (entry << 32 | position) in status[BNPK_ST_BAD_BASE]
+ * (status pre-initialised; EncodingError(offset), encodings/alphabet_encoding.py:34-46).  Raw text is not read.
+ * workspace as for bnpk_row_offsets with n := E. */
+int bnpk_format_offsets(int format, int line_width, size_t n_entries, const bnpk_field *fields, int64_t *out_offsets,
+                        int64_t *status, void *workspace, size_t workspace_bytes, void *stream);
+/* Bytes [out_begin, out_end) of the text whose offsets bnpk_format_offsets made, written to out[0 .. out_end -
+ * out_begin).  Any range may be asked for, so a large text can be formatted in slices. */
+int bnpk_format_records(int format, int line_width, size_t n_entries, const bnpk_field *fields,
+                        const int64_t *out_offsets, int64_t out_begin, int64_t out_end, uint8_t *out, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Host-buffer entry point (end-to-end): the call a reader loop makes with a chunk that is
  * still in host memory.  Copies `chunk_host` (pinned or pageable) to the device in slices on
  * a private copy stream, overlapping each slice's H2D with the fused count of the previous
