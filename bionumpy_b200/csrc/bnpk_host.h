@@ -4,6 +4,7 @@
 #include <atomic>
 #include <cstdio>
 #include <cstring>
+#include <type_traits>
 #include "bnpk_device.cuh"
 
 namespace bnpk {
@@ -36,6 +37,60 @@ int ensure_dyn_smem(const void *kernel, int bytes);
 // optional per-launch timing of the dominant (tile) kernel, see bnpk_profile_* in bnpk.h
 void profile_before(cudaStream_t st);
 void profile_after(cudaStream_t st);
+
+// Calls f(std::integral_constant<int, ENC>{}) with the BNPK_ENC_* that enc_mode names; any other value is refused.
+template <typename F>
+int with_enc(int enc_mode, F &&f) {
+    switch (enc_mode) {
+        case BNPK_ENC_ASCII_ACGT: return f(std::integral_constant<int, BNPK_ENC_ASCII_ACGT>{});
+        case BNPK_ENC_ASCII_ACTG: return f(std::integral_constant<int, BNPK_ENC_ASCII_ACTG>{});
+        case BNPK_ENC_CODES: return f(std::integral_constant<int, BNPK_ENC_CODES>{});
+        case BNPK_ENC_LUT: return f(std::integral_constant<int, BNPK_ENC_LUT>{});
+    }
+    return set_err(BNPK_E_BADARG, "bad enc_mode");
+}
+
+// Whether enc_mode can give the codes of an alphabet of alphabet_size letters: the ASCII encodings only give four-letter
+// codes, raw bytes (alphabet_size 256) are their own codes, and BNPK_ENC_LUT reads lut256.
+inline int check_enc(int enc_mode, const uint8_t *lut256, int alphabet_size) {
+    if (enc_mode < 0 || enc_mode > 3) return set_err(BNPK_E_BADARG, "bad enc_mode");
+    if (alphabet_size != 4 && enc_mode != BNPK_ENC_LUT && enc_mode != BNPK_ENC_CODES)
+        return set_err(BNPK_E_BADARG, "alphabets that are not four letters take BNPK_ENC_LUT or BNPK_ENC_CODES");
+    if (alphabet_size == 256 && enc_mode != BNPK_ENC_CODES)
+        return set_err(BNPK_E_BADARG, "raw bytes (alphabet_size 256) take BNPK_ENC_CODES");
+    if (enc_mode == BNPK_ENC_LUT && !lut256) return set_err(BNPK_E_BADARG, "lut256 required");
+    return 0;
+}
+
+// The grid of a grid-stride kernel: the CTAs its work asks for, at most ctas_per_sm on every SM, and at least one.
+inline unsigned grid_cap(size_t ctas_wanted, int ctas_per_sm) {
+    return (unsigned)std::max<size_t>(1, std::min(ctas_wanted, (size_t)sm_count() * ctas_per_sm));
+}
+
+// kern<<<grid, block, smem, st>>>(args...), counted in bnpk_launch_count; `profiled` times it for bnpk_profile_read.
+template <typename... P, typename... A>
+int launch(const char *name, void (*kern)(P...), unsigned grid, int block, size_t smem, cudaStream_t st, bool profiled,
+           const A &...args) {
+    if (profiled) profile_before(st);
+    kern<<<grid, block, smem, st>>>(args...);
+    if (profiled) profile_after(st);
+    BNPK_LAUNCHED(name);
+    return 0;
+}
+
+// A kernel that takes every CTA slot its shared memory leaves: raises its dynamic shared-memory limit to smem_max,
+// refuses with BNPK_E_BINS and `misfit` when not one CTA of `smem` bytes fits an SM, and launches as many CTAs as are
+// resident at once, at most ctas_wanted (none for no work).
+template <typename... P, typename... A>
+int launch_resident(const char *name, const char *misfit, void (*kern)(P...), size_t ctas_wanted, int block,
+                    size_t smem, size_t smem_max, cudaStream_t st, bool profiled, const A &...args) {
+    BNPK_DYN_SMEM(kern, smem_max);
+    int per_sm = 1;
+    BNPK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, block, smem));
+    if (per_sm < 1) return set_err(BNPK_E_BINS, misfit);
+    if (ctas_wanted == 0) return 0;
+    return launch(name, kern, grid_cap(ctas_wanted, per_sm), block, smem, st, profiled, args...);
+}
 
 size_t tile_workspace_bytes(size_t n);
 bool use_smem_hist(int64_t n_bins, int hist_mode);

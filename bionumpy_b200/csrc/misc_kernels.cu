@@ -382,7 +382,7 @@ int bnpk_count_byte(const uint8_t *chunk, size_t n, uint8_t value, int64_t *coun
     BNPK_CUDA(cudaMemsetAsync(count_out, 0, sizeof(int64_t), st));
     if (n == 0) return 0;
     const size_t want = (n / 16 + 255) / 256;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 8));
+    const unsigned grid = grid_cap(want, 8);
     const uint32_t pattern = 0x01010101u * value;
     count_byte_kernel<<<grid, 256, 0, st>>>(chunk, n, pattern, (unsigned long long *)count_out);
     BNPK_LAUNCHED("count_byte_kernel");
@@ -423,7 +423,7 @@ int bnpk_row_offsets(const int32_t *lens, size_t n_rows, int shrink, int64_t *of
     const size_t need = (kWsHeaderWords + n_tiles) * sizeof(uint64_t);
     if (workspace_bytes < need) return set_err(BNPK_E_WORKSPACE, "workspace too small");
     BNPK_CUDA(cudaMemsetAsync(workspace, 0, need, st));
-    const unsigned grid = (unsigned)std::min<size_t>(n_tiles, (size_t)sm_count() * 4);
+    const unsigned grid = grid_cap(n_tiles, 4);
     row_offsets_kernel<<<grid, kScanThreads, 0, st>>>(lens, n_rows, shrink, offsets, (uint64_t *)workspace);
     BNPK_LAUNCHED("row_offsets_kernel");
     return 0;
@@ -442,10 +442,10 @@ int bnpk_bincount(const int64_t *values, size_t n, int64_t n_bins, int hist_mode
         const size_t smem = (size_t)n_bins * 4;
         int per_sm = 1;
         BNPK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bincount_kernel<true>, 512, smem));
-        const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * std::max(per_sm, 1)));
+        const unsigned grid = grid_cap(want, std::max(per_sm, 1));
         bincount_kernel<true><<<grid, 512, smem, st>>>(values, n, (uint64_t)n_bins, (unsigned long long *)hist, status);
     } else {
-        const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 4));
+        const unsigned grid = grid_cap(want, 4);
         bincount_kernel<false><<<grid, 512, 0, st>>>(values, n, (uint64_t)n_bins, (unsigned long long *)hist, status);
     }
     BNPK_LAUNCHED("bincount_kernel");
@@ -457,7 +457,7 @@ int bnpk_bincount_rows(const int64_t *values, const int64_t *offsets, size_t n_r
     if (n_bins < 1) return set_err(BNPK_E_BINS, "n_bins must be positive");
     if (n_rows == 0) return 0;
     const size_t want = (n_rows + 7) / 8;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 8));
+    const unsigned grid = grid_cap(want, 8);
     bincount_rows_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(values, offsets, n_rows, (uint64_t)n_bins,
                                                                  (unsigned long long *)out, status);
     BNPK_LAUNCHED("bincount_rows_kernel");
@@ -467,7 +467,7 @@ int bnpk_bincount_rows(const int64_t *values, const int64_t *offsets, size_t n_r
 int bnpk_multiline_flags(const uint8_t *chunk, size_t n, const int64_t *line_starts, const int32_t *line_lens, size_t n_lines,
                          int32_t *is_header, int64_t *out2, void *stream) {
     if (n_lines == 0 || n == 0) return 0;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n_lines + 255) / 256, (size_t)sm_count() * 8));
+    const unsigned grid = grid_cap((n_lines + 255) / 256, 8);
     multiline_flags_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(chunk, n, line_starts, line_lens, n_lines, is_header, out2);
     BNPK_LAUNCHED("multiline_flags_kernel");
     return 0;
@@ -477,7 +477,7 @@ int bnpk_multiline_entries(const uint8_t *chunk, const int64_t *line_starts, con
                            const int64_t *hdr_before, size_t keep, int trim_cr, int64_t *h_starts, int32_t *h_lens,
                            int64_t *s_starts, int32_t *s_lens, int64_t *entry_lens, void *stream) {
     if (keep == 0) return 0;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((keep + 255) / 256, (size_t)sm_count() * 8));
+    const unsigned grid = grid_cap((keep + 255) / 256, 8);
     multiline_entries_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(chunk, line_starts, line_lens, is_header, hdr_before, keep, trim_cr,
                                                                      h_starts, h_lens, s_starts, s_lens,
                                                                      (unsigned long long *)entry_lens);
@@ -490,7 +490,7 @@ int bnpk_fasta_gather(const uint8_t *file, size_t file_bytes, size_t n_rows, con
                       const int64_t *out_offsets, uint8_t *out, int64_t *status, void *stream) {
     if (n_rows == 0) return 0;
     const size_t want = (n_rows + 7) / 8;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 8));
+    const unsigned grid = grid_cap(want, 8);
     fasta_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(file, file_bytes, n_rows, contig_offset, row_start, row_len, lenc,
                                                                 lenb, out_offsets, out, status);
     BNPK_LAUNCHED("fasta_gather_kernel");
@@ -501,7 +501,7 @@ int bnpk_bloom_insert(const int64_t *values, size_t n, const int64_t *offsets, i
                       void *stream) {
     if (n_hash < 1 || mask_size == 0) return set_err(BNPK_E_BADARG, "bloom filter needs hash functions and a mask");
     if (n == 0) return 0;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)sm_count() * 16));
+    const unsigned grid = grid_cap((n + 255) / 256, 16);
     bloom_insert_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(values, n, offsets, n_hash, mask, (uint64_t)mask_size);
     BNPK_LAUNCHED("bloom_insert_kernel");
     return 0;
@@ -511,7 +511,7 @@ int bnpk_bloom_query(const int64_t *values, size_t n, const int64_t *offsets, in
                      uint8_t *out, void *stream) {
     if (n_hash < 1 || mask_size == 0) return set_err(BNPK_E_BADARG, "bloom filter needs hash functions and a mask");
     if (n == 0) return 0;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)sm_count() * 16));
+    const unsigned grid = grid_cap((n + 255) / 256, 16);
     bloom_query_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(values, n, offsets, n_hash, mask, (uint64_t)mask_size, out);
     BNPK_LAUNCHED("bloom_query_kernel");
     return 0;
@@ -520,7 +520,7 @@ int bnpk_bloom_query(const int64_t *values, size_t n, const int64_t *offsets, in
 int bnpk_synth_fastq(uint8_t *out, uint64_t first_record, uint64_t n_records, uint64_t seed, void *stream) {
     if (n_records == 0) return 0;
     const uint64_t want = (n_records + 7) / 8;
-    const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)sm_count() * 16));
+    const unsigned grid = grid_cap(want, 16);
     synth_fastq_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(out, first_record, n_records, seed);
     BNPK_LAUNCHED("synth_fastq_kernel");
     return 0;

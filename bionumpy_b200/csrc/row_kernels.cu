@@ -658,35 +658,26 @@ static size_t rows_smem_bytes(bool counting, bool smem_hist, uint64_t n_bins) {
     return b;
 }
 
+static const char *const kRowsMisfit = "rows kernel does not fit shared memory";
+
 template <int RM, int ENC, bool SMEM_HIST, bool DEFERRED>
 static int launch_rows_t(const RowArgs &a, size_t est_rows, cudaStream_t st) {
+    constexpr bool PWM = (RM == RM_PWM || RM == RM_PWM_MAX);
     void (*kern)(const RowArgs);
-    if constexpr (RM == RM_PWM || RM == RM_PWM_MAX) kern = rows_pwm_kernel<RM, ENC>;
+    if constexpr (PWM) kern = rows_pwm_kernel<RM, ENC>;
     else kern = rows_kernel<RM, ENC, SMEM_HIST, DEFERRED>;
     constexpr bool COUNTING = (RM == RM_COUNT || RM == RM_COUNT_MIN);
     size_t smem = rows_smem_bytes(COUNTING, SMEM_HIST, a.n_bins);
-    if constexpr (RM == RM_PWM || RM == RM_PWM_MAX) smem += (size_t)4 * a.window * sizeof(double);
-    BNPK_DYN_SMEM(kern, 200 * 1024);
-    int per_sm = 1;
-    BNPK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kRowThreads, smem));
-    if (per_sm < 1) return set_err(BNPK_E_BINS, "rows kernel does not fit shared memory");
-    const size_t want = (est_rows + kRowWarps - 1) / kRowWarps;
-    const size_t cap = (size_t)sm_count() * per_sm;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min(want, cap));
-    kern<<<grid, kRowThreads, smem, st>>>(a);
-    BNPK_LAUNCHED((RM == RM_PWM || RM == RM_PWM_MAX) ? "rows_pwm_kernel" : "rows_kernel");
-    return 0;
+    if constexpr (PWM) smem += (size_t)4 * a.window * sizeof(double);
+    return launch_resident(PWM ? "rows_pwm_kernel" : "rows_kernel", kRowsMisfit, kern, (est_rows + kRowWarps - 1) / kRowWarps,
+                           kRowThreads, smem, 200 * 1024, st, false, a);
 }
 
 template <int RM, bool SMEM_HIST, bool DEFERRED>
 static int launch_rows_enc(const RowArgs &a, int enc_mode, size_t est_rows, cudaStream_t st) {
-    switch (enc_mode) {
-        case BNPK_ENC_ASCII_ACGT: return launch_rows_t<RM, BNPK_ENC_ASCII_ACGT, SMEM_HIST, DEFERRED>(a, est_rows, st);
-        case BNPK_ENC_ASCII_ACTG: return launch_rows_t<RM, BNPK_ENC_ASCII_ACTG, SMEM_HIST, DEFERRED>(a, est_rows, st);
-        case BNPK_ENC_CODES: return launch_rows_t<RM, BNPK_ENC_CODES, SMEM_HIST, DEFERRED>(a, est_rows, st);
-        case BNPK_ENC_LUT: return launch_rows_t<RM, BNPK_ENC_LUT, SMEM_HIST, DEFERRED>(a, est_rows, st);
-    }
-    return set_err(BNPK_E_BADARG, "bad enc_mode");
+    return with_enc(enc_mode, [&](auto enc) {
+        return launch_rows_t<RM, decltype(enc)::value, SMEM_HIST, DEFERRED>(a, est_rows, st);
+    });
 }
 
 // The kernels' view of a row entry point's rows (n_bins 1 for the modes that count nothing); the caller fills in its
@@ -703,22 +694,15 @@ static int check_common(int enc_mode, const uint8_t *lut256, int k, int window) 
     if (k < 1 || k > 31) return set_err(BNPK_E_K, "k must be larger than 0 and smaller than 32");
     if (window != 0 && window < k) return set_err(BNPK_E_WINDOW, "kmer size must be smaller than window size");
     if (window > kSegBytes / 2) return set_err(BNPK_E_WINDOW, "window_size above 1024 is not supported");
-    if (enc_mode < 0 || enc_mode > 3) return set_err(BNPK_E_BADARG, "bad enc_mode");
-    if (enc_mode == BNPK_ENC_LUT && !lut256) return set_err(BNPK_E_BADARG, "lut256 required");
-    return 0;
+    return check_enc(enc_mode, lut256, 4);
 }
 
 template <bool MINZ>
 static int launch_uncount(const RowArgs &a, int enc_mode, cudaStream_t st) {
-    const size_t smem = kWarpWords * 4 + 256;
-    switch (enc_mode) {
-        case BNPK_ENC_ASCII_ACGT: uncount_kernel<BNPK_ENC_ASCII_ACGT, MINZ><<<1, 32, smem, st>>>(a); break;
-        case BNPK_ENC_ASCII_ACTG: uncount_kernel<BNPK_ENC_ASCII_ACTG, MINZ><<<1, 32, smem, st>>>(a); break;
-        case BNPK_ENC_CODES: uncount_kernel<BNPK_ENC_CODES, MINZ><<<1, 32, smem, st>>>(a); break;
-        default: uncount_kernel<BNPK_ENC_LUT, MINZ><<<1, 32, smem, st>>>(a); break;
-    }
-    BNPK_LAUNCHED("uncount_kernel");
-    return 0;
+    return with_enc(enc_mode, [&](auto enc) {
+        return launch("uncount_kernel", uncount_kernel<decltype(enc)::value, MINZ>, 1, 32, kWarpWords * 4 + 256, st,
+                      false, a);
+    });
 }
 
 int count_fixups_impl(const uint8_t *chunk, size_t n, int lpe, int enc_mode, const uint8_t *lut256, int k,
@@ -740,10 +724,7 @@ static int check_pwm(int enc_mode, const uint8_t *lut256, int alphabet_size, con
     if (motif_len < 1 || motif_len > kPwmMaxLen) return set_err(BNPK_E_BADARG, "motif_len must be in 1..1024");
     if (alphabet_size < 2 || alphabet_size > 255) return set_err(BNPK_E_BADARG, "alphabet_size must be in 2..255");
     if (alphabet_size * motif_len > kPwmMaxCells) return set_err(BNPK_E_BADARG, "alphabet_size * motif_len above 8192");
-    if (enc_mode < 0 || enc_mode > 3) return set_err(BNPK_E_BADARG, "bad enc_mode");
-    if (alphabet_size != 4 && enc_mode != BNPK_ENC_LUT && enc_mode != BNPK_ENC_CODES)
-        return set_err(BNPK_E_BADARG, "alphabets that are not four letters take BNPK_ENC_LUT or BNPK_ENC_CODES");
-    if (enc_mode == BNPK_ENC_LUT && !lut256) return set_err(BNPK_E_BADARG, "lut256 required");
+    if (int rc = check_enc(enc_mode, lut256, alphabet_size)) return rc;
     if (!matrix) return set_err(BNPK_E_BADARG, "matrix required");
     return 0;
 }
@@ -762,10 +743,9 @@ static int launch_pwm(const uint8_t *base, size_t base_bytes, const int64_t *sta
     auto kern = rows_pwm_generic_kernel<SCORES>;
     const size_t smem = (size_t)alphabet_size * motif_len * sizeof(double) + 256;
     BNPK_DYN_SMEM(kern, kPwmMaxCells * sizeof(double) + 256);
-    const size_t want = (n_rows + 7) / 8;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 8));
-    kern<<<grid, 256, smem, st>>>(base, starts, lens, n_rows, enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size,
-                                  matrix, motif_len, tail, offsets, out, status);
+    kern<<<grid_cap((n_rows + 7) / 8, 8), 256, smem, st>>>(base, starts, lens, n_rows,
+                                                           enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size,
+                                                           matrix, motif_len, tail, offsets, out, status);
     BNPK_LAUNCHED("rows_pwm_generic_kernel");
     return 0;
 }
@@ -773,13 +753,8 @@ static int launch_pwm(const uint8_t *base, size_t base_bytes, const int64_t *sta
 // The limits of bnpk_rows_match*, and the kernels' view of the pattern in `m`.
 static int check_match(int enc_mode, const uint8_t *lut256, int alphabet_size, const uint32_t *sets,
                        const int32_t *sub_lens, int n_sub, int same, MatchArgs &m) {
-    if (enc_mode < 0 || enc_mode > 3) return set_err(BNPK_E_BADARG, "bad enc_mode");
     if (alphabet_size < 2 || alphabet_size > 256) return set_err(BNPK_E_BADARG, "alphabet_size must be in 2..256");
-    if (alphabet_size != 4 && enc_mode != BNPK_ENC_LUT && enc_mode != BNPK_ENC_CODES)
-        return set_err(BNPK_E_BADARG, "alphabets that are not four letters take BNPK_ENC_LUT or BNPK_ENC_CODES");
-    if (alphabet_size == 256 && enc_mode != BNPK_ENC_CODES)
-        return set_err(BNPK_E_BADARG, "raw bytes (alphabet_size 256) take BNPK_ENC_CODES");
-    if (enc_mode == BNPK_ENC_LUT && !lut256) return set_err(BNPK_E_BADARG, "lut256 required");
+    if (int rc = check_enc(enc_mode, lut256, alphabet_size)) return rc;
     if (!sets || !sub_lens) return set_err(BNPK_E_BADARG, "sets and sub_lens required");
     if (n_sub < 1 || n_sub > kMatchMaxSubs) return set_err(BNPK_E_BADARG, "n_sub must be in 1..64");
     if (same != 0 && same != 1) return set_err(BNPK_E_BADARG, "same must be 0 or 1");
@@ -807,33 +782,70 @@ static int launch_match(const uint8_t *base, size_t base_bytes, const int64_t *s
     if (alphabet_size == 4) {
         RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
         a.k = 1; a.window = m.span; a.offsets = offsets; a.out = out; a.status = status;
-        void (*kern)(const RowArgs, const MatchArgs);
-        switch (enc_mode) {
-            case BNPK_ENC_ASCII_ACGT: kern = rows_match_kernel<RM, BNPK_ENC_ASCII_ACGT>; break;
-            case BNPK_ENC_ASCII_ACTG: kern = rows_match_kernel<RM, BNPK_ENC_ASCII_ACTG>; break;
-            case BNPK_ENC_CODES: kern = rows_match_kernel<RM, BNPK_ENC_CODES>; break;
-            default: kern = rows_match_kernel<RM, BNPK_ENC_LUT>; break;
-        }
-        const size_t smem = rows_smem_bytes(false, false, 0) + kMatchSmemHead + (size_t)m.n_words * 4;
-        BNPK_DYN_SMEM(kern, rows_smem_bytes(false, false, 0) + kMatchSmemHead + kMatchMaxWords * 4);
-        int per_sm = 1;
-        BNPK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kRowThreads, smem));
-        if (per_sm < 1) return set_err(BNPK_E_BINS, "rows kernel does not fit shared memory");
-        const size_t want = (n_rows + kRowWarps - 1) / kRowWarps;
-        const unsigned grid = (unsigned)std::max<size_t>(1, std::min(want, (size_t)sm_count() * per_sm));
-        kern<<<grid, kRowThreads, smem, st>>>(a, m);
-        BNPK_LAUNCHED("rows_match_kernel");
-        return 0;
+        const size_t smem_head = rows_smem_bytes(false, false, 0) + kMatchSmemHead;
+        return with_enc(enc_mode, [&](auto enc) {
+            return launch_resident("rows_match_kernel", kRowsMisfit, rows_match_kernel<RM, decltype(enc)::value>,
+                                   (n_rows + kRowWarps - 1) / kRowWarps, kRowThreads, smem_head + (size_t)m.n_words * 4,
+                                   smem_head + kMatchMaxWords * 4, st, false, a, m);
+        });
     }
     auto kern = rows_match_generic_kernel<OUT>;
     const size_t smem = kMatchSmemHead + (size_t)m.n_words * 4 + 256;
     BNPK_DYN_SMEM(kern, kMatchSmemHead + kMatchMaxWords * 4 + 256);
-    const size_t want = (n_rows + 7) / 8;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 8));
-    kern<<<grid, 256, smem, st>>>(base, starts, lens, n_rows, enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size,
-                                  m, offsets, out, status);
+    kern<<<grid_cap((n_rows + 7) / 8, 8), 256, smem, st>>>(base, starts, lens, n_rows,
+                                                           enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size,
+                                                           m, offsets, out, status);
     BNPK_LAUNCHED("rows_match_generic_kernel");
     return 0;
+}
+
+static uint64_t canon_pattern(int complement_xor) {
+    return complement_xor == 3 ? ~0ull : complement_xor == 2 ? 0xAAAAAAAAAAAAAAAAull : 0x5555555555555555ull;
+}
+
+static int check_canonical(bool canonical, int complement_xor) {
+    if (canonical && (complement_xor < 1 || complement_xor > 3))
+        return set_err(BNPK_E_BADARG, "complement_xor must be 1, 2 or 3");
+    return 0;
+}
+
+// bnpk_rows_kmer_hash, bnpk_rows_kmer_hash_canonical and bnpk_rows_minimizers: the k-mer hashes of every row
+// (canonical ones with `canonical`), or their minima over every window of `window` bases.
+static int rows_kmer_hash(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                          size_t n_rows, int enc_mode, const uint8_t *lut256, int k, int window, bool canonical,
+                          int complement_xor, const int64_t *offsets, int64_t *out, int64_t *status, void *stream) {
+    if (int rc = check_common(enc_mode, lut256, k, window)) return rc;
+    if (int rc = check_canonical(canonical, complement_xor)) return rc;
+    if (n_rows == 0) return 0;
+    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
+    a.k = k; a.window = window; a.offsets = offsets; a.out = out; a.status = status;
+    if (canonical) a.canon_xor = canon_pattern(complement_xor);
+    cudaStream_t st = (cudaStream_t)stream;
+    return window ? launch_rows_enc<RM_MINIMIZER, false, false>(a, enc_mode, n_rows, st)
+                  : launch_rows_enc<RM_HASH, false, false>(a, enc_mode, n_rows, st);
+}
+
+// bnpk_rows_kmer_count and bnpk_rows_kmer_count_canonical: the k-mers of every row (canonical ones with `canonical`),
+// or their window minima, counted into hist.
+static int rows_kmer_count(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                           size_t n_rows, int enc_mode, const uint8_t *lut256, int k, int window, bool canonical,
+                           int complement_xor, int64_t n_bins, int hist_mode, int64_t *hist, int64_t *status,
+                           void *stream) {
+    if (int rc = check_common(enc_mode, lut256, k, window)) return rc;
+    if (int rc = check_canonical(canonical, complement_xor)) return rc;
+    if (n_bins < 1) return set_err(BNPK_E_BINS, "n_bins must be positive");
+    if (hist_mode == BNPK_HIST_SMEM && n_bins > kSmemMaxBins) return set_err(BNPK_E_BINS, "too many bins for the shared-memory histogram");
+    if (n_rows == 0) return 0;
+    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
+    a.k = k; a.window = window; a.n_bins = (uint64_t)n_bins; a.hist = (unsigned long long *)hist; a.status = status;
+    if (canonical) a.canon_xor = canon_pattern(complement_xor);
+    const bool sm = use_smem_hist(n_bins, hist_mode);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (window)
+        return sm ? launch_rows_enc<RM_COUNT_MIN, true, false>(a, enc_mode, n_rows, st)
+                  : launch_rows_enc<RM_COUNT_MIN, false, false>(a, enc_mode, n_rows, st);
+    return sm ? launch_rows_enc<RM_COUNT, true, false>(a, enc_mode, n_rows, st)
+              : launch_rows_enc<RM_COUNT, false, false>(a, enc_mode, n_rows, st);
 }
 
 }  // namespace bnpk
@@ -855,11 +867,8 @@ int bnpk_rows_encode(const uint8_t *base, size_t base_bytes, const int64_t *star
 int bnpk_rows_kmer_hash(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
                         int enc_mode, const uint8_t *lut256, int k, const int64_t *offsets, int64_t *hashes_out,
                         int64_t *status, void *stream) {
-    if (int rc = check_common(enc_mode, lut256, k, 0)) return rc;
-    if (n_rows == 0) return 0;
-    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
-    a.k = k; a.offsets = offsets; a.out = hashes_out; a.status = status;
-    return launch_rows_enc<RM_HASH, false, false>(a, enc_mode, n_rows, (cudaStream_t)stream);
+    return rows_kmer_hash(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, k, 0, false, 0, offsets, hashes_out,
+                          status, stream);
 }
 
 int bnpk_rows_generic_hash(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
@@ -868,10 +877,8 @@ int bnpk_rows_generic_hash(const uint8_t *base, size_t base_bytes, const int64_t
     if (k < 1 || k > 63) return set_err(BNPK_E_K, "k must be in 1..63 for the generic hash");
     if (alphabet_size < 2 || alphabet_size > 255) return set_err(BNPK_E_BADARG, "alphabet_size must be in 2..255");
     if (n_rows == 0) return 0;
-    const size_t want = (n_rows + 7) / 8;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 8));
-    rows_generic_hash_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(base, base_bytes, starts, lens, n_rows, lut256,
-                                                                    alphabet_size, k, offsets, hashes_out, status);
+    rows_generic_hash_kernel<<<grid_cap((n_rows + 7) / 8, 8), 256, 0, (cudaStream_t)stream>>>(
+        base, base_bytes, starts, lens, n_rows, lut256, alphabet_size, k, offsets, hashes_out, status);
     BNPK_LAUNCHED("rows_generic_hash_kernel");
     return 0;
 }
@@ -880,61 +887,29 @@ int bnpk_rows_minimizers(const uint8_t *base, size_t base_bytes, const int64_t *
                          int enc_mode, const uint8_t *lut256, int k, int window_size, const int64_t *offsets,
                          int64_t *mins_out, int64_t *status, void *stream) {
     if (window_size < 1) return set_err(BNPK_E_WINDOW, "window_size must be positive");
-    if (int rc = check_common(enc_mode, lut256, k, window_size)) return rc;
-    if (n_rows == 0) return 0;
-    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
-    a.k = k; a.window = window_size; a.offsets = offsets; a.out = mins_out; a.status = status;
-    return launch_rows_enc<RM_MINIMIZER, false, false>(a, enc_mode, n_rows, (cudaStream_t)stream);
+    return rows_kmer_hash(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, k, window_size, false, 0, offsets,
+                          mins_out, status, stream);
 }
 
 int bnpk_rows_kmer_count(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
                          int enc_mode, const uint8_t *lut256, int k, int window_size, int64_t n_bins, int hist_mode,
                          int64_t *hist, int64_t *status, void *stream) {
-    if (int rc = check_common(enc_mode, lut256, k, window_size)) return rc;
-    if (n_bins < 1) return set_err(BNPK_E_BINS, "n_bins must be positive");
-    if (hist_mode == BNPK_HIST_SMEM && n_bins > kSmemMaxBins) return set_err(BNPK_E_BINS, "too many bins for the shared-memory histogram");
-    if (n_rows == 0) return 0;
-    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
-    a.k = k; a.window = window_size; a.n_bins = (uint64_t)n_bins; a.hist = (unsigned long long *)hist; a.status = status;
-    const bool sm = use_smem_hist(n_bins, hist_mode);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (window_size)
-        return sm ? launch_rows_enc<RM_COUNT_MIN, true, false>(a, enc_mode, n_rows, st)
-                  : launch_rows_enc<RM_COUNT_MIN, false, false>(a, enc_mode, n_rows, st);
-    return sm ? launch_rows_enc<RM_COUNT, true, false>(a, enc_mode, n_rows, st)
-              : launch_rows_enc<RM_COUNT, false, false>(a, enc_mode, n_rows, st);
-}
-
-static uint64_t canon_pattern(int complement_xor) {
-    return complement_xor == 3 ? ~0ull : complement_xor == 2 ? 0xAAAAAAAAAAAAAAAAull : 0x5555555555555555ull;
+    return rows_kmer_count(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, k, window_size, false, 0, n_bins,
+                           hist_mode, hist, status, stream);
 }
 
 int bnpk_rows_kmer_hash_canonical(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
                                   size_t n_rows, int enc_mode, const uint8_t *lut256, int k, int complement_xor,
                                   const int64_t *offsets, int64_t *hashes_out, int64_t *status, void *stream) {
-    if (int rc = check_common(enc_mode, lut256, k, 0)) return rc;
-    if (complement_xor < 1 || complement_xor > 3) return set_err(BNPK_E_BADARG, "complement_xor must be 1, 2 or 3");
-    if (n_rows == 0) return 0;
-    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
-    a.k = k; a.offsets = offsets; a.out = hashes_out; a.status = status;
-    a.canon_xor = canon_pattern(complement_xor);
-    return launch_rows_enc<RM_HASH, false, false>(a, enc_mode, n_rows, (cudaStream_t)stream);
+    return rows_kmer_hash(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, k, 0, true, complement_xor, offsets,
+                          hashes_out, status, stream);
 }
 
 int bnpk_rows_kmer_count_canonical(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
                                    size_t n_rows, int enc_mode, const uint8_t *lut256, int k, int complement_xor,
                                    int64_t n_bins, int hist_mode, int64_t *hist, int64_t *status, void *stream) {
-    if (int rc = check_common(enc_mode, lut256, k, 0)) return rc;
-    if (complement_xor < 1 || complement_xor > 3) return set_err(BNPK_E_BADARG, "complement_xor must be 1, 2 or 3");
-    if (n_bins < 1) return set_err(BNPK_E_BINS, "n_bins must be positive");
-    if (hist_mode == BNPK_HIST_SMEM && n_bins > kSmemMaxBins) return set_err(BNPK_E_BINS, "too many bins for the shared-memory histogram");
-    if (n_rows == 0) return 0;
-    RowArgs a = row_args(base, base_bytes, starts, lens, n_rows, lut256);
-    a.k = k; a.n_bins = (uint64_t)n_bins; a.hist = (unsigned long long *)hist; a.status = status;
-    a.canon_xor = canon_pattern(complement_xor);
-    cudaStream_t st = (cudaStream_t)stream;
-    return use_smem_hist(n_bins, hist_mode) ? launch_rows_enc<RM_COUNT, true, false>(a, enc_mode, n_rows, st)
-                                            : launch_rows_enc<RM_COUNT, false, false>(a, enc_mode, n_rows, st);
+    return rows_kmer_count(base, base_bytes, starts, lens, n_rows, enc_mode, lut256, k, 0, true, complement_xor, n_bins,
+                           hist_mode, hist, status, stream);
 }
 
 static bool is_pow2(size_t c) { return c && (c & (c - 1)) == 0; }
@@ -962,8 +937,8 @@ int bnpk_kmer_table_rehash(const int64_t *keys, const int64_t *counts, size_t ca
     KmerTable t;
     t.keys = (unsigned long long *)new_keys; t.counts = (unsigned long long *)new_counts;
     t.mask = new_capacity - 1; t.n_used = (unsigned long long *)n_used;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>((capacity + 255) / 256, (size_t)sm_count() * 8));
-    table_rehash_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(keys, counts, capacity, t, status);
+    table_rehash_kernel<<<grid_cap((capacity + 255) / 256, 8), 256, 0, (cudaStream_t)stream>>>(keys, counts, capacity, t,
+                                                                                               status);
     BNPK_LAUNCHED("table_rehash_kernel");
     return 0;
 }
@@ -973,9 +948,9 @@ int bnpk_rows_reverse_complement(const uint8_t *base, size_t base_bytes, const i
     (void)base_bytes;
     if (!lut256) return set_err(BNPK_E_BADARG, "lut256 required");
     if (n_rows == 0) return 0;
-    const size_t want = (n_rows + 7) / 8;
-    const unsigned grid = (unsigned)std::max<size_t>(1, std::min<size_t>(want, (size_t)sm_count() * 8));
-    rows_reverse_complement_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(base, starts, lens, n_rows, lut256, offsets, out);
+    rows_reverse_complement_kernel<<<grid_cap((n_rows + 7) / 8, 8), 256, 0, (cudaStream_t)stream>>>(base, starts, lens,
+                                                                                                     n_rows, lut256,
+                                                                                                     offsets, out);
     BNPK_LAUNCHED("rows_reverse_complement_kernel");
     return 0;
 }

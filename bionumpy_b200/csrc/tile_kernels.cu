@@ -443,20 +443,10 @@ static size_t tile_smem_bytes(int mode, uint64_t n_bins, bool smem_hist) {
 
 template <int MODE, int ENC, bool SMEM_HIST, bool MINIMIZER>
 static int launch_tile(const TileArgs &a, cudaStream_t st) {
-    auto kern = tile_kernel<MODE, ENC, SMEM_HIST, MINIMIZER>;
-    const size_t smem = tile_smem_bytes(MODE, a.n_bins, SMEM_HIST);
-    BNPK_DYN_SMEM(kern, 200 * 1024);
-    int per_sm = 1;
-    BNPK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kCtaThreads, smem));
-    if (per_sm < 1) return set_err(BNPK_E_BINS, "tile kernel does not fit shared memory");
-    const int64_t n_tiles = a.tile_end - a.tile_begin;
-    if (n_tiles <= 0) return 0;
-    const int64_t grid = std::min<int64_t>(n_tiles, (int64_t)sm_count() * per_sm);
-    profile_before(st);
-    kern<<<(unsigned)grid, kCtaThreads, smem, st>>>(a);
-    profile_after(st);
-    BNPK_LAUNCHED("tile_kernel");
-    return 0;
+    const int64_t n_tiles = std::max<int64_t>(a.tile_end - a.tile_begin, 0);
+    return launch_resident("tile_kernel", "tile kernel does not fit shared memory",
+                           tile_kernel<MODE, ENC, SMEM_HIST, MINIMIZER>, (size_t)n_tiles, kCtaThreads,
+                           tile_smem_bytes(MODE, a.n_bins, SMEM_HIST), 200 * 1024, st, true, a);
 }
 
 template <int ENC>
@@ -471,13 +461,7 @@ static int launch_count(const TileArgs &a, int enc_mode, bool smem_hist, cudaStr
     if (wsm_count_eligible(a, smem_hist)) return launch_wsm_count(a, enc_mode, st);
     if (ws_count_eligible(a, smem_hist)) return launch_ws_count(a, enc_mode, st);
     if (tma_count_eligible(a, smem_hist)) return launch_tma_count(a, enc_mode, st);
-    switch (enc_mode) {
-        case BNPK_ENC_ASCII_ACGT: return launch_count_enc<BNPK_ENC_ASCII_ACGT>(a, smem_hist, st);
-        case BNPK_ENC_ASCII_ACTG: return launch_count_enc<BNPK_ENC_ASCII_ACTG>(a, smem_hist, st);
-        case BNPK_ENC_CODES: return launch_count_enc<BNPK_ENC_CODES>(a, smem_hist, st);
-        case BNPK_ENC_LUT: return launch_count_enc<BNPK_ENC_LUT>(a, smem_hist, st);
-    }
-    return set_err(BNPK_E_BADARG, "bad enc_mode");
+    return with_enc(enc_mode, [&](auto enc) { return launch_count_enc<decltype(enc)::value>(a, smem_hist, st); });
 }
 
 static size_t deferred_capacity(size_t n) { return n / kHaloBytes + n / 1024 + 16; }
@@ -515,7 +499,7 @@ int chunk_kmer_count_impl(const uint8_t *chunk, size_t n, size_t slice_begin, si
     if (window > 1024) return set_err(BNPK_E_WINDOW, "window_size above 1024 is not supported");
     if (n_bins < 1) return set_err(BNPK_E_BINS, "n_bins must be positive");
     if (hist_mode == BNPK_HIST_SMEM && n_bins > kSmemMaxBins) return set_err(BNPK_E_BINS, "too many bins for the shared-memory histogram");
-    if (enc_mode == BNPK_ENC_LUT && !lut256) return set_err(BNPK_E_BADARG, "lut256 required");
+    if (int rc = check_enc(enc_mode, lut256, 4)) return rc;
     if ((lpe != 2 && lpe != 4) || slice_end > n || slice_begin > slice_end)
         return set_err(BNPK_E_BADARG, "lines_per_entry must be 2 or 4; slice must lie inside the chunk");
     if (workspace_bytes < tile_workspace_bytes(n)) return set_err(BNPK_E_WORKSPACE, "workspace too small");

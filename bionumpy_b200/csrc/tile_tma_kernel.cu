@@ -378,16 +378,11 @@ __global__ void __launch_bounds__(kCta, 1) tile_tma_kernel(const TileArgs a) {
 template <int ENC, int HIST>
 static int launch_t(const TileArgs &a, cudaStream_t st) {
     auto kern = tile_tma_kernel<ENC, HIST>;
-    const size_t smem = (size_t)kFixedBytes;
     BNPK_DYN_SMEM(kern, kFixedBytes);
     const int64_t n_tiles = a.tile_end - a.tile_begin;
     if (n_tiles <= 0) return 0;
-    const int64_t grid = std::min<int64_t>((n_tiles + kGroups - 1) / kGroups, (int64_t)sm_count());
-    profile_before(st);
-    kern<<<(unsigned)grid, kCta, smem, st>>>(a);
-    profile_after(st);
-    BNPK_LAUNCHED("tile_tma_kernel");
-    return 0;
+    return launch("tile_tma_kernel", kern, grid_cap((size_t)(n_tiles + kGroups - 1) / kGroups, 1), kCta, kFixedBytes, st,
+                  true, a);
 }
 
 template <int ENC>
@@ -405,13 +400,7 @@ bool tma_count_eligible(const TileArgs &a, bool smem_hist) {
 }
 
 int launch_tma_count(const TileArgs &a, int enc_mode, cudaStream_t st) {
-    switch (enc_mode) {
-        case BNPK_ENC_ASCII_ACGT: return tma::launch_enc<BNPK_ENC_ASCII_ACGT>(a, st);
-        case BNPK_ENC_ASCII_ACTG: return tma::launch_enc<BNPK_ENC_ASCII_ACTG>(a, st);
-        case BNPK_ENC_CODES: return tma::launch_enc<BNPK_ENC_CODES>(a, st);
-        case BNPK_ENC_LUT: return tma::launch_enc<BNPK_ENC_LUT>(a, st);
-    }
-    return set_err(BNPK_E_BADARG, "bad enc_mode");
+    return with_enc(enc_mode, [&](auto enc) { return tma::launch_enc<decltype(enc)::value>(a, st); });
 }
 
 }  // namespace bnpk

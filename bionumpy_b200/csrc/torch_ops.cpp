@@ -23,9 +23,26 @@ void check(int rc, const char *what) {
     TORCH_CHECK(rc == 0, "bnpk::", what, ": ", bnpk_last_error(), " (code ", rc, ")");
 }
 const uint8_t *u8(const Tensor &t) { return t.defined() && t.numel() ? t.data_ptr<uint8_t>() : nullptr; }
-void need(const Tensor &t, c10::ScalarType st, const char *name) {
+// t is a contiguous CUDA tensor of dtype st, on the device of `on` when that is given: a kernel reads every pointer it
+// gets on the device it runs on.
+void need(const Tensor &t, c10::ScalarType st, const char *name, const Tensor &on = Tensor()) {
     TORCH_CHECK(t.is_cuda() && t.is_contiguous() && t.scalar_type() == st, "bnpk: ", name,
                 " must be a contiguous CUDA tensor of the right dtype");
+    TORCH_CHECK(!on.defined() || t.device() == on.device(), "bnpk: ", name, " is on ", t.device(), ", not on ",
+                on.device());
+}
+// an optional 256-byte table: the kernels read all of it
+const uint8_t *need_lut(const c10::optional<Tensor> &lut, const char *name, const Tensor &on) {
+    if (!lut) return nullptr;
+    need(*lut, torch::kUInt8, name, on);
+    TORCH_CHECK(lut->numel() == 256, "bnpk: ", name, " must have 256 entries");
+    return lut->data_ptr<uint8_t>();
+}
+// out_offsets[r] for the rows r < n_rows, and the total at n_rows
+const int64_t *need_offsets(const Tensor &offsets, size_t n_rows, const Tensor &on) {
+    need(offsets, torch::kInt64, "offsets", on);
+    TORCH_CHECK((size_t)offsets.numel() >= n_rows + 1, "bnpk: offsets need one entry per row and the total");
+    return offsets.data_ptr<int64_t>();
 }
 void *cur_stream(const Tensor &t) { return (void *)at::cuda::getCurrentCUDAStream(t.get_device()).stream(); }
 Tensor new_status(const Tensor &like) {
@@ -37,21 +54,47 @@ Tensor new_workspace(const Tensor &like, size_t n) {
     return torch::empty({(int64_t)bnpk_tile_workspace_bytes(n)}, like.options().dtype(torch::kUInt8));
 }
 
+// The rows of a row op: bytes base[starts[r], starts[r] + lens[r]) for r < n_rows, and the op's 256-byte lut (or
+// null).  call(fn, more...) is fn(base, base_bytes, starts, lens, n_rows, more...), the head of every bnpk_rows_*.
+struct Rows {
+    const uint8_t *base;
+    size_t base_bytes;
+    const int64_t *starts;
+    const int32_t *lens;
+    size_t n_rows;
+    const uint8_t *lut;
+    template <typename F, typename... A>
+    int call(F fn, A... more) const { return fn(base, base_bytes, starts, lens, n_rows, more...); }
+};
+
+// base uint8, starts int64 and lens int32 of one length, and lut uint8[256] or None: contiguous CUDA tensors, all on
+// the device of `on` (default: base's).
+Rows need_rows(const Tensor &base, const Tensor &starts, const Tensor &lens, const c10::optional<Tensor> &lut,
+               const Tensor &on = Tensor()) {
+    const Tensor &dev = on.defined() ? on : base;
+    need(base, torch::kUInt8, "base", dev);
+    need(starts, torch::kInt64, "starts", dev);
+    need(lens, torch::kInt32, "lens", dev);
+    TORCH_CHECK(starts.numel() == lens.numel(), "bnpk: starts and lens differ in length");
+    return Rows{u8(base), (size_t)base.numel(), starts.data_ptr<int64_t>(), lens.data_ptr<int32_t>(),
+                (size_t)lens.numel(), need_lut(lut, "lut", dev)};
+}
+
 // K6: chunk bytes -> histogram (accumulated into hist).  Returns the status block.
 Tensor chunk_kmer_count(const Tensor &chunk, int64_t k, int64_t window_size, Tensor hist, int64_t lines_per_entry,
                         int64_t header_char, bool check_plus, int64_t trim_cr, int64_t enc_mode,
                         const c10::optional<Tensor> &lut, int64_t hist_mode) {
     need(chunk, torch::kUInt8, "chunk");
-    need(hist, torch::kInt64, "hist");
-    TORCH_CHECK(hist.get_device() == chunk.get_device(), "bnpk: chunk and hist on different devices");
+    need(hist, torch::kInt64, "hist", chunk);
+    const uint8_t *l = need_lut(lut, "lut", chunk);
     c10::cuda::CUDAGuard guard(chunk.device());
     Tensor status = new_status(chunk);
     const size_t n = (size_t)chunk.numel();
     Tensor ws = new_workspace(chunk, n);
     check(bnpk_chunk_kmer_count(chunk.data_ptr<uint8_t>(), n, 0, n, 1, (int)lines_per_entry, (uint8_t)header_char,
-                                check_plus, (int)trim_cr, (int)enc_mode, lut ? u8(*lut) : nullptr, (int)k,
-                                (int)window_size, hist.numel(), (int)hist_mode, hist.data_ptr<int64_t>(),
-                                status.data_ptr<int64_t>(), ws.data_ptr<uint8_t>(), (size_t)ws.numel(), cur_stream(chunk)),
+                                check_plus, (int)trim_cr, (int)enc_mode, l, (int)k, (int)window_size, hist.numel(),
+                                (int)hist_mode, hist.data_ptr<int64_t>(), status.data_ptr<int64_t>(), ws.data_ptr<uint8_t>(),
+                                (size_t)ws.numel(), cur_stream(chunk)),
           "chunk_kmer_count");
     return status;
 }
@@ -86,23 +129,16 @@ Tensor row_offsets(const Tensor &lens, int64_t shrink) {
     return out;
 }
 
-void need_rows(const Tensor &base, const Tensor &starts, const Tensor &lens) {
-    need(base, torch::kUInt8, "base");
-    need(starts, torch::kInt64, "starts");
-    need(lens, torch::kInt32, "lens");
-    TORCH_CHECK(starts.numel() == lens.numel(), "bnpk: starts and lens differ in length");
-}
-
 // K2: codes uint8[total] (total = offsets[-1], given by the caller: no sync here)
 std::tuple<Tensor, Tensor> rows_encode(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t enc_mode,
                                        const c10::optional<Tensor> &lut, const Tensor &offsets, int64_t total) {
-    need_rows(base, starts, lens);
+    const Rows r = need_rows(base, starts, lens, lut);
+    const int64_t *offs = need_offsets(offsets, r.n_rows, base);
     c10::cuda::CUDAGuard guard(base.device());
     Tensor out = torch::empty({total}, base.options());
     Tensor status = new_status(base);
-    check(bnpk_rows_encode(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
-                           lens.data_ptr<int32_t>(), (size_t)lens.numel(), (int)enc_mode, lut ? u8(*lut) : nullptr,
-                           offsets.data_ptr<int64_t>(), out.data_ptr<uint8_t>(), status.data_ptr<int64_t>(), cur_stream(base)),
+    check(r.call(bnpk_rows_encode, (int)enc_mode, r.lut, offs, out.data_ptr<uint8_t>(), status.data_ptr<int64_t>(),
+                 cur_stream(base)),
           "rows_encode");
     return {out, status};
 }
@@ -111,25 +147,21 @@ std::tuple<Tensor, Tensor> rows_encode(const Tensor &base, const Tensor &starts,
 std::tuple<Tensor, Tensor> rows_kmer_hash(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t enc_mode,
                                           const c10::optional<Tensor> &lut, int64_t k, int64_t window_size,
                                           int64_t complement_xor, const Tensor &offsets, int64_t total) {
-    need_rows(base, starts, lens);
+    const Rows r = need_rows(base, starts, lens, lut);
+    const int64_t *offs = need_offsets(offsets, r.n_rows, base);
+    TORCH_CHECK(window_size == 0 || complement_xor == 0, "bnpk: minimizers are not canonical (complement_xor must be 0)");
     c10::cuda::CUDAGuard guard(base.device());
     Tensor out = torch::empty({total}, base.options().dtype(torch::kInt64));
     Tensor status = new_status(base);
-    const uint8_t *l = lut ? u8(*lut) : nullptr;
+    int64_t *o = out.data_ptr<int64_t>(), *st = status.data_ptr<int64_t>();
     int rc;
     if (window_size)
-        rc = bnpk_rows_minimizers(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(), lens.data_ptr<int32_t>(),
-                                  (size_t)lens.numel(), (int)enc_mode, l, (int)k, (int)window_size, offsets.data_ptr<int64_t>(),
-                                  out.data_ptr<int64_t>(), status.data_ptr<int64_t>(), cur_stream(base));
+        rc = r.call(bnpk_rows_minimizers, (int)enc_mode, r.lut, (int)k, (int)window_size, offs, o, st, cur_stream(base));
     else if (complement_xor)
-        rc = bnpk_rows_kmer_hash_canonical(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
-                                           lens.data_ptr<int32_t>(), (size_t)lens.numel(), (int)enc_mode, l, (int)k,
-                                           (int)complement_xor, offsets.data_ptr<int64_t>(), out.data_ptr<int64_t>(),
-                                           status.data_ptr<int64_t>(), cur_stream(base));
+        rc = r.call(bnpk_rows_kmer_hash_canonical, (int)enc_mode, r.lut, (int)k, (int)complement_xor, offs, o, st,
+                    cur_stream(base));
     else
-        rc = bnpk_rows_kmer_hash(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(), lens.data_ptr<int32_t>(),
-                                 (size_t)lens.numel(), (int)enc_mode, l, (int)k, offsets.data_ptr<int64_t>(),
-                                 out.data_ptr<int64_t>(), status.data_ptr<int64_t>(), cur_stream(base));
+        rc = r.call(bnpk_rows_kmer_hash, (int)enc_mode, r.lut, (int)k, offs, o, st, cur_stream(base));
     check(rc, "rows_kmer_hash");
     return {out, status};
 }
@@ -138,21 +170,18 @@ std::tuple<Tensor, Tensor> rows_kmer_hash(const Tensor &base, const Tensor &star
 Tensor rows_kmer_count(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t enc_mode,
                        const c10::optional<Tensor> &lut, int64_t k, int64_t window_size, int64_t complement_xor,
                        Tensor hist, int64_t hist_mode) {
-    need_rows(base, starts, lens);
-    need(hist, torch::kInt64, "hist");
+    const Rows r = need_rows(base, starts, lens, lut);
+    need(hist, torch::kInt64, "hist", base);
+    TORCH_CHECK(window_size == 0 || complement_xor == 0, "bnpk: minimizers are not canonical (complement_xor must be 0)");
     c10::cuda::CUDAGuard guard(base.device());
     Tensor status = new_status(base);
-    const uint8_t *l = lut ? u8(*lut) : nullptr;
     int rc;
     if (complement_xor)
-        rc = bnpk_rows_kmer_count_canonical(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
-                                            lens.data_ptr<int32_t>(), (size_t)lens.numel(), (int)enc_mode, l, (int)k,
-                                            (int)complement_xor, hist.numel(), (int)hist_mode, hist.data_ptr<int64_t>(),
-                                            status.data_ptr<int64_t>(), cur_stream(base));
+        rc = r.call(bnpk_rows_kmer_count_canonical, (int)enc_mode, r.lut, (int)k, (int)complement_xor, hist.numel(),
+                    (int)hist_mode, hist.data_ptr<int64_t>(), status.data_ptr<int64_t>(), cur_stream(base));
     else
-        rc = bnpk_rows_kmer_count(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(), lens.data_ptr<int32_t>(),
-                                  (size_t)lens.numel(), (int)enc_mode, l, (int)k, (int)window_size, hist.numel(), (int)hist_mode,
-                                  hist.data_ptr<int64_t>(), status.data_ptr<int64_t>(), cur_stream(base));
+        rc = r.call(bnpk_rows_kmer_count, (int)enc_mode, r.lut, (int)k, (int)window_size, hist.numel(), (int)hist_mode,
+                    hist.data_ptr<int64_t>(), status.data_ptr<int64_t>(), cur_stream(base));
     check(rc, "rows_kmer_count");
     return status;
 }
@@ -161,31 +190,27 @@ Tensor rows_kmer_count(const Tensor &base, const Tensor &starts, const Tensor &l
 Tensor rows_kmer_table_insert(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t enc_mode,
                               const c10::optional<Tensor> &lut, int64_t k, int64_t complement_xor, Tensor keys,
                               Tensor counts, Tensor n_used) {
-    need_rows(base, starts, lens);
-    need(keys, torch::kInt64, "keys");
-    need(counts, torch::kInt64, "counts");
-    need(n_used, torch::kInt64, "n_used");
+    const Rows r = need_rows(base, starts, lens, lut);
+    need(keys, torch::kInt64, "keys", base);
+    need(counts, torch::kInt64, "counts", base);
+    need(n_used, torch::kInt64, "n_used", base);
     TORCH_CHECK(keys.numel() == counts.numel() && n_used.numel() == 1, "bnpk: keys/counts differ in length or n_used is not one word");
     c10::cuda::CUDAGuard guard(base.device());
     Tensor status = new_status(base);
-    check(bnpk_rows_kmer_table_insert(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
-                                      lens.data_ptr<int32_t>(), (size_t)lens.numel(), (int)enc_mode, lut ? u8(*lut) : nullptr,
-                                      (int)k, (int)complement_xor, keys.data_ptr<int64_t>(), counts.data_ptr<int64_t>(),
-                                      (size_t)keys.numel(), n_used.data_ptr<int64_t>(), status.data_ptr<int64_t>(),
-                                      cur_stream(base)),
+    check(r.call(bnpk_rows_kmer_table_insert, (int)enc_mode, r.lut, (int)k, (int)complement_xor, keys.data_ptr<int64_t>(),
+                 counts.data_ptr<int64_t>(), (size_t)keys.numel(), n_used.data_ptr<int64_t>(), status.data_ptr<int64_t>(),
+                 cur_stream(base)),
           "rows_kmer_table_insert");
     return status;
 }
 
 Tensor rows_reverse_complement(const Tensor &base, const Tensor &starts, const Tensor &lens, const Tensor &lut,
                                const Tensor &offsets, int64_t total) {
-    need_rows(base, starts, lens);
-    need(lut, torch::kUInt8, "lut");
+    const Rows r = need_rows(base, starts, lens, lut);
+    const int64_t *offs = need_offsets(offsets, r.n_rows, base);
     c10::cuda::CUDAGuard guard(base.device());
     Tensor out = torch::empty({total}, base.options());
-    check(bnpk_rows_reverse_complement(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
-                                       lens.data_ptr<int32_t>(), (size_t)lens.numel(), lut.data_ptr<uint8_t>(),
-                                       offsets.data_ptr<int64_t>(), out.data_ptr<uint8_t>(), cur_stream(base)),
+    check(r.call(bnpk_rows_reverse_complement, r.lut, offs, out.data_ptr<uint8_t>(), cur_stream(base)),
           "rows_reverse_complement");
     return out;
 }
@@ -194,17 +219,15 @@ Tensor rows_reverse_complement(const Tensor &base, const Tensor &starts, const T
 std::tuple<Tensor, Tensor> rows_pwm_scores(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t enc_mode,
                                            const c10::optional<Tensor> &lut, const Tensor &matrix, bool tail,
                                            const Tensor &offsets, int64_t total) {
-    need_rows(base, starts, lens);
-    need(matrix, torch::kFloat64, "matrix");
+    const Rows r = need_rows(base, starts, lens, lut);
+    const int64_t *offs = need_offsets(offsets, r.n_rows, base);
+    need(matrix, torch::kFloat64, "matrix", base);
     TORCH_CHECK(matrix.dim() == 2, "bnpk: matrix must be [motif_len, alphabet_size]");
     c10::cuda::CUDAGuard guard(base.device());
     Tensor out = torch::empty({total}, base.options().dtype(torch::kFloat64));
     Tensor status = new_status(base);
-    check(bnpk_rows_pwm_scores(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
-                               lens.data_ptr<int32_t>(), (size_t)lens.numel(), (int)enc_mode, lut ? u8(*lut) : nullptr,
-                               (int)matrix.size(1), matrix.data_ptr<double>(), (int)matrix.size(0), tail,
-                               offsets.data_ptr<int64_t>(), out.data_ptr<double>(), status.data_ptr<int64_t>(),
-                               cur_stream(base)),
+    check(r.call(bnpk_rows_pwm_scores, (int)enc_mode, r.lut, (int)matrix.size(1), matrix.data_ptr<double>(),
+                 (int)matrix.size(0), (int)tail, offs, out.data_ptr<double>(), status.data_ptr<int64_t>(), cur_stream(base)),
           "rows_pwm_scores");
     return {out, status};
 }
@@ -213,17 +236,16 @@ std::tuple<Tensor, Tensor> rows_pwm_scores(const Tensor &base, const Tensor &sta
 std::tuple<Tensor, Tensor> rows_match(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t enc_mode,
                                       const c10::optional<Tensor> &lut, int64_t alphabet_size, const Tensor &sets,
                                       c10::IntArrayRef sub_lens, bool same, const Tensor &offsets, int64_t total) {
-    need_rows(base, starts, lens);
-    need(sets, torch::kInt32, "sets");
+    const Rows r = need_rows(base, starts, lens, lut);
+    const int64_t *offs = need_offsets(offsets, r.n_rows, base);
+    need(sets, torch::kInt32, "sets", base);
     std::vector<int32_t> sl(sub_lens.begin(), sub_lens.end());
     c10::cuda::CUDAGuard guard(base.device());
     Tensor out = torch::empty({total}, base.options().dtype(torch::kUInt8));
     Tensor status = new_status(base);
-    check(bnpk_rows_match(base.data_ptr<uint8_t>(), (size_t)base.numel(), starts.data_ptr<int64_t>(),
-                          lens.data_ptr<int32_t>(), (size_t)lens.numel(), (int)enc_mode, lut ? u8(*lut) : nullptr,
-                          (int)alphabet_size, reinterpret_cast<const uint32_t *>(sets.data_ptr<int32_t>()), sl.data(),
-                          (int)sl.size(), same, offsets.data_ptr<int64_t>(), out.data_ptr<uint8_t>(),
-                          status.data_ptr<int64_t>(), cur_stream(base)),
+    check(r.call(bnpk_rows_match, (int)enc_mode, r.lut, (int)alphabet_size,
+                 reinterpret_cast<const uint32_t *>(sets.data_ptr<int32_t>()), sl.data(), (int)sl.size(),
+                 (int)same, offs, out.data_ptr<uint8_t>(), status.data_ptr<int64_t>(), cur_stream(base)),
           "rows_match");
     return {out, status};
 }
@@ -231,7 +253,7 @@ std::tuple<Tensor, Tensor> rows_match(const Tensor &base, const Tensor &starts, 
 // K5 (accumulates into hist)
 Tensor bincount(const Tensor &values, Tensor hist, int64_t hist_mode) {
     need(values, torch::kInt64, "values");
-    need(hist, torch::kInt64, "hist");
+    need(hist, torch::kInt64, "hist", values);
     c10::cuda::CUDAGuard guard(values.device());
     Tensor status = new_status(values);
     check(bnpk_bincount(values.data_ptr<int64_t>(), (size_t)values.numel(), hist.numel(), (int)hist_mode,
@@ -241,17 +263,17 @@ Tensor bincount(const Tensor &values, Tensor hist, int64_t hist_mode) {
 }
 
 // Writers: fields = [name base, starts, lens, sequence base, starts, lens(, quality base, starts, lens)], luts = one
-// optional 256-byte table per field.  format_offsets returns (offsets int64[E+1], status); format_records writes bytes
-// [out_begin, out_end) of the text (the caller reads offsets[-1] for the total: no sync here).
+// optional 256-byte table per field, all on the device of the name base.  format_offsets returns (offsets int64[E+1],
+// status); format_records writes bytes [out_begin, out_end) of the text (the caller reads offsets[-1] for the total: no
+// sync here).
 std::vector<bnpk_field> make_fields(const std::vector<Tensor> &fields, const std::vector<c10::optional<Tensor>> &luts) {
     TORCH_CHECK(fields.size() == 6 || fields.size() == 9, "bnpk: fields are (base, starts, lens) of 2 or 3 fields");
     TORCH_CHECK(luts.size() * 3 == fields.size(), "bnpk: one lut (or None) per field");
     std::vector<bnpk_field> out(3, bnpk_field{nullptr, 0, nullptr, nullptr, nullptr});
     for (size_t f = 0; f < luts.size(); ++f) {
-        need_rows(fields[3 * f], fields[3 * f + 1], fields[3 * f + 2]);
-        TORCH_CHECK(fields[3 * f + 2].numel() == fields[2].numel(), "bnpk: fields differ in entry count");
-        out[f] = bnpk_field{u8(fields[3 * f]), (size_t)fields[3 * f].numel(), fields[3 * f + 1].data_ptr<int64_t>(),
-                            fields[3 * f + 2].data_ptr<int32_t>(), luts[f] ? u8(*luts[f]) : nullptr};
+        const Rows r = need_rows(fields[3 * f], fields[3 * f + 1], fields[3 * f + 2], luts[f], fields[0]);
+        TORCH_CHECK(r.n_rows == (size_t)fields[2].numel(), "bnpk: fields differ in entry count");
+        out[f] = bnpk_field{r.base, r.base_bytes, r.starts, r.lens, r.lut};
     }
     return out;
 }
@@ -274,12 +296,12 @@ Tensor format_records(int64_t format, int64_t line_width, const std::vector<Tens
                       const std::vector<c10::optional<Tensor>> &luts, const Tensor &offsets, int64_t out_begin,
                       int64_t out_end) {
     std::vector<bnpk_field> f = make_fields(fields, luts);
-    need(offsets, torch::kInt64, "offsets");
+    const int64_t *offs = need_offsets(offsets, (size_t)fields[2].numel(), fields[0]);
     TORCH_CHECK(out_end >= out_begin, "bnpk: out_end < out_begin");
     c10::cuda::CUDAGuard guard(fields[0].device());
     Tensor out = torch::empty({out_end - out_begin}, fields[0].options().dtype(torch::kUInt8));
     check(bnpk_format_records((int)format, (int)line_width, (size_t)fields[2].numel(), f.data(),
-                              offsets.data_ptr<int64_t>(), out_begin, out_end, out.numel() ? out.data_ptr<uint8_t>() : nullptr,
+                              offs, out_begin, out_end, out.numel() ? out.data_ptr<uint8_t>() : nullptr,
                               cur_stream(fields[0])),
           "format_records");
     return out;

@@ -341,8 +341,7 @@ int fill_args(FmtArgs &a, int format, int line_width, size_t n_entries, const bn
 }
 
 unsigned fmt_grid(int64_t span_bytes) {
-    const int64_t tiles = (span_bytes + kFmtTile - 1) / kFmtTile;
-    return (unsigned)std::max<int64_t>(1, std::min<int64_t>(tiles, (int64_t)sm_count() * 8));
+    return grid_cap((size_t)((span_bytes + kFmtTile - 1) / kFmtTile), 8);
 }
 
 }  // namespace
@@ -365,7 +364,7 @@ int bnpk_format_offsets(int format, int line_width, size_t n_entries, const bnpk
     const size_t need = (kWsHeaderWords + n_tiles) * sizeof(uint64_t);
     if (workspace_bytes < need) return set_err(BNPK_E_WORKSPACE, "workspace too small");
     BNPK_CUDA(cudaMemsetAsync(workspace, 0, need, st));
-    const unsigned grid = (unsigned)std::min<size_t>(n_tiles, (size_t)sm_count() * 4);
+    const unsigned grid = grid_cap(n_tiles, 4);
     format_offsets_kernel<<<grid, kOffThreads, 0, st>>>(a, out_offsets, (uint64_t *)workspace);
     BNPK_LAUNCHED("format_offsets_kernel");
     if (!a.lut[1]) return 0;                 // raw text: every byte is written as it is

@@ -152,6 +152,8 @@ def _rows_args(base, starts, lens):
     _need_cuda(lens, "lens")
     if base.dtype != torch.uint8 or starts.dtype != torch.int64 or lens.dtype != torch.int32:
         raise TypeError("base must be uint8, starts int64, lens int32")
+    if starts.numel() != lens.numel():
+        raise ValueError("starts and lens differ in length")
     return ptr(base), base.numel(), ptr(starts), ptr(lens), lens.numel()
 
 
@@ -422,23 +424,18 @@ def _format_fields(fields):
         if f is None:
             continue
         base, starts, lens, lut = f
-        _need_cuda(base, "base")
-        _need_cuda(starts, "starts")
-        _need_cuda(lens, "lens")
-        if base.dtype != torch.uint8 or starts.dtype != torch.int64 or lens.dtype != torch.int32:
-            raise TypeError("base must be uint8, starts int64, lens int32")
+        base_p, base_bytes, starts_p, lens_p, rows = _rows_args(base, starts, lens)
         if lut is not None:
             _need_cuda(lut, "lut")
             if lut.dtype != torch.uint8 or lut.numel() != 256:
                 raise TypeError("lut must be 256 uint8")
         if n is None:
-            n, dev = lens.numel(), base.device
-        if lens.numel() != n or starts.numel() != n:
+            n, dev = rows, base.device
+        if rows != n:
             raise ValueError("every field needs one row per entry")
         if any(t.device != dev for t in (base, starts, lens) + ((lut,) if lut is not None else ())):
             raise ValueError("the fields are on different devices")
-        arr[i] = nv.Field(base.data_ptr() or None, base.numel(), starts.data_ptr() or None, lens.data_ptr() or None,
-                          lut.data_ptr() if lut is not None else None)
+        arr[i] = nv.Field(base_p.value, base_bytes, starts_p.value, lens_p.value, lut.data_ptr() if lut is not None else None)
     return arr, n or 0, dev
 
 

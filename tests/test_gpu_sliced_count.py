@@ -483,8 +483,8 @@ def test_chunk_count_rejects_bad_arguments_before_touching_memory():
     n = 100000
     ws_bytes = int(lib.bnpk_tile_workspace_bytes(n))
 
-    def call(n=n, b=0, e=n, lpe=4, k=31, window=0, ws=ws_bytes):
-        return lib.bnpk_chunk_kmer_count(None, n, b, e, 1, lpe, ord("@"), 1, -1, ENC_ACGT, None, k, window, 1 << 14,
+    def call(n=n, b=0, e=n, lpe=4, k=31, window=0, ws=ws_bytes, enc=ENC_ACGT):
+        return lib.bnpk_chunk_kmer_count(None, n, b, e, 1, lpe, ord("@"), 1, -1, enc, None, k, window, 1 << 14,
                                          HIST_AUTO, None, None, None, ws, None)
 
     assert call(e=n + 1) == nv.E_BADARG                       # slice_end > n
@@ -493,4 +493,6 @@ def test_chunk_count_rejects_bad_arguments_before_touching_memory():
     assert call(ws=ws_bytes - 1) == nv.E_WORKSPACE
     assert call(k=21, window=20) == nv.E_WINDOW
     assert call(k=32) == nv.E_K
+    assert call(enc=-1) == call(enc=4) == nv.E_BADARG
+    assert call(enc=nv.ENC_LUT) == nv.E_BADARG                # without lut256
     assert call(n=0, e=0, ws=int(lib.bnpk_tile_workspace_bytes(0))) == 0     # an empty chunk does nothing
