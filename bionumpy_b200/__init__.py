@@ -14,17 +14,18 @@ from .encoded_array import (EncodedArray, EncodedRaggedArray, as_encoded_array, 
                             from_encoded_array, EncodingException)
 from .ragged import RaggedArray, RaggedShape
 from .encodings import (AlphabetEncoding, DNAEncoding, ACTGEncoding, ACGTEncoding, KmerEncoding, EncodingError,
-                        AminoAcidEncoding, RNAENcoding)
+                        AminoAcidEncoding, RNAENcoding, StrandEncoding)
 from . import encodings, sequence, io, streams
 from .sequence import (get_kmers, get_minimizers, count_encoded, count_kmers, count_hashed, count_kmers_hashed,
                        EncodedCounts, complement, get_reverse_complement, get_motif_scores, match_string)
 from .streams import streamable, bincount, BnpStream
-from .io import bnp_open, FormatException, IndexedFasta
+from .io import bnp_open, FormatException, IndexedFasta, open_indexed
 from .sequence import KmerIndex, KmerLookup, BloomFilter
 from .sequence import count_kmers_exact, KmerCounter, KmerCounts
 from .io.buffers import CudaFastQBuffer, CudaTwoLineFastaBuffer, FastQBuffer, TwoLineFastaBuffer
 from .io.multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
-from .datatypes import SequenceEntry, SequenceEntryWithQuality, replace
+from .datatypes import SequenceEntry, SequenceEntryWithQuality, Interval, StrandedInterval, Bed6, replace
+from . import datatypes
 from .io.files import count_entries
 from .io.write import NpBufferedWriter
 

@@ -21,6 +21,9 @@ E_BADARG, E_K, E_WINDOW, E_WORKSPACE, E_BINS = -1, -2, -3, -4, -5
  ST_TABLE_FULL) = range(14)
 ST_WORDS = 16
 FMT_FASTQ, FMT_FASTA, FMT_FASTA_WRAPPED = 0, 1, 2
+MAX_COLUMNS = 16
+COL_SKIP, COL_TEXT, COL_INT, COL_INT_OR_DOT, COL_STRAND = 0, 1, 2, 3, 4
+BAD_TABS, BAD_COLUMNS, BAD_INT, BAD_STRAND = 1, 2, 3, 4
 INT64_MAX = (1 << 63) - 1
 SMEM_MAX_BINS = 32768
 
@@ -71,12 +74,21 @@ SIGNATURES = {
     "bnpk_synth_fastq": (_i, [_vp, _u64, _u64, _u64, _vp]),
     "bnpk_format_offsets": (_i, [_i, _i, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "bnpk_format_records": (_i, [_i, _i, _sz, _vp, _vp, _i64, _i64, _vp, _vp]),
+    "bnpk_delimited_columns": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _i, _vp, _vp]),
+    "bnpk_name_lookup": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "bnpk_interval_gather": (_i, [_vp, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                  _vp]),
 }
 
 
 class Field(ctypes.Structure):
     """bnpk_field: a ragged view (base, starts, lens) and an optional device LUT applied on the way out."""
     _fields_ = [("base", _vp), ("base_bytes", _sz), ("starts", _vp), ("lens", _vp), ("lut256", _vp)]
+
+
+class Column(ctypes.Structure):
+    """bnpk_column: how one tab-separated column is written (COL_*), its output and, for text, its lengths."""
+    _fields_ = [("kind", _i), ("out", _vp), ("lens", _vp)]
 
 
 class NativeLibraryError(RuntimeError):

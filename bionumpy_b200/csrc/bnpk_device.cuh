@@ -48,6 +48,30 @@ __device__ __forceinline__ uint4 ld_stream(const uint4 *p) {
                  : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
     return r;
 }
+// 16 bytes from an arbitrary address, as two aligned 16-byte loads and a funnel shift (both loads touch only the
+// aligned blocks that hold bytes of [p, p + 16), so they stay inside the allocation)
+__device__ __forceinline__ void load16(const uint8_t *p, uint32_t (&o)[4]) {
+    const uintptr_t addr = reinterpret_cast<uintptr_t>(p);
+    const uint4 *q = reinterpret_cast<const uint4 *>(addr & ~(uintptr_t)15);
+    const int s = (int)(addr & 15);
+    const uint4 lo = __ldg(q);
+    if (s == 0) {
+        o[0] = lo.x; o[1] = lo.y; o[2] = lo.z; o[3] = lo.w;
+        return;
+    }
+    const uint4 hi = __ldg(q + 1);
+    const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    const int k = s >> 2, sh = (s & 3) * 8;
+    uint32_t t[5];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+        const uint32_t c0 = w[j], c1 = j + 1 < 8 ? w[j + 1] : 0u, c2 = j + 2 < 8 ? w[j + 2] : 0u,
+                       c3 = j + 3 < 8 ? w[j + 3] : 0u;
+        t[j] = k == 0 ? c0 : k == 1 ? c1 : k == 2 ? c2 : c3;
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) o[j] = __funnelshift_r(t[j], t[j + 1], sh);
+}
 
 __device__ __forceinline__ uint64_t warp_sum_u64(uint64_t v) {
 #pragma unroll

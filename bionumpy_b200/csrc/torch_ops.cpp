@@ -307,6 +307,119 @@ Tensor format_records(int64_t format, int64_t line_width, const std::vector<Tens
     return out;
 }
 
+// BED columns: per column of `kinds` (BNPK_COL_*) a value tensor (int64 text starts / int64 values / uint8 strand codes,
+// empty for a skipped column) and a lens tensor (int32 for text, else empty); and the status block
+std::tuple<std::vector<Tensor>, std::vector<Tensor>, Tensor> delimited_columns(const Tensor &chunk, const Tensor &starts,
+                                                                               const Tensor &lens, c10::IntArrayRef kinds) {
+    const Rows r = need_rows(chunk, starts, lens, c10::nullopt);
+    TORCH_CHECK(!kinds.empty() && kinds.size() <= BNPK_MAX_COLUMNS, "bnpk: 1 to BNPK_MAX_COLUMNS columns");
+    c10::cuda::CUDAGuard guard(chunk.device());
+    const int64_t n = (int64_t)r.n_rows;
+    std::vector<Tensor> values, text_lens;
+    std::vector<bnpk_column> cols(kinds.size());
+    for (size_t c = 0; c < kinds.size(); ++c) {
+        const int64_t k = kinds[c];
+        const bool named = k == BNPK_COL_TEXT || k == BNPK_COL_INT || k == BNPK_COL_INT_OR_DOT || k == BNPK_COL_STRAND;
+        values.push_back(torch::empty({named ? n : 0}, chunk.options().dtype(k == BNPK_COL_STRAND ? torch::kUInt8 : torch::kInt64)));
+        text_lens.push_back(torch::empty({k == BNPK_COL_TEXT ? n : 0}, chunk.options().dtype(torch::kInt32)));
+        cols[c] = bnpk_column{(int)k, named ? values.back().data_ptr() : nullptr,
+                              k == BNPK_COL_TEXT ? text_lens.back().data_ptr<int32_t>() : nullptr};
+    }
+    Tensor status = new_status(chunk);
+    check(bnpk_delimited_columns(r.base, r.base_bytes, r.starts, r.lens, r.n_rows, cols.data(), (int)cols.size(),
+                                 status.data_ptr<int64_t>(), cur_stream(chunk)),
+          "delimited_columns");
+    return {values, text_lens, status};
+}
+
+// contig index of every row's name in the sorted table (names, name_offsets int64[C+1]), -1 = unknown; and status
+std::tuple<Tensor, Tensor> name_lookup(const Tensor &base, const Tensor &starts, const Tensor &lens, const Tensor &names,
+                                       const Tensor &name_offsets) {
+    const Rows r = need_rows(base, starts, lens, c10::nullopt);
+    need(names, torch::kUInt8, "names", base);
+    need(name_offsets, torch::kInt64, "name_offsets", base);
+    TORCH_CHECK(name_offsets.numel() >= 1, "bnpk: name_offsets needs C + 1 entries");
+    c10::cuda::CUDAGuard guard(base.device());
+    Tensor ids = torch::empty({(int64_t)r.n_rows}, base.options().dtype(torch::kInt32));
+    Tensor status = new_status(base);
+    check(bnpk_name_lookup(r.base, r.base_bytes, r.starts, r.lens, r.n_rows, u8(names), name_offsets.data_ptr<int64_t>(),
+                           (size_t)name_offsets.numel() - 1, ids.data_ptr<int32_t>(), status.data_ptr<int64_t>(),
+                           cur_stream(base)),
+          "name_lookup");
+    return {ids, status};
+}
+
+// interval gather over a file image: ids (int32) index contigs = [offset int64, lenc int32, lenb int32, length int64];
+// no ids = one flat contig.  check: (row_lens int32, status); copy: uint8[total] at offsets (int64[R+1])
+struct Intervals {
+    const int32_t *ids = nullptr;
+    const int64_t *offset = nullptr, *length = nullptr;
+    const int32_t *lenc = nullptr, *lenb = nullptr;
+    size_t n_contigs = 0;
+};
+Intervals need_intervals(const Tensor &file, const Tensor &start, const Tensor &stop, const c10::optional<Tensor> &ids,
+                         const std::vector<Tensor> &contigs) {
+    need(file, torch::kUInt8, "file");
+    need(start, torch::kInt64, "start", file);
+    need(stop, torch::kInt64, "stop", file);
+    TORCH_CHECK(start.numel() == stop.numel(), "bnpk: start and stop differ in length");
+    Intervals iv;
+    if (!ids) return iv;
+    need(*ids, torch::kInt32, "ids", file);
+    TORCH_CHECK(ids->numel() == start.numel(), "bnpk: one contig id per interval");
+    TORCH_CHECK(contigs.size() == 4, "bnpk: contigs are [offset, lenc, lenb, length]");
+    need(contigs[0], torch::kInt64, "contig_offset", file);
+    need(contigs[1], torch::kInt32, "lenc", file);
+    need(contigs[2], torch::kInt32, "lenb", file);
+    need(contigs[3], torch::kInt64, "contig_len", file);
+    const int64_t c = contigs[0].numel();
+    TORCH_CHECK(contigs[1].numel() == c && contigs[2].numel() == c && contigs[3].numel() == c,
+                "bnpk: the contig columns differ in length");
+    iv.ids = ids->data_ptr<int32_t>();
+    iv.offset = contigs[0].data_ptr<int64_t>();
+    iv.lenc = contigs[1].data_ptr<int32_t>();
+    iv.lenb = contigs[2].data_ptr<int32_t>();
+    iv.length = contigs[3].data_ptr<int64_t>();
+    iv.n_contigs = (size_t)c;
+    return iv;
+}
+
+std::tuple<Tensor, Tensor> interval_check(const Tensor &file, const Tensor &start, const Tensor &stop,
+                                          const c10::optional<Tensor> &ids, const std::vector<Tensor> &contigs) {
+    const Intervals iv = need_intervals(file, start, stop, ids, contigs);
+    c10::cuda::CUDAGuard guard(file.device());
+    Tensor row_lens = torch::empty({start.numel()}, file.options().dtype(torch::kInt32));
+    Tensor status = new_status(file);
+    check(bnpk_interval_gather(u8(file), (size_t)file.numel(), (size_t)start.numel(), iv.ids, iv.offset, iv.lenc, iv.lenb,
+                               iv.length, iv.n_contigs, start.data_ptr<int64_t>(), stop.data_ptr<int64_t>(), nullptr,
+                               nullptr, row_lens.data_ptr<int32_t>(), nullptr, nullptr, status.data_ptr<int64_t>(),
+                               cur_stream(file)),
+          "interval_check");
+    return {row_lens, status};
+}
+
+Tensor interval_copy(const Tensor &file, const Tensor &start, const Tensor &stop, const c10::optional<Tensor> &ids,
+                     const std::vector<Tensor> &contigs, const c10::optional<Tensor> &strand,
+                     const c10::optional<Tensor> &complement_lut, const Tensor &offsets, int64_t total) {
+    const Intervals iv = need_intervals(file, start, stop, ids, contigs);
+    const int64_t *offs = need_offsets(offsets, (size_t)start.numel(), file);
+    const uint8_t *s = nullptr;
+    if (strand) {
+        need(*strand, torch::kUInt8, "strand", file);
+        TORCH_CHECK(strand->numel() == start.numel(), "bnpk: one strand flag per interval");
+        s = strand->data_ptr<uint8_t>();
+    }
+    const uint8_t *lut = need_lut(complement_lut, "complement_lut", file);
+    c10::cuda::CUDAGuard guard(file.device());
+    Tensor out = torch::empty({total}, file.options());
+    if (total)
+        check(bnpk_interval_gather(u8(file), (size_t)file.numel(), (size_t)start.numel(), iv.ids, iv.offset, iv.lenc,
+                                   iv.lenb, iv.length, iv.n_contigs, start.data_ptr<int64_t>(), stop.data_ptr<int64_t>(),
+                                   s, lut, nullptr, offs, out.data_ptr<uint8_t>(), nullptr, cur_stream(file)),
+              "interval_copy");
+    return out;
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bnpk, m) {
@@ -333,6 +446,11 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("format_offsets(int format, int line_width, Tensor[] fields, Tensor?[] luts) -> (Tensor, Tensor)");
     m.def("format_records(int format, int line_width, Tensor[] fields, Tensor?[] luts, Tensor offsets, int out_begin, "
           "int out_end) -> Tensor");
+    m.def("delimited_columns(Tensor chunk, Tensor starts, Tensor lens, int[] kinds) -> (Tensor[], Tensor[], Tensor)");
+    m.def("name_lookup(Tensor base, Tensor starts, Tensor lens, Tensor names, Tensor name_offsets) -> (Tensor, Tensor)");
+    m.def("interval_check(Tensor file, Tensor start, Tensor stop, Tensor? ids, Tensor[] contigs) -> (Tensor, Tensor)");
+    m.def("interval_copy(Tensor file, Tensor start, Tensor stop, Tensor? ids, Tensor[] contigs, Tensor? strand, "
+          "Tensor? complement_lut, Tensor offsets, int total) -> Tensor");
 }
 
 TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
@@ -349,4 +467,8 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("bincount", &bincount);
     m.impl("format_offsets", &format_offsets);
     m.impl("format_records", &format_records);
+    m.impl("delimited_columns", &delimited_columns);
+    m.impl("name_lookup", &name_lookup);
+    m.impl("interval_check", &interval_check);
+    m.impl("interval_copy", &interval_copy);
 }

@@ -73,3 +73,61 @@ class SequenceEntry(_Entries):
 
 class SequenceEntryWithQuality(_Entries):
     _fields = ("name", "sequence", "quality")
+
+
+def _interval_field(field, value):
+    """Interval and Bed6 fields: text columns (chromosome, name) as text, integer columns (start, stop, score) as int64
+    CUDA tensors and strand as StrandEncoding codes."""
+    if field in ("chromosome", "name"):
+        return _from_strings(field, value)
+    from . import config
+    if field == "strand":
+        from .encoded_array import EncodedArray
+        from .encodings import StrandEncoding
+        if isinstance(value, EncodedArray):
+            return value
+        if isinstance(value, str):
+            value = list(value)
+        codes = np.array(["+-.".index(v) for v in value], dtype=np.uint8)
+        return EncodedArray(torch.from_numpy(codes).to(config.default_device()), StrandEncoding)
+    if isinstance(value, torch.Tensor):
+        return value
+    if field == "score" and isinstance(value, list):
+        value = [0 if v == "." else int(v) for v in value]        # Optional[int]: "." is 0 (io/strops.py:69-83)
+    return torch.as_tensor(np.asarray(value, dtype=np.int64)).to(config.default_device())
+
+
+class _IntervalEntries(_Entries):
+    """Records whose fields can be assigned (``peaks.start = mid - 50``), as the reference's dataclasses allow."""
+
+    def __init__(self, *values, buffer=None):
+        super().__init__(buffer=buffer)
+        for f, v in zip(self._fields, values):
+            self._values[f] = _interval_field(f, v)
+
+    def __setattr__(self, name, value):
+        if name in self._fields:
+            self._values[name] = _interval_field(name, value)
+        else:
+            super().__setattr__(name, value)
+
+    @classmethod
+    def from_entry_tuples(cls, tuples):
+        """bnpdataclass.from_entry_tuples: one tuple per entry."""
+        columns = list(zip(*tuples)) if len(tuples) else [[] for _ in cls._fields]
+        return cls(*[list(c) for c in columns])
+
+
+class Interval(_IntervalEntries):
+    """datatypes/__init__.py:51-54: chromosome, start, stop (0-based, end-exclusive)."""
+    _fields = ("chromosome", "start", "stop")
+
+
+class StrandedInterval(_IntervalEntries):
+    """datatypes/__init__.py:57-59: Interval + strand."""
+    _fields = ("chromosome", "start", "stop", "strand")
+
+
+class Bed6(_IntervalEntries):
+    """datatypes/__init__.py:67-70: Interval + name, score (Optional[int]) and strand."""
+    _fields = ("chromosome", "start", "stop", "name", "score", "strand")

@@ -1,5 +1,5 @@
 from ..encoded_array import BaseEncoding, Encoding, OneToOneEncoding, ASCIIEncoding
 from .alphabet_encoding import (AlphabetEncoding, ACTGEncoding, ACGTEncoding, DNAEncoding, ACUGEncoding,
-                                RNAENcoding, AminoAcidEncoding)
+                                RNAENcoding, AminoAcidEncoding, StrandEncoding)
 from .kmer_encodings import KmerEncoding
 from .exceptions import EncodingError

@@ -100,3 +100,4 @@ DNAEncoding = ACGTEncoding
 ACUGEncoding = AlphabetEncoding("ACUG")
 RNAENcoding = ACUGEncoding
 AminoAcidEncoding = AlphabetEncoding('ACDEFGHIKLMNPQRSTVWY*')
+StrandEncoding = AlphabetEncoding("+-.")      # alphabet_encoding.py:120: '+' 0, '-' 1, '.' 2

@@ -6,5 +6,6 @@ from .bgzf import BgzfWriter
 from .write import NpBufferedWriter
 from .parser import CudaFileReader, NpDataclassReader
 from .multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
-from .indexed_fasta import IndexedFasta, read_index, create_index
+from .indexed_fasta import IndexedFasta, read_index, create_index, open_indexed
+from .delimited import DelimitedBuffer, BedBuffer, Bed6Buffer
 from .motifs import read_motif

@@ -25,8 +25,11 @@ def _buffer_type_for(suffix):
         return buffer_types[suffix]
     if suffix in (".fa", ".fasta", ".fna", ".faa"):
         return _multiline()
-    raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA k-mer path "
-                       f"(supported: .fq .fastq .fa .fasta and their .gz forms); pass buffer_type=")
+    if suffix == ".bed":
+        from .delimited import BedBuffer
+        return BedBuffer
+    raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
+                       f"(supported: .fq .fastq .fa .fasta .bed and their .gz forms); pass buffer_type=")
 
 
 def _suffix(path):
@@ -47,6 +50,9 @@ def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
     if buffer_type is None:
         buffer_type = _buffer_type_for(suffix)
     if mode in WRITE_MODES:
+        from .delimited import DelimitedBuffer
+        if isinstance(buffer_type, type) and issubclass(buffer_type, DelimitedBuffer):
+            raise NotImplementedError(f"writing {suffix} files is not supported")
         from .write import NpBufferedWriter
         raw = open(path, WRITE_MODES[mode])
         if is_gzip:

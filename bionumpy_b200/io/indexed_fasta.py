@@ -14,6 +14,7 @@ import torch
 from .. import _native as nv
 from .. import config, ops
 from ..encoded_array import EncodedArray, EncodedRaggedArray, BaseEncoding
+from ..rows import RowView
 
 
 def read_index(filename) -> dict:
@@ -109,9 +110,29 @@ class IndexedFasta:
         out, _ = self._gather([chromosome], [0], [self._index[chromosome]["rlen"]])
         return EncodedArray(out, BaseEncoding)
 
+    def _name_table(self):
+        """The contig names sorted as bytes, concatenated on the device with their offsets, and each contig's
+        (offset, lenc, lenb, length) in that order: built once, for bnpk_name_lookup and bnpk_interval_gather."""
+        if getattr(self, "_table", None) is None:
+            dev = self._file.device
+            names = sorted(self._index, key=lambda n: n.encode())
+            raw = [n.encode() for n in names]
+            ends = np.cumsum([0] + [len(b) for b in raw]).astype(np.int64)
+            idx = [self._index[n] for n in names]
+            t = lambda v, dt: torch.tensor(v, dtype=dt, device=dev)
+            text = torch.frombuffer(bytearray(b"".join(raw) or b"\0"), dtype=torch.uint8).to(dev)
+            contigs = (t([i["offset"] for i in idx], torch.int64), t([i["lenc"] for i in idx], torch.int32),
+                       t([i["lenb"] for i in idx], torch.int32), t([i["rlen"] for i in idx], torch.int64))
+            self._table = (names, text, torch.from_numpy(ends).to(dev), contigs)
+        return self._table
+
     def get_interval_sequences(self, intervals) -> EncodedRaggedArray:
         """indexed_fasta.py:165-206: ``intervals`` has .chromosome (names), .start, .stop (or is an iterable of
-        (chromosome, start, stop))."""
+        (chromosome, start, stop)).  Intervals on the device (an Interval or Bed6 chunk) are looked up and gathered
+        on the device with one synchronisation, for the output size; an interval outside its contig raises
+        ValueError and an unknown chromosome KeyError."""
+        if _on_device(intervals):
+            return self._device_interval_sequences(intervals)
         if hasattr(intervals, "chromosome"):
             names = [c if isinstance(c, str) else c.to_string() for c in intervals.chromosome]
             starts = [int(x) for x in intervals.start]
@@ -121,3 +142,35 @@ class IndexedFasta:
         lens = [b - a for a, b in zip(starts, stops)]
         out, row_len = self._gather(list(names), list(starts), lens)
         return EncodedRaggedArray(EncodedArray(out, BaseEncoding), row_len.to(torch.int32))
+
+    def _device_interval_sequences(self, intervals):
+        names, text, name_offsets, contigs = self._name_table()
+        rows = RowView(intervals.chromosome)
+        start, stop = intervals.start.to(torch.int64).contiguous(), intervals.stop.to(torch.int64).contiguous()
+        ids, st_names = ops.name_lookup(rows.base, rows.starts, rows.lens, text, name_offsets)
+        row_lens, st_rows = ops.interval_check(self._file, start, stop, ids, contigs)
+        offsets = ops.row_offsets(row_lens)
+        total, bad_name, bad_row = (int(x) for x in torch.cat(
+            [offsets[-1:], st_names[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1], st_rows[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]
+        ).cpu().tolist())
+        if bad_name != nv.INT64_MAX:
+            raise KeyError(intervals.chromosome[bad_name].to_string())
+        if bad_row != nv.INT64_MAX:
+            name = intervals.chromosome[bad_row].to_string()
+            raise ValueError(f"interval {bad_row} ({name}:{int(start[bad_row])}-{int(stop[bad_row])}) is not inside "
+                             f"the contig ({self._index[name]['rlen']} bases)")
+        out = ops.interval_copy(self._file, start, stop, offsets, total, ids, contigs)
+        return EncodedRaggedArray(EncodedArray(out, BaseEncoding), row_lens)
+
+
+def _on_device(intervals):
+    """Whether ``intervals`` is a record chunk whose chromosome, start and stop already live on the device."""
+    chrom = getattr(intervals, "chromosome", None)
+    start, stop = getattr(intervals, "start", None), getattr(intervals, "stop", None)
+    return (isinstance(chrom, EncodedRaggedArray) and chrom.device.type == "cuda" and
+            all(isinstance(t, torch.Tensor) and t.is_cuda for t in (start, stop)))
+
+
+def open_indexed(filename) -> IndexedFasta:
+    """io/indexed_files.py:16-37: an IndexedFasta of ``filename`` (its .fai next to it, else built)."""
+    return IndexedFasta(filename)

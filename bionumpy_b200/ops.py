@@ -470,3 +470,102 @@ def format_records(fmt, line_width, fields, offsets, out_begin=0, out_end=None, 
     check(lib().bnpk_format_records(fmt, line_width, n, ctypes.cast(arr, ctypes.c_void_p), ptr(offsets), out_begin,
                                     out_end, ptr(out) if out.numel() else None, stream_ptr()))
     return out
+
+
+@_on_device
+def delimited_columns(chunk, starts, lens, kinds, status=None):
+    """The tab-separated columns of the lines (starts, lens) of ``chunk``, one nv.COL_* kind per column.  Returns
+    (columns, status): per column None (COL_SKIP), (starts int64, lens int32) of text, int64 values or uint8 strand
+    codes; the first fault is (line << 8 | column << 3 | nv.BAD_*) in status[ST_BAD_BASE]."""
+    _rows_args(chunk, starts, lens)
+    n, dev = lens.numel(), chunk.device
+    if not 1 <= len(kinds) <= nv.MAX_COLUMNS:
+        raise ValueError(f"1 to {nv.MAX_COLUMNS} columns")
+    arr = (nv.Column * len(kinds))()
+    cols = []
+    for i, kind in enumerate(kinds):
+        if kind == nv.COL_TEXT:
+            col = (torch.empty(n, dtype=torch.int64, device=dev), torch.empty(n, dtype=torch.int32, device=dev))
+            arr[i] = nv.Column(kind, col[0].data_ptr(), col[1].data_ptr())
+        elif kind in (nv.COL_INT, nv.COL_INT_OR_DOT, nv.COL_STRAND):
+            col = torch.empty(n, dtype=torch.uint8 if kind == nv.COL_STRAND else torch.int64, device=dev)
+            arr[i] = nv.Column(kind, col.data_ptr(), None)
+        else:
+            col = None
+            arr[i] = nv.Column(kind, None, None)
+        cols.append(col)
+    if status is None:
+        status = nv.new_status(dev)
+    check(lib().bnpk_delimited_columns(ptr(chunk), chunk.numel(), ptr(starts), ptr(lens), n,
+                                       ctypes.cast(arr, ctypes.c_void_p), len(kinds), ptr(status), stream_ptr()))
+    return cols, status
+
+
+@_on_device
+def name_lookup(base, starts, lens, names, name_offsets, status=None):
+    """The index of each row's bytes in the sorted name table (names uint8, name_offsets int64[C+1]): int32, -1 for an
+    unknown name, whose row is reported in status[ST_BAD_BASE].  Returns (ids, status)."""
+    base_p, base_bytes, starts_p, lens_p, n = _rows_args(base, starts, lens)
+    _need_cuda(names, "names")
+    _need_cuda(name_offsets, "name_offsets")
+    if names.dtype != torch.uint8 or name_offsets.dtype != torch.int64:
+        raise TypeError("names must be uint8 and name_offsets int64")
+    ids = torch.empty(n, dtype=torch.int32, device=base.device)
+    if status is None:
+        status = nv.new_status(base.device)
+    check(lib().bnpk_name_lookup(base_p, base_bytes, starts_p, lens_p, n, ptr(names), ptr(name_offsets),
+                                 name_offsets.numel() - 1, ptr(ids), ptr(status), stream_ptr()))
+    return ids, status
+
+
+def _interval_args(file, start, stop, ids, contigs):
+    _need_cuda(file, "file")
+    for t, name in ((start, "start"), (stop, "stop")):
+        _need_cuda(t, name)
+        if t.dtype != torch.int64:
+            raise TypeError(f"{name} must be int64")
+    if start.numel() != stop.numel() or (ids is not None and ids.numel() != start.numel()):
+        raise ValueError("start, stop and ids differ in length")
+    if ids is None:
+        return [ptr(file), file.numel(), start.numel(), None, None, None, None, None, 0, ptr(start), ptr(stop)]
+    offset, lenc, lenb, length = contigs
+    for t, name, dt in ((ids, "ids", torch.int32), (offset, "contig_offset", torch.int64), (lenc, "lenc", torch.int32),
+                        (lenb, "lenb", torch.int32), (length, "contig_len", torch.int64)):
+        _need_cuda(t, name)
+        if t.dtype != dt:
+            raise TypeError(f"{name} must be {dt}")
+    return [ptr(file), file.numel(), start.numel(), ptr(ids), ptr(offset), ptr(lenc), ptr(lenb), ptr(length),
+            offset.numel(), ptr(start), ptr(stop)]
+
+
+@_on_device
+def interval_check(file, start, stop, ids=None, contigs=None, status=None):
+    """The check pass of bnpk_interval_gather: (row_lens int32 = stop - start, 0 for a bad row; status with the first
+    bad row in ST_BAD_BASE).  ``contigs`` = (offset int64, lenc int32, lenb int32, length int64) indexed by ``ids``
+    (int32); without ids the file is one contig without line ends."""
+    args = _interval_args(file, start, stop, ids, contigs)
+    row_lens = torch.empty(start.numel(), dtype=torch.int32, device=file.device)
+    if status is None:
+        status = nv.new_status(file.device)
+    check(lib().bnpk_interval_gather(*args, None, None, ptr(row_lens), None, None, ptr(status), stream_ptr()))
+    return row_lens, status
+
+
+@_on_device
+def interval_copy(file, start, stop, offsets, total, ids=None, contigs=None, strand=None, complement_lut=None):
+    """The copy pass: uint8[total], row r at offsets[r] (int64[R+1] of interval_check's row_lens), a row whose
+    strand[r] (uint8) is not 0 reverse-complemented through ``complement_lut`` (uint8[256])."""
+    args = _interval_args(file, start, stop, ids, contigs)
+    _need_cuda(offsets, "offsets")
+    if offsets.dtype != torch.int64 or offsets.numel() != start.numel() + 1:
+        raise ValueError("offsets must be int64[R+1]")
+    if strand is not None:
+        _need_cuda(strand, "strand")
+        _need_cuda(complement_lut, "complement_lut")
+        if strand.dtype != torch.uint8 or strand.numel() != start.numel() or complement_lut.numel() != 256:
+            raise ValueError("strand must be uint8[R] and complement_lut uint8[256]")
+    out = torch.empty(total, dtype=torch.uint8, device=file.device)
+    if total:
+        check(lib().bnpk_interval_gather(*args, ptr(strand), ptr(complement_lut), None, ptr(offsets), ptr(out), None,
+                                         stream_ptr()))
+    return out

@@ -292,10 +292,17 @@ class RaggedArray:
         raise NotImplementedError(axis)
 
     def mean(self, axis=None, **kwargs):
-        """np.mean in float64: axis=-1 gives one value per row, NaN for an empty row."""
+        """np.mean in float64: axis=-1 gives one value per row, NaN for an empty row; axis=0 one value per column when
+        every row has the same length."""
         flat = self.ravel().to(torch.float64)
         if axis is None:
             return flat.mean()
+        if axis == 0:
+            n = len(self)
+            width = int(self._lens[0].item()) if n else 0
+            if n == 0 or bool((self._lens != width).any().item()):
+                raise NotImplementedError("mean(axis=0) needs rows of one length")
+            return flat.reshape(n, width).mean(0)
         if axis in (-1, 1):
             out = torch.zeros(len(self), dtype=torch.float64, device=flat.device)
             return out.index_add_(0, self._row_index(), flat) / self._lens.to(torch.float64)

@@ -76,6 +76,47 @@ def get_reverse_complement(sequence):
     return EncodedRaggedArray(EncodedArray(out, sequence.encoding), rows.lens)
 
 
+def _interval_sequences(sequence, intervals, stranded):
+    """sequence[intervals.start:intervals.stop] row by row (dna.py:68-106), a '-' row reverse-complemented when
+    ``stranded``: bnpk_interval_gather in flat mode, one synchronisation for the output size."""
+    sequence = as_encoded_array(sequence)
+    assert isinstance(sequence, EncodedArray) and sequence.ndim == 1, "intervals index one 1-D sequence"
+    raw = sequence.raw()
+    if not raw.is_cuda:
+        raise nv.NativeLibraryError("interval sequences need a CUDA tensor: bionumpy_b200 has no CPU fallback")
+    raw = raw.to(torch.uint8).contiguous()
+    start, stop = (torch.as_tensor(v).to(raw.device, torch.int64).contiguous() for v in (intervals.start, intervals.stop))
+    row_lens, status = ops.interval_check(raw, start, stop)
+    offsets = ops.row_offsets(row_lens)
+    total, bad = (int(x) for x in torch.cat([offsets[-1:], status[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]).cpu().tolist())
+    if bad != nv.INT64_MAX:
+        raise ValueError(f"interval {bad} ({int(start[bad])}-{int(stop[bad])}) is not inside the sequence "
+                         f"({raw.numel()} bases)")
+    strand = lut = None
+    if stranded:
+        from ..encodings import StrandEncoding
+        s = intervals.strand
+        minus = 1 if getattr(s, "encoding", None) == StrandEncoding else ord("-")
+        strand = (torch.as_tensor(s.raw() if hasattr(s, "raw") else s).reshape(-1).to(raw.device) == minus)
+        strand = strand.to(torch.uint8).contiguous()
+        lut = _device_table(sequence.encoding, raw.device)
+    out = ops.interval_copy(raw, start, stop, offsets, total, strand=strand, complement_lut=lut)
+    return EncodedRaggedArray(EncodedArray(out, sequence.encoding), row_lens)
+
+
+@streamable()
+def get_strand_specific_sequences(encoded_array, stranded_intervals) -> EncodedRaggedArray:
+    """dna.py:68-88: the sequence of every interval, reverse-complemented where its strand is '-' (the complement of
+    the sequence's encoding: for ASCII text A, C, G, T, N, every other byte 0)."""
+    return _interval_sequences(encoded_array, stranded_intervals, True)
+
+
+@streamable()
+def get_sequences(sequence, intervals) -> EncodedRaggedArray:
+    """dna.py:91-106: the sequence of every interval, strands ignored."""
+    return _interval_sequences(sequence, intervals, False)
+
+
 def complement_xor_of(alphabet_encoding) -> int:
     """The complement of a four-letter DNA/RNA alphabet as an XOR on the 2-bit code (3 for ACGT order, 2 for ACTG /
     ACUG order); raises for alphabets where it is not an XOR."""

@@ -316,6 +316,62 @@ int bnpk_multiline_entries(const uint8_t *chunk, const int64_t *line_starts, con
                            const int64_t *hdr_before, size_t keep, int trim_cr, int64_t *h_starts, int32_t *h_lens,
                            int64_t *s_starts, int32_t *s_lens, int64_t *entry_lens, void *stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Intervals (BED; io/delimited_buffers.py:29-316, io/indexed_fasta.py:165-206, sequence/dna.py:68-106).
+ *
+ * bnpk_delimited_columns: the tab-separated columns of every line of a chunk, over the per-line arrays of
+ *   bnpk_line_split(lines_per_entry = 1).  The column count is the first line's; `columns` is a HOST array of n_columns
+ *   bnpk_column (n_columns <= BNPK_MAX_COLUMNS), column c of every line is written as its kind says:
+ *     BNPK_COL_SKIP        nothing (the column is still counted)
+ *     BNPK_COL_TEXT        out = int64[n_lines] chunk offset of the field, lens = int32[n_lines] its length
+ *     BNPK_COL_INT         out = int64[n_lines]: an optional '-' or '+' and 1 to 18 digits
+ *     BNPK_COL_INT_OR_DOT  as BNPK_COL_INT, and "." reads as 0 (Optional[int], io/strops.py:69-83)
+ *     BNPK_COL_STRAND      out = uint8[n_lines] StrandEncoding code: '+' 0, '-' 1, '.' 2
+ *   When the first line ends in '\r', a '\r' that ends a line is not part of its last column.  The first fault is
+ *   atomicMin-ed into status[BNPK_ST_BAD_BASE] as (line << 8 | column << 3 | BNPK_BAD_*) (status pre-initialised).
+ *   BNPK_E_BADARG for a NULL pointer with n_lines > 0, n_columns outside 1..BNPK_MAX_COLUMNS, an unknown kind or a
+ *   missing output.
+ * bnpk_name_lookup: out_ids[r] = the index k of the name table with names[name_offsets[k] .. name_offsets[k + 1]) equal
+ *   to the bytes of row r (base[starts[r] .. + lens[r])), compared byte for byte over their full lengths.  The table
+ *   must be sorted as bytes (a name before every longer name it is a prefix of).  A row with no name gets -1 and is
+ *   atomicMin-ed into status[BNPK_ST_BAD_BASE].
+ * bnpk_interval_gather: row r = bases [start[r], stop[r]) of contig ids[r], whose first base is file byte
+ *   contig_offset[id], with lenc[id] bases per line of lenb[id] bytes, contig_len[id] bases.  ids == NULL is the flat
+ *   mode: one contig of file_bytes bases, no line ends (contig_* are not read).  A row with start < 0, stop < start,
+ *   stop > the contig length, more than INT32_MAX bases, a contig id outside 0..n_contigs-1 or a base outside the file is atomicMin-ed into
+ *   status[BNPK_ST_BAD_BASE].  Two passes:
+ *     out == NULL   check pass: row_lens[r] = stop - start for a good row, 0 for a reported one
+ *     out != NULL   copy pass: out[out_offsets[r] + i], out_offsets int64[R+1] of the check pass' row_lens; a row whose
+ *                   strand[r] != 0 (strand may be NULL) is written reverse-complemented through complement_lut256.
+ * ------------------------------------------------------------------------------------- */
+#define BNPK_MAX_COLUMNS 16
+#define BNPK_COL_SKIP        0
+#define BNPK_COL_TEXT        1
+#define BNPK_COL_INT         2
+#define BNPK_COL_INT_OR_DOT  3
+#define BNPK_COL_STRAND      4
+#define BNPK_BAD_TABS        1   /* the line's tab count differs from the first line's      */
+#define BNPK_BAD_COLUMNS     2   /* the line has fewer columns than `columns` names         */
+#define BNPK_BAD_INT         3   /* not an integer of at most 18 digits                     */
+#define BNPK_BAD_STRAND      4   /* not one of '+', '-', '.'                                */
+
+typedef struct bnpk_column {
+    int kind;
+    void *out;
+    int32_t *lens;
+} bnpk_column;
+
+int bnpk_delimited_columns(const uint8_t *chunk, size_t n, const int64_t *line_starts, const int32_t *line_lens,
+                           size_t n_lines, const bnpk_column *columns, int n_columns, int64_t *status, void *stream);
+int bnpk_name_lookup(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
+                     const uint8_t *names, const int64_t *name_offsets, size_t n_names, int32_t *out_ids,
+                     int64_t *status, void *stream);
+int bnpk_interval_gather(const uint8_t *file, size_t file_bytes, size_t n_rows, const int32_t *ids,
+                         const int64_t *contig_offset, const int32_t *lenc, const int32_t *lenb, const int64_t *contig_len,
+                         size_t n_contigs, const int64_t *start, const int64_t *stop, const uint8_t *strand,
+                         const uint8_t *complement_lut256, int32_t *row_lens, const int64_t *out_offsets, uint8_t *out,
+                         int64_t *status, void *stream);
+
 /* Bloom filter over k-mer hashes (sequence/bloom_filter.py:15-42): hash function i is v ^ offsets[i]; the filter is
  * one byte per position (the reference's bool mask).  insert: mask[(v ^ offsets[i]) % mask_size] = 1 for every value and
  * function; query: out[j] = AND over the functions. */
