@@ -68,7 +68,6 @@ SIGNATURES = {
     "bnpk_pipeline_kmer_count_host_on": (_i, [_vp, _vp, _sz, _i, _u8, _i, _i, _i, _vp, _i, _i, _i64, _i, _vp, _vp, _vp]),
     "bnpk_multiline_flags": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
     "bnpk_multiline_entries": (_i, [_vp, _vp, _vp, _vp, _vp, _sz, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "bnpk_fasta_gather": (_i, [_vp, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bnpk_bloom_insert": (_i, [_vp, _sz, _vp, _i, _vp, _sz, _vp]),
     "bnpk_bloom_query": (_i, [_vp, _sz, _vp, _i, _vp, _sz, _vp, _vp]),
     "bnpk_synth_fastq": (_i, [_vp, _u64, _u64, _u64, _vp]),

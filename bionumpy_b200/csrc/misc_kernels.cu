@@ -252,32 +252,6 @@ __global__ void __launch_bounds__(256) multiline_entries_kernel(const uint8_t *c
 }
 
 // ------------------------------------------------------------------------------------------
-// Indexed FASTA (io/indexed_fasta.py:101-206): sequence positions -> file bytes, skipping the line ends.
-// Row r = bases [row_start[r], row_start[r] + row_len[r]) of the contig whose first base is file byte
-// contig_offset[r], written with lenc[r] bases per line of lenb[r] bytes.  One warp per row, coalesced writes.
-// ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) fasta_gather_kernel(const uint8_t *file, size_t file_bytes, size_t n_rows,
-                                                           const int64_t *contig_offset, const int64_t *row_start,
-                                                           const int64_t *row_len, const int32_t *lenc, const int32_t *lenb,
-                                                           const int64_t *out_offsets, uint8_t *out, int64_t *status) {
-    const int lane = threadIdx.x & 31;
-    const size_t warp_global = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const size_t n_warps = ((size_t)gridDim.x * blockDim.x) >> 5;
-    for (size_t r = warp_global; r < n_rows; r += n_warps) {
-        const int64_t base = contig_offset[r], s = row_start[r], L = row_len[r], o = out_offsets[r];
-        const int64_t c = lenc[r], b = lenb[r];
-        for (int64_t i = lane; i < L; i += 32) {
-            const int64_t p = s + i;
-            const int64_t byte = base + (p / c) * b + p % c;
-            uint8_t v = 0;
-            if (byte >= 0 && (size_t)byte < file_bytes) v = file[byte];
-            else atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)(((int64_t)r << 32) | i));
-            out[o + i] = v;
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------
 // Bloom filter over k-mer hashes (sequence/bloom_filter.py:15-42): bit j of the filter is the byte mask[j];
 // hash function i is v ^ offsets[i], reduced mod the mask size as NumPy's int64 `%` does (a floor modulo: a negative
 // v ^ offsets[i] lands in [0, mask_size) like a positive one, on the slot NumPy picks).
@@ -482,18 +456,6 @@ int bnpk_multiline_entries(const uint8_t *chunk, const int64_t *line_starts, con
                                                                      h_starts, h_lens, s_starts, s_lens,
                                                                      (unsigned long long *)entry_lens);
     BNPK_LAUNCHED("multiline_entries_kernel");
-    return 0;
-}
-
-int bnpk_fasta_gather(const uint8_t *file, size_t file_bytes, size_t n_rows, const int64_t *contig_offset,
-                      const int64_t *row_start, const int64_t *row_len, const int32_t *lenc, const int32_t *lenb,
-                      const int64_t *out_offsets, uint8_t *out, int64_t *status, void *stream) {
-    if (n_rows == 0) return 0;
-    const size_t want = (n_rows + 7) / 8;
-    const unsigned grid = grid_cap(want, 8);
-    fasta_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(file, file_bytes, n_rows, contig_offset, row_start, row_len, lenc,
-                                                                lenb, out_offsets, out, status);
-    BNPK_LAUNCHED("fasta_gather_kernel");
     return 0;
 }
 

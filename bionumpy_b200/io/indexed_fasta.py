@@ -1,10 +1,11 @@
 """IndexedFasta on the device (mirror of bionumpy/io/indexed_fasta.py:13-206).
 
-The FASTA file is brought to the device once (pinned, prefetching ingest); a contig or a set of intervals is then a
-gather that skips the line ends (bnpk_fasta_gather) -- where the reference seeks and reads per interval and deletes the
-newline bytes on the host (indexed_fasta.py:101-131, 133-206).  The index is the .fai next to the file (read_index,
-indexed_fasta.py:13-31); without one it is built from the file image (create_index, :34-58: name, length, offset of the
-first base, bases per line, bytes per line)."""
+The FASTA file is brought to the device once (pinned, prefetching ingest); a set of intervals is then one gather that
+checks every interval against its contig and skips the line ends (bnpk_interval_gather, through ops.interval_gather),
+and a whole contig is the consecutive intervals that cover it -- where the reference seeks and reads per interval and
+deletes the newline bytes on the host (indexed_fasta.py:101-131, 133-206).  The index is the .fai next to the file
+(read_index, indexed_fasta.py:13-31); without one it is built from the file image (create_index, :34-58: name, length,
+offset of the first base, bases per line, bytes per line)."""
 import os
 from pathlib import Path
 
@@ -15,6 +16,11 @@ from .. import _native as nv
 from .. import config, ops
 from ..encoded_array import EncodedArray, EncodedRaggedArray, BaseEncoding
 from ..rows import RowView
+
+# Bases per interval of a whole-contig fetch.  The gather gives a row eight lanes, so a contig goes as many short rows:
+# the 1.53 Mbases of sacCer3's chrIV take 36 ms as one row and 0.24-0.37 ms as rows of 1024 (as of 256; 0.68 ms as rows
+# of 16384) on an H100 80GB HBM3 at a 700 W power limit.
+_PIECE = 1024
 
 
 def read_index(filename) -> dict:
@@ -86,33 +92,23 @@ class IndexedFasta:
     def __repr__(self):
         return f"Indexed Fasta File with chromosome sizes: {self.get_contig_lengths()}"
 
-    def _gather(self, names, starts, lens):
-        dev = self._file.device
-        idx = [self._index[n] for n in names]
-        t = lambda v, dt: torch.tensor(v, dtype=dt, device=dev)
-        row_len = t(lens, torch.int64)
-        offsets = torch.zeros(len(idx) + 1, dtype=torch.int64, device=dev)
-        offsets[1:] = torch.cumsum(row_len, 0)
-        out = torch.empty(int(sum(lens)), dtype=torch.uint8, device=dev)
-        status = nv.new_status(dev)
-        # (the argument tensors stay referenced until the launch is queued)
-        c_off, r_start = t([i["offset"] for i in idx], torch.int64), t(starts, torch.int64)
-        lenc, lenb = t([max(i["lenc"], 1) for i in idx], torch.int32), t([max(i["lenb"], 1) for i in idx], torch.int32)
-        nv.check(nv.lib().bnpk_fasta_gather(nv.ptr(self._file), self._file.numel(), len(idx), nv.ptr(c_off), nv.ptr(r_start),
-                                            nv.ptr(row_len), nv.ptr(lenc), nv.ptr(lenb), nv.ptr(offsets), nv.ptr(out),
-                                            nv.ptr(status), nv.stream_ptr()))
-        bad = ops.read_status(status).bad_base()
-        assert bad is None, f"interval {bad[0]} reaches beyond the file"
-        return out, row_len
-
     def __getitem__(self, chromosome: str) -> EncodedArray:
-        """The whole sequence of a contig (indexed_fasta.py:101-131)."""
-        out, _ = self._gather([chromosome], [0], [self._index[chromosome]["rlen"]])
+        """The whole sequence of a contig (indexed_fasta.py:101-131): its consecutive intervals of _PIECE bases, whose
+        rows lie one after the other in the gather's output."""
+        rlen = self._index[chromosome]["rlen"]
+        contig_ids, _, _, contigs = self._name_table()
+        start = torch.arange(0, rlen, _PIECE, dtype=torch.int64, device=self._file.device)
+        stop = (start + _PIECE).clamp(max=rlen)
+        ids = torch.full_like(start, contig_ids[chromosome], dtype=torch.int32)
+        out, _, bad, _ = ops.interval_gather(self._file, start, stop, ids, contigs)
+        if bad is not None:
+            raise AssertionError(f"contig {chromosome} reaches beyond the file")
         return EncodedArray(out, BaseEncoding)
 
     def _name_table(self):
-        """The contig names sorted as bytes, concatenated on the device with their offsets, and each contig's
-        (offset, lenc, lenb, length) in that order: built once, for bnpk_name_lookup and bnpk_interval_gather."""
+        """The contig names sorted as bytes: each name's place in that order (the contig id), the names concatenated
+        on the device with their offsets, and each contig's (offset, lenc, lenb, length) by id: built once, for
+        bnpk_name_lookup and bnpk_interval_gather."""
         if getattr(self, "_table", None) is None:
             dev = self._file.device
             names = sorted(self._index, key=lambda n: n.encode())
@@ -123,48 +119,49 @@ class IndexedFasta:
             text = torch.frombuffer(bytearray(b"".join(raw) or b"\0"), dtype=torch.uint8).to(dev)
             contigs = (t([i["offset"] for i in idx], torch.int64), t([i["lenc"] for i in idx], torch.int32),
                        t([i["lenb"] for i in idx], torch.int32), t([i["rlen"] for i in idx], torch.int64))
-            self._table = (names, text, torch.from_numpy(ends).to(dev), contigs)
+            self._table = ({n: k for k, n in enumerate(names)}, text, torch.from_numpy(ends).to(dev), contigs)
         return self._table
 
     def get_interval_sequences(self, intervals) -> EncodedRaggedArray:
         """indexed_fasta.py:165-206: ``intervals`` has .chromosome (names), .start, .stop (or is an iterable of
-        (chromosome, start, stop)).  Intervals on the device (an Interval or Bed6 chunk) are looked up and gathered
-        on the device with one synchronisation, for the output size; an interval outside its contig raises
-        ValueError and an unknown chromosome KeyError."""
-        if _on_device(intervals):
-            return self._device_interval_sequences(intervals)
-        if hasattr(intervals, "chromosome"):
-            names = [c if isinstance(c, str) else c.to_string() for c in intervals.chromosome]
-            starts = [int(x) for x in intervals.start]
-            stops = [int(x) for x in intervals.stop]
+        (chromosome, start, stop)).  Every interval is gathered on the device with one synchronisation, for the
+        output size.  Intervals on the device (an Interval or Bed6 chunk) have their names looked up there: an
+        interval outside its contig raises ValueError and an unknown chromosome KeyError.  Host intervals are
+        uploaded once: an unknown chromosome raises KeyError, an interval outside its contig or the file
+        AssertionError.  An interval holds at most INT32_MAX bases, as row lengths are int32; a longer one is reported
+        like one outside its contig (fa[name] goes in pieces and has no such limit)."""
+        contig_ids, text, name_offsets, contigs = self._name_table()
+        on_device = _on_device(intervals)
+        if on_device:
+            rows = RowView(intervals.chromosome)
+            start, stop = intervals.start.to(torch.int64).contiguous(), intervals.stop.to(torch.int64).contiguous()
+            ids, st_names = ops.name_lookup(rows.base, rows.starts, rows.lens, text, name_offsets)
+            bad_names = [st_names[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]
+            name_of = lambda r: intervals.chromosome[r].to_string()
         else:
-            names, starts, stops = zip(*[(c, int(a), int(b)) for c, a, b in intervals])
-        lens = [b - a for a, b in zip(starts, stops)]
-        out, row_len = self._gather(list(names), list(starts), lens)
-        return EncodedRaggedArray(EncodedArray(out, BaseEncoding), row_len.to(torch.int32))
-
-    def _device_interval_sequences(self, intervals):
-        names, text, name_offsets, contigs = self._name_table()
-        rows = RowView(intervals.chromosome)
-        start, stop = intervals.start.to(torch.int64).contiguous(), intervals.stop.to(torch.int64).contiguous()
-        ids, st_names = ops.name_lookup(rows.base, rows.starts, rows.lens, text, name_offsets)
-        row_lens, st_rows = ops.interval_check(self._file, start, stop, ids, contigs)
-        offsets = ops.row_offsets(row_lens)
-        total, bad_name, bad_row = (int(x) for x in torch.cat(
-            [offsets[-1:], st_names[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1], st_rows[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]
-        ).cpu().tolist())
-        if bad_name != nv.INT64_MAX:
-            raise KeyError(intervals.chromosome[bad_name].to_string())
-        if bad_row != nv.INT64_MAX:
-            name = intervals.chromosome[bad_row].to_string()
-            raise ValueError(f"interval {bad_row} ({name}:{int(start[bad_row])}-{int(stop[bad_row])}) is not inside "
-                             f"the contig ({self._index[name]['rlen']} bases)")
-        out = ops.interval_copy(self._file, start, stop, offsets, total, ids, contigs)
+            if hasattr(intervals, "chromosome"):
+                intervals = zip(intervals.chromosome, intervals.start, intervals.stop)
+            rows = [(c if isinstance(c, str) else c.to_string(), int(a), int(b)) for c, a, b in intervals]
+            name_of = lambda r: rows[r][0]
+            cols = torch.tensor([[contig_ids[n] for n, _, _ in rows], [a for _, a, _ in rows], [b for _, _, b in rows]],
+                                dtype=torch.int64).to(self._file.device)
+            ids, start, stop, bad_names = cols[0].to(torch.int32), cols[1], cols[2], []
+        out, row_lens, bad_row, bad_name = ops.interval_gather(self._file, start, stop, ids, contigs, extra=bad_names)
+        if bad_name and bad_name[0] != nv.INT64_MAX:
+            raise KeyError(name_of(bad_name[0]))
+        if bad_row is not None:
+            name = name_of(bad_row)
+            where = f"interval {bad_row} ({name}:{int(start[bad_row])}-{int(stop[bad_row])})"
+            rlen = self._index[name]["rlen"]
+            if on_device:
+                raise ValueError(f"{where} is not inside the contig ({rlen} bases)")
+            raise AssertionError(f"{where} reaches beyond the file or its contig ({rlen} bases)")
         return EncodedRaggedArray(EncodedArray(out, BaseEncoding), row_lens)
 
 
 def _on_device(intervals):
-    """Whether ``intervals`` is a record chunk whose chromosome, start and stop already live on the device."""
+    """Whether ``intervals`` is a record chunk whose chromosome, start and stop already live on the device, so that
+    the names are looked up there; anything else is read on the host and uploaded."""
     chrom = getattr(intervals, "chromosome", None)
     start, stop = getattr(intervals, "start", None), getattr(intervals, "stop", None)
     return (isinstance(chrom, EncodedRaggedArray) and chrom.device.type == "cuda" and

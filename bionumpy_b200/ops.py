@@ -569,3 +569,16 @@ def interval_copy(file, start, stop, offsets, total, ids=None, contigs=None, str
         check(lib().bnpk_interval_gather(*args, ptr(strand), ptr(complement_lut), None, ptr(offsets), ptr(out), None,
                                          stream_ptr()))
     return out
+
+
+def interval_gather(file, start, stop, ids=None, contigs=None, strand=None, complement_lut=None, extra=()):
+    """Both passes of bnpk_interval_gather around the one synchronisation a gather needs: the check pass, the row
+    offsets, then a single .cpu() of the output size, the first bad row and the ``extra`` one-word device tensors (a
+    caller's own status words).  Returns (out, row_lens, bad_row, extra words).  With a bad row the copy pass is not
+    launched and ``out`` is None: the caller words the error.  A row of more than INT32_MAX bases is a bad row."""
+    row_lens, status = interval_check(file, start, stop, ids, contigs)
+    offsets = row_offsets(row_lens)
+    total, bad, *words = torch.cat([offsets[-1:], status[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1], *extra]).cpu().tolist()
+    if bad != nv.INT64_MAX:
+        return None, row_lens, bad, words
+    return interval_copy(file, start, stop, offsets, total, ids, contigs, strand, complement_lut), row_lens, None, words

@@ -86,12 +86,6 @@ def _interval_sequences(sequence, intervals, stranded):
         raise nv.NativeLibraryError("interval sequences need a CUDA tensor: bionumpy_b200 has no CPU fallback")
     raw = raw.to(torch.uint8).contiguous()
     start, stop = (torch.as_tensor(v).to(raw.device, torch.int64).contiguous() for v in (intervals.start, intervals.stop))
-    row_lens, status = ops.interval_check(raw, start, stop)
-    offsets = ops.row_offsets(row_lens)
-    total, bad = (int(x) for x in torch.cat([offsets[-1:], status[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]).cpu().tolist())
-    if bad != nv.INT64_MAX:
-        raise ValueError(f"interval {bad} ({int(start[bad])}-{int(stop[bad])}) is not inside the sequence "
-                         f"({raw.numel()} bases)")
     strand = lut = None
     if stranded:
         from ..encodings import StrandEncoding
@@ -100,7 +94,10 @@ def _interval_sequences(sequence, intervals, stranded):
         strand = (torch.as_tensor(s.raw() if hasattr(s, "raw") else s).reshape(-1).to(raw.device) == minus)
         strand = strand.to(torch.uint8).contiguous()
         lut = _device_table(sequence.encoding, raw.device)
-    out = ops.interval_copy(raw, start, stop, offsets, total, strand=strand, complement_lut=lut)
+    out, row_lens, bad, _ = ops.interval_gather(raw, start, stop, strand=strand, complement_lut=lut)
+    if bad is not None:
+        raise ValueError(f"interval {bad} ({int(start[bad])}-{int(stop[bad])}) is not inside the sequence "
+                         f"({raw.numel()} bases)")
     return EncodedRaggedArray(EncodedArray(out, sequence.encoding), row_lens)
 
 

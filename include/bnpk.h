@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define BNPK_ABI_VERSION 2
+#define BNPK_ABI_VERSION 3
 
 /* argument errors */
 #define BNPK_E_BADARG   (-1)
@@ -293,16 +293,6 @@ int bnpk_bincount(const int64_t *values, size_t n, int64_t n_bins, int hist_mode
 int bnpk_bincount_rows(const int64_t *values, const int64_t *offsets, size_t n_rows, int64_t n_bins,
                        int64_t *out, int64_t *status, void *stream);
 
-/* ---------------------------------------------------------------------------------------
- * Indexed FASTA (io/indexed_fasta.py:101-206, IndexedFasta.__getitem__ / get_interval_sequences): rows of bases out of
- * a device-resident FASTA file image, line ends skipped.  Row r = bases [row_start[r], row_start[r] + row_len[r]) of
- * the contig whose first base is file byte contig_offset[r] (.fai column 3), lenc[r] bases per line of lenb[r] bytes
- * (.fai columns 4, 5).  out[out_offsets[r] + i]; a position outside the file is reported in status[BNPK_ST_BAD_BASE].
- * ------------------------------------------------------------------------------------- */
-int bnpk_fasta_gather(const uint8_t *file, size_t file_bytes, size_t n_rows, const int64_t *contig_offset,
-                      const int64_t *row_start, const int64_t *row_len, const int32_t *lenc, const int32_t *lenb,
-                      const int64_t *out_offsets, uint8_t *out, int64_t *status, void *stream);
-
 /* Multi-line FASTA bookkeeping over the per-line arrays of bnpk_line_split(lines_per_entry = 1)
  * (MultiLineFastaBuffer.from_raw_buffer / get_data, io/multiline_buffer.py:46-62,89-106):
  *   bnpk_multiline_flags    is_header[i] (line starts with '>'), out2[0] = 1 + the last line whose newline is followed by
@@ -336,7 +326,9 @@ int bnpk_multiline_entries(const uint8_t *chunk, const int64_t *line_starts, con
  *   must be sorted as bytes (a name before every longer name it is a prefix of).  A row with no name gets -1 and is
  *   atomicMin-ed into status[BNPK_ST_BAD_BASE].
  * bnpk_interval_gather: row r = bases [start[r], stop[r]) of contig ids[r], whose first base is file byte
- *   contig_offset[id], with lenc[id] bases per line of lenb[id] bytes, contig_len[id] bases.  ids == NULL is the flat
+ *   contig_offset[id] (.fai column 3), with lenc[id] bases per line of lenb[id] bytes (.fai columns 4, 5), contig_len[id]
+ *   bases, line ends skipped; IndexedFasta.__getitem__ (io/indexed_fasta.py:101-131) is the consecutive rows that cover
+ *   [0, contig_len[id]), get_interval_sequences any rows.  ids == NULL is the flat
  *   mode: one contig of file_bytes bases, no line ends (contig_* are not read).  A row with start < 0, stop < start,
  *   stop > the contig length, more than INT32_MAX bases, a contig id outside 0..n_contigs-1 or a base outside the file is atomicMin-ed into
  *   status[BNPK_ST_BAD_BASE].  Two passes:

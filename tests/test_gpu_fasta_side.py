@@ -1,10 +1,11 @@
 """The genome-side input path against the oracle, bit for bit: the multi-line FASTA buffer and reader
-(multiline_flags_kernel, multiline_entries_kernel, io/multiline.py), indexed FASTA (fasta_gather_kernel,
-io/indexed_fasta.py), the Bloom filter (bloom_insert_kernel, bloom_query_kernel), KmerIndex / KmerLookup, the byte
-count (count_byte_kernel) and the per-row bincount (bincount_rows_kernel).
+(multiline_flags_kernel, multiline_entries_kernel, io/multiline.py), indexed FASTA (interval_check_kernel,
+interval_copy_kernel, io/indexed_fasta.py), the Bloom filter (bloom_insert_kernel, bloom_query_kernel), KmerIndex /
+KmerLookup, the byte count (count_byte_kernel) and the per-row bincount (bincount_rows_kernel).
 
 Every case that has to reach a second grid-stride pass sizes itself from bnpk_sm_count() and the launch shape the
-kernel's entry point in csrc/misc_kernels.cu uses, so the cases stay meaningful on any SM count."""
+kernel's entry point uses (csrc/misc_kernels.cu; csrc/interval_kernels.cu for the indexed FASTA gather), so the cases
+stay meaningful on any SM count."""
 import numpy as np
 import pytest
 import torch
@@ -13,10 +14,12 @@ from oracle import bnp_oracle as oracle
 
 pytestmark = pytest.mark.gpu
 
-# launch shapes of csrc/misc_kernels.cu: blocks per SM x threads per block (x work per thread)
+# launch shapes of csrc/misc_kernels.cu and csrc/interval_kernels.cu: blocks per SM x threads per block (x work per thread)
 THREADS = 256
 LINE_BLOCKS_PER_SM = 8          # bnpk_multiline_flags / bnpk_multiline_entries: one line per thread
-WARP_ROW_BLOCKS_PER_SM = 8      # bnpk_fasta_gather / bnpk_bincount_rows: one row per warp
+WARP_ROW_BLOCKS_PER_SM = 8      # bnpk_bincount_rows: one row per warp
+COPY_BLOCKS_PER_SM = 8          # bnpk_interval_gather, copy pass: one row per COPY_LANES_PER_ROW threads
+COPY_LANES_PER_ROW = 8
 BLOOM_BLOCKS_PER_SM = 16        # bnpk_bloom_insert / bnpk_bloom_query: one value per thread
 COUNT_BYTE_BLOCKS_PER_SM = 8    # bnpk_count_byte: one 16-byte unit per thread
 POISON = np.frombuffer(b">\r\n", dtype=np.uint8)
@@ -335,7 +338,7 @@ def test_indexed_fasta_vs_oracle(bnp, sm_count, tmp_path, eol, trailing):
     assert create_index(path) == idx
     assert [v["rlen"] for v in idx.values()] == [len(s) for _, s, _ in contigs]
     assert all(v["lenb"] - v["lenc"] == len(eol) for v in idx.values() if v["rlen"])
-    one_pass = sm_count * WARP_ROW_BLOCKS_PER_SM * (THREADS // 32)
+    one_pass = sm_count * COPY_BLOCKS_PER_SM * (THREADS // COPY_LANES_PER_ROW)
     iv = _intervals(rng, contigs, one_pass + 777)
     assert len(iv) > one_pass
 
@@ -354,7 +357,8 @@ def test_indexed_fasta_vs_oracle(bnp, sm_count, tmp_path, eol, trailing):
 
 def test_indexed_fasta_interval_to_the_last_byte(bnp, tmp_path):
     """A file without a final newline: an interval that ends on the file's last byte works, one byte further is
-    reported by the gather kernel's bounds guard and raises."""
+    reported by the gather's check pass and raises; so does an interval that ends past its contig but inside the
+    file, in the bytes of the next contig."""
     rng = np.random.default_rng(5)
     for L, w in ((120, 60), (121, 60), (5, 1), (4097, 4096)):
         contigs = [("a", _letters(rng, 33), 7), ("z", _letters(rng, L), w)]
@@ -368,6 +372,8 @@ def test_indexed_fasta_interval_to_the_last_byte(bnp, tmp_path):
             fa.get_interval_sequences([("a", 0, 3), ("z", L - 1, L + 1)])
         with pytest.raises(AssertionError, match="beyond the file"):
             fa.get_interval_sequences([("z", 0, L + 1)])
+        with pytest.raises(AssertionError, match="beyond the file"):
+            fa.get_interval_sequences([("a", 0, 34)])
 
 
 # ------------------------------------------------------------------------------------------------------------------

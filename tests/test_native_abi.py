@@ -20,7 +20,7 @@ def test_library_exports_every_declared_symbol():
     for name in names:
         assert hasattr(lib, name), f"{name} declared in include/bnpk.h but not exported"
     assert set(names) == set(_native.SIGNATURES), set(names) ^ set(_native.SIGNATURES)
-    assert lib.bnpk_abi_version() == 2
+    assert lib.bnpk_abi_version() == 3
 
 
 def test_header_constants_match_python_mirror():

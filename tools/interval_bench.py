@@ -6,7 +6,8 @@ host list path and the NumPy oracle.
 Workload 1: a synthetic 10 M-line BED (chromosome, start, stop; tests/interval_oracle.synthetic_bed) on the device:
 bnpk_delimited_columns alone (CUDA-event median over the lines of bnpk_line_split) and BedBuffer.from_raw_buffer end to
 end.  Workload 2: 1 M x 100 bp intervals on sacCer3: the interval copy kernel alone and get_interval_sequences end to end
-from device intervals; the list path (host ints) on 10 k intervals; the oracle on one core.  Prints one JSON line with
+from device intervals; the list path (host ints) on 10 k intervals; the whole of chrIV (the longest contig, 1.5 Mbases)
+as fa["chrIV"], wall time around a synchronise; the oracle on one core.  Prints one JSON line with
 the card's name and power limit (read-only nvidia-smi query in the same run); --check compares the outputs with the
 oracle and the generator's truth."""
 import argparse
@@ -109,6 +110,8 @@ def gather_case(n, iters, check):
     m = 10_000
     host = list(zip(chroms[:m], starts[:m].tolist(), (starts[:m] + 100).tolist()))
     out["list_path_10k_s"] = round(wall_s(lambda: fa.get_interval_sequences(host), 1), 4)
+    out["whole_contig"] = {"name": "chrIV", "bases": index["chrIV"]["rlen"],
+                           "ms": round(wall_s(lambda: fa["chrIV"], iters) * 1e3, 3)}
     t0 = time.perf_counter()
     flat, _ = io_.interval_sequences(raw, index, chroms[:m], starts[:m].tolist(), (starts[:m] + 100).tolist())
     out["cpu_oracle_10k_s"] = round(time.perf_counter() - t0, 4)
@@ -123,7 +126,8 @@ def gather_case(n, iters, check):
         whole = np.concatenate([contig[k] for k in names])
         base = np.concatenate([[0], np.cumsum([index[k]["rlen"] for k in names])])[ci]
         want = whole[(base + starts)[:, None] + np.arange(100)].reshape(-1)
-        out["identical"] = bool(ok and np.array_equal(got, want))
+        out["identical"] = bool(ok and np.array_equal(got, want) and
+                                np.array_equal(fa["chrIV"].raw().cpu().numpy(), contig["chrIV"]))
     return out
 
 
