@@ -26,6 +26,8 @@ from .io.buffers import CudaFastQBuffer, CudaTwoLineFastaBuffer, FastQBuffer, Tw
 from .io.multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
 from .datatypes import SequenceEntry, SequenceEntryWithQuality, Interval, StrandedInterval, Bed6, replace
 from . import datatypes
+from . import arithmetics, genomic_data
+from .genomic_data import Genome
 from .io.files import count_entries
 from .io.write import NpBufferedWriter
 

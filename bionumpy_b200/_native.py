@@ -24,6 +24,8 @@ FMT_FASTQ, FMT_FASTA, FMT_FASTA_WRAPPED = 0, 1, 2
 MAX_COLUMNS = 16
 COL_SKIP, COL_TEXT, COL_INT, COL_INT_OR_DOT, COL_STRAND = 0, 1, 2, 3, 4
 BAD_TABS, BAD_COLUMNS, BAD_INT, BAD_STRAND = 1, 2, 3, 4
+PILEUP_COUNT, PILEUP_ANY = 0, 1
+RUNS_MAX, RUNS_MIN, RUNS_SUM, RUNS_ANY = 0, 1, 2, 3
 INT64_MAX = (1 << 63) - 1
 SMEM_MAX_BINS = 32768
 
@@ -77,6 +79,12 @@ SIGNATURES = {
     "bnpk_name_lookup": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
     "bnpk_interval_gather": (_i, [_vp, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                   _vp]),
+    "bnpk_interval_events": (_i, [_vp, _vp, _vp, _vp, _vp, _sz, _i64, _sz, _vp, _vp, _vp, _vp, _vp]),
+    "bnpk_pileup_runs": (_i, [_vp, _sz, _i64, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "bnpk_runs_reduce": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _sz, _vp]),
+    "bnpk_runs_extract": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _vp, _vp]),
+    "bnpk_interval_merge": (_i, [_vp, _vp, _vp, _sz, _i64, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "bnpk_rows_equal_prev": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp]),
 }
 
 

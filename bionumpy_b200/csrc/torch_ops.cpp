@@ -420,6 +420,131 @@ Tensor interval_copy(const Tensor &file, const Tensor &start, const Tensor &stop
     return out;
 }
 
+// pileups: event keys int64[2R] and the first bad row in the status block; ids (int32) index contig_offset and
+// contig_len (int64), no ids = one contig of `size`
+std::tuple<Tensor, Tensor> interval_events(const Tensor &start, const Tensor &stop, const c10::optional<Tensor> &ids,
+                                           const c10::optional<Tensor> &contig_offset,
+                                           const c10::optional<Tensor> &contig_len, int64_t size) {
+    need(start, torch::kInt64, "start");
+    need(stop, torch::kInt64, "stop", start);
+    TORCH_CHECK(start.numel() == stop.numel(), "bnpk: start and stop differ in length");
+    const int32_t *id = nullptr;
+    const int64_t *off = nullptr, *len = nullptr;
+    size_t n_contigs = 0;
+    if (ids) {
+        need(*ids, torch::kInt32, "ids", start);
+        TORCH_CHECK(ids->numel() == start.numel(), "bnpk: one contig id per interval");
+        TORCH_CHECK(contig_offset && contig_len, "bnpk: contig ids need contig_offset and contig_len");
+        need(*contig_offset, torch::kInt64, "contig_offset", start);
+        need(*contig_len, torch::kInt64, "contig_len", start);
+        TORCH_CHECK(contig_offset->numel() == contig_len->numel(), "bnpk: the contig columns differ in length");
+        id = ids->data_ptr<int32_t>();
+        off = contig_offset->data_ptr<int64_t>();
+        len = contig_len->data_ptr<int64_t>();
+        n_contigs = (size_t)contig_offset->numel();
+    }
+    c10::cuda::CUDAGuard guard(start.device());
+    Tensor keys = torch::empty({2 * start.numel()}, start.options());
+    Tensor status = new_status(start);
+    check(bnpk_interval_events(start.data_ptr<int64_t>(), stop.data_ptr<int64_t>(), id, off, len, n_contigs, size,
+                               (size_t)start.numel(), keys.data_ptr<int64_t>(), nullptr, nullptr,
+                               status.data_ptr<int64_t>(), cur_stream(start)),
+          "interval_events");
+    return {keys, status};
+}
+
+// runs of the coverage of sorted event keys: (run_starts int64[K + 2], run_values int64[K + 1], n_runs int64[1])
+std::tuple<Tensor, Tensor, Tensor> pileup_runs(const Tensor &keys, int64_t size, int64_t mode) {
+    need(keys, torch::kInt64, "keys");
+    c10::cuda::CUDAGuard guard(keys.device());
+    const int64_t n = keys.numel();
+    Tensor starts = torch::empty({n + 2}, keys.options());
+    Tensor values = torch::empty({n + 1}, keys.options());
+    Tensor n_runs = torch::empty({1}, keys.options());
+    Tensor ws = new_workspace(keys, (size_t)std::max<int64_t>(n, 1));
+    check(bnpk_pileup_runs(n ? keys.data_ptr<int64_t>() : nullptr, (size_t)n, size, (int)mode,
+                           starts.data_ptr<int64_t>(), values.data_ptr<int64_t>(), n_runs.data_ptr<int64_t>(),
+                           ws.data_ptr<uint8_t>(), (size_t)ws.numel(), cur_stream(keys)),
+          "pileup_runs");
+    return {starts, values, n_runs};
+}
+
+// a track: run_starts int64[R + 1] and values int64[R]
+void need_track(const Tensor &run_starts, const Tensor &values) {
+    need(run_starts, torch::kInt64, "run_starts");
+    need(values, torch::kInt64, "values", run_starts);
+    TORCH_CHECK(values.numel() >= 1 && run_starts.numel() == values.numel() + 1,
+                "bnpk: a track is R >= 1 values and R + 1 run starts");
+}
+
+Tensor runs_reduce(const Tensor &run_starts, const Tensor &values, const Tensor &q_start, const Tensor &q_stop,
+                   int64_t mode) {
+    need_track(run_starts, values);
+    need(q_start, torch::kInt64, "q_start", run_starts);
+    need(q_stop, torch::kInt64, "q_stop", run_starts);
+    TORCH_CHECK(q_start.numel() == q_stop.numel(), "bnpk: q_start and q_stop differ in length");
+    c10::cuda::CUDAGuard guard(run_starts.device());
+    const int64_t n = q_start.numel();
+    Tensor out = torch::empty({n}, run_starts.options());
+    Tensor scratch = torch::empty({3 * n + 1}, run_starts.options());
+    Tensor ws = new_workspace(run_starts, (size_t)std::max<int64_t>(n, 1));
+    check(bnpk_runs_reduce(run_starts.data_ptr<int64_t>(), values.data_ptr<int64_t>(), (size_t)values.numel(),
+                           q_start.data_ptr<int64_t>(), q_stop.data_ptr<int64_t>(), (size_t)n, (int)mode,
+                           out.data_ptr<int64_t>(), scratch.data_ptr<int64_t>(), ws.data_ptr<uint8_t>(),
+                           (size_t)ws.numel(), cur_stream(run_starts)),
+          "runs_reduce");
+    return out;
+}
+
+Tensor runs_extract(const Tensor &run_starts, const Tensor &values, const Tensor &q_start, const Tensor &offsets,
+                    int64_t total) {
+    need_track(run_starts, values);
+    need(q_start, torch::kInt64, "q_start", run_starts);
+    const int64_t *offs = need_offsets(offsets, (size_t)q_start.numel(), run_starts);
+    c10::cuda::CUDAGuard guard(run_starts.device());
+    Tensor out = torch::empty({total}, run_starts.options());
+    if (total)
+        check(bnpk_runs_extract(run_starts.data_ptr<int64_t>(), values.data_ptr<int64_t>(), (size_t)values.numel(),
+                                q_start.data_ptr<int64_t>(), (size_t)q_start.numel(), offs, out.data_ptr<int64_t>(),
+                                cur_stream(run_starts)),
+              "runs_extract");
+    return out;
+}
+
+// merge: (out_rows int64[R], out_stops int64[R], n_out int64[1], status)
+std::tuple<Tensor, Tensor, Tensor, Tensor> interval_merge(const Tensor &start, const Tensor &stop,
+                                                          const c10::optional<Tensor> &same_prev, int64_t distance) {
+    need(start, torch::kInt64, "start");
+    need(stop, torch::kInt64, "stop", start);
+    TORCH_CHECK(start.numel() == stop.numel(), "bnpk: start and stop differ in length");
+    const uint8_t *sp = nullptr;
+    if (same_prev) {
+        need(*same_prev, torch::kUInt8, "same_prev", start);
+        TORCH_CHECK(same_prev->numel() == start.numel(), "bnpk: one same_prev flag per row");
+        sp = u8(*same_prev);
+    }
+    c10::cuda::CUDAGuard guard(start.device());
+    const int64_t n = start.numel();
+    Tensor rows = torch::empty({n}, start.options());
+    Tensor stops = torch::empty({n}, start.options());
+    Tensor n_out = torch::empty({1}, start.options());
+    Tensor status = new_status(start);
+    Tensor ws = new_workspace(start, (size_t)std::max<int64_t>(n, 1));
+    check(bnpk_interval_merge(start.data_ptr<int64_t>(), stop.data_ptr<int64_t>(), sp, (size_t)n, distance,
+                              rows.data_ptr<int64_t>(), stops.data_ptr<int64_t>(), n_out.data_ptr<int64_t>(),
+                              status.data_ptr<int64_t>(), ws.data_ptr<uint8_t>(), (size_t)ws.numel(), cur_stream(start)),
+          "interval_merge");
+    return {rows, stops, n_out, status};
+}
+
+Tensor rows_equal_prev(const Tensor &base, const Tensor &starts, const Tensor &lens) {
+    const Rows r = need_rows(base, starts, lens, c10::nullopt);
+    c10::cuda::CUDAGuard guard(base.device());
+    Tensor flag = torch::empty({(int64_t)r.n_rows}, base.options());
+    check(r.call(bnpk_rows_equal_prev, flag.data_ptr<uint8_t>(), cur_stream(base)), "rows_equal_prev");
+    return flag;
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bnpk, m) {
@@ -451,6 +576,13 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("interval_check(Tensor file, Tensor start, Tensor stop, Tensor? ids, Tensor[] contigs) -> (Tensor, Tensor)");
     m.def("interval_copy(Tensor file, Tensor start, Tensor stop, Tensor? ids, Tensor[] contigs, Tensor? strand, "
           "Tensor? complement_lut, Tensor offsets, int total) -> Tensor");
+    m.def("interval_events(Tensor start, Tensor stop, Tensor? ids, Tensor? contig_offset, Tensor? contig_len, int size) "
+          "-> (Tensor, Tensor)");
+    m.def("pileup_runs(Tensor keys, int size, int mode) -> (Tensor, Tensor, Tensor)");
+    m.def("runs_reduce(Tensor run_starts, Tensor values, Tensor q_start, Tensor q_stop, int mode) -> Tensor");
+    m.def("runs_extract(Tensor run_starts, Tensor values, Tensor q_start, Tensor offsets, int total) -> Tensor");
+    m.def("interval_merge(Tensor start, Tensor stop, Tensor? same_prev, int distance) -> (Tensor, Tensor, Tensor, Tensor)");
+    m.def("rows_equal_prev(Tensor base, Tensor starts, Tensor lens) -> Tensor");
 }
 
 TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
@@ -471,4 +603,10 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("name_lookup", &name_lookup);
     m.impl("interval_check", &interval_check);
     m.impl("interval_copy", &interval_copy);
+    m.impl("interval_events", &interval_events);
+    m.impl("pileup_runs", &pileup_runs);
+    m.impl("runs_reduce", &runs_reduce);
+    m.impl("runs_extract", &runs_extract);
+    m.impl("interval_merge", &interval_merge);
+    m.impl("rows_equal_prev", &rows_equal_prev);
 }

@@ -582,3 +582,117 @@ def interval_gather(file, start, stop, ids=None, contigs=None, strand=None, comp
     if bad != nv.INT64_MAX:
         return None, row_lens, bad, words
     return interval_copy(file, start, stop, offsets, total, ids, contigs, strand, complement_lut), row_lens, None, words
+
+
+def _int64_args(*named):
+    for t, name in named:
+        _need_cuda(t, name)
+        if t.dtype != torch.int64:
+            raise TypeError(f"{name} must be int64")
+
+
+@_on_device
+def interval_events(start, stop, ids=None, contig_offset=None, contig_len=None, size=0, keys=True, glob=False,
+                    status=None):
+    """bnpk_interval_events: (keys int64[2R] or None, global start, global stop (or None), status).  ``ids`` (int32)
+    index contig_offset / contig_len (int64; an offset < 0 leaves the contig out); without ids every row is on one
+    contig of ``size``.  A bad row is reported in status[ST_BAD_BASE]."""
+    _int64_args((start, "start"), (stop, "stop"))
+    n = start.numel()
+    if stop.numel() != n or (ids is not None and ids.numel() != n):
+        raise ValueError("start, stop and ids differ in length")
+    n_contigs = 0
+    if ids is not None:
+        _need_cuda(ids, "ids")
+        _int64_args((contig_offset, "contig_offset"), (contig_len, "contig_len"))
+        if ids.dtype != torch.int32 or contig_offset.numel() != contig_len.numel():
+            raise TypeError("ids must be int32 and the contig columns of one length")
+        n_contigs = contig_offset.numel()
+    dev = start.device
+    k = torch.empty(2 * n, dtype=torch.int64, device=dev) if keys else None
+    gs, ge = (torch.empty(n, dtype=torch.int64, device=dev) for _ in range(2)) if glob else (None, None)
+    if status is None:
+        status = nv.new_status(dev)
+    check(lib().bnpk_interval_events(ptr(start), ptr(stop), ptr(ids), ptr(contig_offset), ptr(contig_len), n_contigs,
+                                     size, n, ptr(k), ptr(gs), ptr(ge), ptr(status), stream_ptr()))
+    return k, gs, ge, status
+
+
+@_on_device
+def pileup_runs(sorted_keys, size, mode=nv.PILEUP_COUNT):
+    """bnpk_pileup_runs on sorted event keys: (run_starts int64[K + 2], run_values int64[K + 1], n_runs int64[1]), the
+    first n_runs + 1 starts and n_runs values valid (nothing is read back)."""
+    _int64_args((sorted_keys, "keys"))
+    n, dev = sorted_keys.numel(), sorted_keys.device
+    starts = torch.empty(n + 2, dtype=torch.int64, device=dev)
+    values = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    n_runs = torch.empty(1, dtype=torch.int64, device=dev)
+    ws = nv.workspace(max(n, 1), dev)
+    check(lib().bnpk_pileup_runs(ptr(sorted_keys), n, size, mode, ptr(starts), ptr(values), ptr(n_runs), ptr(ws),
+                                 ws.numel(), stream_ptr()))
+    return starts, values, n_runs
+
+
+def _runs_args(run_starts, values):
+    _int64_args((run_starts, "run_starts"), (values, "values"))
+    if run_starts.numel() != values.numel() + 1 or values.numel() < 1:
+        raise ValueError("a track is R >= 1 values and R + 1 run starts")
+    return ptr(run_starts), ptr(values), values.numel()
+
+
+@_on_device
+def runs_reduce(run_starts, values, q_start, q_stop, mode):
+    """bnpk_runs_reduce: int64[Q], one reduction (nv.RUNS_*) per query [q_start, q_stop); no synchronisation."""
+    runs = _runs_args(run_starts, values)
+    _int64_args((q_start, "q_start"), (q_stop, "q_stop"))
+    if q_start.numel() != q_stop.numel():
+        raise ValueError("q_start and q_stop differ in length")
+    n, dev = q_start.numel(), q_start.device
+    out = torch.empty(n, dtype=torch.int64, device=dev)
+    scratch = torch.empty(3 * n + 1, dtype=torch.int64, device=dev)
+    ws = nv.workspace(max(n, 1), dev)
+    check(lib().bnpk_runs_reduce(*runs, ptr(q_start), ptr(q_stop), n, mode, ptr(out), ptr(scratch), ptr(ws),
+                                 ws.numel(), stream_ptr()))
+    return out
+
+
+@_on_device
+def runs_extract(run_starts, values, q_start, out_offsets, total):
+    """bnpk_runs_extract: int64[total], query q's values at out_offsets[q] (int64[Q + 1])."""
+    runs = _runs_args(run_starts, values)
+    _int64_args((q_start, "q_start"), (out_offsets, "out_offsets"))
+    if out_offsets.numel() != q_start.numel() + 1:
+        raise ValueError("out_offsets must be int64[Q + 1]")
+    out = torch.empty(total, dtype=torch.int64, device=q_start.device)
+    if total:
+        check(lib().bnpk_runs_extract(*runs, ptr(q_start), q_start.numel(), ptr(out_offsets), ptr(out), stream_ptr()))
+    return out
+
+
+@_on_device
+def interval_merge(start, stop, same_prev=None, distance=0, status=None):
+    """bnpk_interval_merge: (out_rows int64[R], out_stops int64[R], n_out int64[1], status), the first n_out entries
+    valid; a start that decreases inside a segment is reported in status[ST_BAD_BASE]."""
+    _int64_args((start, "start"), (stop, "stop"))
+    n, dev = start.numel(), start.device
+    if stop.numel() != n or (same_prev is not None and (same_prev.numel() != n or same_prev.dtype != torch.uint8)):
+        raise ValueError("start, stop and same_prev (uint8) differ in length")
+    if same_prev is not None:
+        _need_cuda(same_prev, "same_prev")
+    rows, stops = (torch.empty(n, dtype=torch.int64, device=dev) for _ in range(2))
+    n_out = torch.empty(1, dtype=torch.int64, device=dev)
+    if status is None:
+        status = nv.new_status(dev)
+    ws = nv.workspace(max(n, 1), dev)
+    check(lib().bnpk_interval_merge(ptr(start), ptr(stop), ptr(same_prev), n, max(int(distance), 0), ptr(rows),
+                                    ptr(stops), ptr(n_out), ptr(status), ptr(ws), ws.numel(), stream_ptr()))
+    return rows, stops, n_out, status
+
+
+@_on_device
+def rows_equal_prev(base, starts, lens):
+    """bnpk_rows_equal_prev: uint8[R], 1 where a row's bytes equal the previous row's."""
+    args = _rows_args(base, starts, lens)
+    flag = torch.empty(lens.numel(), dtype=torch.uint8, device=base.device)
+    check(lib().bnpk_rows_equal_prev(*args, ptr(flag), stream_ptr()))
+    return flag

@@ -364,6 +364,63 @@ int bnpk_interval_gather(const uint8_t *file, size_t file_bytes, size_t n_rows, 
                          const uint8_t *complement_lut256, int32_t *row_lens, const int64_t *out_offsets, uint8_t *out,
                          int64_t *status, void *stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Pileups, run-length tracks and interval merges (get_pileup, get_boolean_mask, merge_intervals
+ * arithmetics/intervals.py:137-304; GenomicRunLengthArray and GenomicArray, genomic_data/genomic_track.py).
+ * Positions are int64 in [0, 2^59).  A track of size S is R runs: run_starts int64[R + 1] (run_starts[0] = 0,
+ * increasing, run_starts[R] = S) and values int64[R]; no two neighbouring runs have the same value.
+ *
+ * bnpk_interval_events: row r = [start[r], stop[r]) of contig ids[r] (contig_offset[id] is its first global position,
+ *   contig_len[id] its size; a contig with contig_offset < 0 is left out: its rows are not checked and become empty
+ *   intervals at 0).  ids == NULL: every row is on one contig [0, size).  A row with start < 0, stop < start,
+ *   stop > the contig size or an id outside 0..n_contigs-1 is atomicMin-ed into status[BNPK_ST_BAD_BASE] and becomes
+ *   an empty interval at 0.  keys int64[2R] (may be NULL): keys[2r] = global start << 1 | 1, keys[2r + 1] = global
+ *   stop << 1; g_start / g_stop int64[R] (may be NULL): the global start and stop.
+ * bnpk_pileup_runs: the runs of the coverage of the intervals whose event keys (bnpk_interval_events) are sorted in
+ *   keys[0 .. n_keys): BNPK_PILEUP_COUNT the number of intervals over each position, BNPK_PILEUP_ANY 1 where there is
+ *   at least one and 0 elsewhere.  Writes *n_runs = R (<= n_keys + 1), run_starts[0 .. R] (capacity n_keys + 2) and
+ *   run_values[0 .. R) (capacity n_keys + 1).  Keys at positions >= size add nothing.  workspace as for
+ *   bnpk_row_offsets with n := n_keys (2 look-back words per 2048 keys).
+ * bnpk_runs_reduce: out[q] = the reduction over positions [q_start[q], q_stop[q]) (clipped to [0, S)) of the track:
+ *   BNPK_RUNS_MAX / BNPK_RUNS_MIN the largest / smallest value, BNPK_RUNS_SUM the sum of value x positions (int64,
+ *   wrapping), BNPK_RUNS_ANY 1 if a value is not 0.  An empty query gives INT64_MIN, INT64_MAX, 0 and 0.  scratch
+ *   is device int64[3 * n_q + 1]; workspace as for bnpk_row_offsets with n := n_q.  No synchronisation.
+ * bnpk_runs_extract: out[out_offsets[q] + i] = the value at position q_start[q] + i, for i < out_offsets[q + 1] -
+ *   out_offsets[q]; every such position must lie in [0, S).
+ * bnpk_interval_merge: merge_intervals (arithmetics/intervals.py:270-304) over rows sorted by start inside each
+ *   segment; a segment is a maximal block of rows whose same_prev[r] != 0 (row r continues row r - 1's segment;
+ *   same_prev NULL: one segment).  stops = the running max of stop in the segment; row r starts a group iff it starts
+ *   a segment or start[r] > stops[r - 1] + distance.  out_rows[g] = the first row of group g, out_stops[g] = the
+ *   group's largest stop, *n_out = the number of groups.  A row whose start is smaller than the previous row's in the
+ *   same segment is atomicMin-ed into status[BNPK_ST_BAD_BASE].  workspace as for bnpk_row_offsets with n := n_rows.
+ * bnpk_rows_equal_prev: flag[r] = 1 iff r > 0 and the bytes of row r equal those of row r - 1 (same length, every
+ *   byte), else 0.
+ * BNPK_E_BADARG before any device work for an unknown mode, a size or distance outside [0, 2^59), and a missing
+ * pointer the call needs.
+ * ------------------------------------------------------------------------------------- */
+#define BNPK_PILEUP_COUNT 0
+#define BNPK_PILEUP_ANY   1
+#define BNPK_RUNS_MAX 0
+#define BNPK_RUNS_MIN 1
+#define BNPK_RUNS_SUM 2
+#define BNPK_RUNS_ANY 3
+
+int bnpk_interval_events(const int64_t *start, const int64_t *stop, const int32_t *ids, const int64_t *contig_offset,
+                         const int64_t *contig_len, size_t n_contigs, int64_t size, size_t n_rows, int64_t *keys,
+                         int64_t *g_start, int64_t *g_stop, int64_t *status, void *stream);
+int bnpk_pileup_runs(const int64_t *keys, size_t n_keys, int64_t size, int mode, int64_t *run_starts,
+                     int64_t *run_values, int64_t *n_runs, void *workspace, size_t workspace_bytes, void *stream);
+int bnpk_runs_reduce(const int64_t *run_starts, const int64_t *values, size_t n_runs, const int64_t *q_start,
+                     const int64_t *q_stop, size_t n_q, int mode, int64_t *out, int64_t *scratch, void *workspace,
+                     size_t workspace_bytes, void *stream);
+int bnpk_runs_extract(const int64_t *run_starts, const int64_t *values, size_t n_runs, const int64_t *q_start,
+                      size_t n_q, const int64_t *out_offsets, int64_t *out, void *stream);
+int bnpk_interval_merge(const int64_t *start, const int64_t *stop, const uint8_t *same_prev, size_t n_rows,
+                        int64_t distance, int64_t *out_rows, int64_t *out_stops, int64_t *n_out, int64_t *status,
+                        void *workspace, size_t workspace_bytes, void *stream);
+int bnpk_rows_equal_prev(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                         size_t n_rows, uint8_t *flag, void *stream);
+
 /* Bloom filter over k-mer hashes (sequence/bloom_filter.py:15-42): hash function i is v ^ offsets[i]; the filter is
  * one byte per position (the reference's bool mask).  insert: mask[(v ^ offsets[i]) % mask_size] = 1 for every value and
  * function; query: out[j] = AND over the functions. */
