@@ -158,7 +158,16 @@ class GenomicRunLengthArray:
         return self._values.to(torch.int64).contiguous()
 
     def _cast(self, t):
-        return t.to(self._values.dtype) if self._values.dtype != torch.bool else t != 0
+        """int64 kernel output in the track's dtype.  Every value of the track lies in its dtype's range, so clamping
+        to that range first changes only the int64 identity of an empty row's max / min, which becomes the dtype's
+        lowest / highest value as RaggedArray gives (a plain cast would wrap INT64_MIN to 0 and INT64_MAX to -1)."""
+        dtype = self._values.dtype
+        if dtype == torch.bool:
+            return t != 0
+        if dtype != torch.int64:
+            info = torch.iinfo(dtype)
+            t = t.clamp(info.min, info.max)
+        return t.to(dtype)
 
     def astype(self, dtype):
         """The runs with their values converted to another integer or bool type (a conversion that maps two

@@ -18,7 +18,9 @@ def _as_index_tensor(x, device, dtype=torch.int64):
 
 def segment_max(values, rows, n_rows):
     """out[r] = max of values[i] with rows[i] == r, NaN if one of them is NaN; the dtype's lowest value (-inf for
-    floats) where there is none."""
+    floats, False for bool: the max of bools is any) where there is none."""
+    if values.dtype == torch.bool:
+        return segment_sum(values, rows, n_rows) > 0
     low = -float("inf") if values.is_floating_point() else torch.iinfo(values.dtype).min
     out = torch.full((n_rows,), low, dtype=values.dtype, device=values.device)
     out.scatter_reduce_(0, rows, values, "amax", include_self=True)
@@ -31,7 +33,9 @@ def segment_max(values, rows, n_rows):
 
 def segment_min(values, rows, n_rows):
     """out[r] = min of values[i] with rows[i] == r, NaN if one of them is NaN; the dtype's highest value (+inf for
-    floats) where there is none."""
+    floats, True for bool: the min of bools is all) where there is none."""
+    if values.dtype == torch.bool:
+        return segment_sum(~values, rows, n_rows) == 0
     return -segment_max(-values, rows, n_rows) if values.is_floating_point() else \
         _segment_min_int(values, rows, n_rows)
 

@@ -66,6 +66,122 @@ def reduce_runs(run_starts, run_ends, values, a, b, how):
     return np.array(out)
 
 
+def dense_of(starts, ends, values, dtype=None):
+    """The dense array of a track given by its runs (the inverse of runs_of), in ``dtype`` (default the values')."""
+    values = np.asarray(values)
+    counts = np.asarray(ends, dtype=np.int64) - np.asarray(starts, dtype=np.int64)
+    return np.repeat(values.astype(dtype or values.dtype), counts)
+
+
+def extremes(dtype):
+    """Values a track of ``dtype`` must survive: both ends of its range, their neighbours, -1, 0 and 1."""
+    dtype = np.dtype(dtype)
+    if dtype == np.bool_:
+        return np.array([False, True])
+    info = np.iinfo(dtype)
+    vals = {info.min, info.min + 1, info.max - 1, info.max, 0, 1} | ({-1} if info.min < 0 else set())
+    return np.array(sorted(vals), dtype=dtype)
+
+
+def random_dense(rng, size, dtype, max_run=4):
+    """A dense track of ``size`` positions in runs of 1..max_run equal values: half of the runs take a value of
+    extremes(dtype), the rest a random value of the whole range (neighbouring runs may be equal)."""
+    dtype = np.dtype(dtype)
+    lens = rng.integers(1, max_run + 1, size + 1)
+    n_runs = int(np.searchsorted(np.cumsum(lens), size)) + 1
+    lens = lens[:n_runs]
+    if dtype == np.bool_:
+        vals = rng.integers(0, 2, n_runs).astype(bool)
+    else:
+        info = np.iinfo(dtype)
+        vals = rng.integers(info.min, info.max, n_runs, dtype=dtype, endpoint=True)
+        pick = rng.integers(0, 2, n_runs).astype(bool)
+        ext = extremes(dtype)
+        vals[pick] = ext[rng.integers(0, ext.size, int(pick.sum()))]
+    return np.repeat(vals, lens)[:size]
+
+
+def empty_value(how, dtype):
+    """What a reduction gives for a row with no values (RaggedArray's rule): max the dtype's lowest value and min its
+    highest (False / True for bool), sum 0, mean NaN, any False."""
+    dtype = np.dtype(dtype)
+    if how in ("max", "min"):
+        if dtype == np.bool_:
+            return how == "min"
+        info = np.iinfo(dtype)
+        return info.min if how == "max" else info.max
+    return {"sum": 0, "mean": np.nan, "any": False}[how]
+
+
+def clip_queries(a, b, size):
+    """[a, b) clipped to [0, size) as the run-length arrays clip them: a to [0, size], b to [a, size]."""
+    a = np.clip(np.asarray(a, dtype=np.int64), 0, size)
+    b = np.minimum(np.maximum(np.asarray(b, dtype=np.int64), a), size)
+    return a, b
+
+
+def reduce_dense(dense, a, b, how):
+    """max / min / sum / mean / any of ``dense`` over [a, b) for every query, each query clipped to [0, size) first,
+    from the dense values alone (never the runs).  Vectorised: prefix sums for sum / mean / any and
+    np.maximum.reduceat / np.minimum.reduceat for max / min, so millions of queries and positions take well under a
+    second.  max / min keep the track's dtype; sum is int64 and wraps modulo 2^64 as the kernels do (NumPy's int64
+    array arithmetic wraps silently), so comparing int64 values compares the sums modulo 2^64; mean is float64 of that
+    int64 sum over the length, which is the true mean, rounded once, only where the true sum is below 2^53 in
+    magnitude (mean_is_exact); any is bool.  Empty rows give empty_value(how, dense.dtype)."""
+    dense = np.asarray(dense)
+    a, b = clip_queries(a, b, dense.size)
+    empty = b <= a
+    if how in ("max", "min"):
+        # a uint8 view of bool keeps reduceat to plain integer code; one spare element keeps every index in range
+        work = dense.view(np.uint8) if dense.dtype == np.bool_ else dense
+        work = np.concatenate([work, work[:1] if work.size else np.zeros(1, work.dtype)])
+        ufunc = np.maximum if how == "max" else np.minimum
+        got = ufunc.reduceat(work, np.stack([a, b], 1).reshape(-1))[0::2] if a.size else work[:0]
+        got = got.astype(dense.dtype)
+        got[empty] = empty_value(how, dense.dtype)
+        return got
+    if how == "any":
+        nonzero = np.concatenate([[0], np.cumsum(dense != 0, dtype=np.int64)])
+        return nonzero[b] - nonzero[a] > 0
+    prefix = np.concatenate([[0], np.cumsum(dense.astype(np.int64), dtype=np.int64)])
+    total = prefix[b] - prefix[a]
+    if how == "sum":
+        return total
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return total.astype(np.float64) / (b - a).astype(np.float64)
+
+
+def mean_is_exact(dense, a, b):
+    """Where the mean of reduce_dense is exact: the sum of |value| over the clipped row is below 2^52 (a float64
+    running sum of the row, in any order, is then exact too)."""
+    dense = np.asarray(dense)
+    a, b = clip_queries(a, b, dense.size)
+    mag = np.concatenate([[0.0], np.cumsum(np.abs(dense.astype(np.float64)))])
+    return mag[b] - mag[a] < 2.0 ** 52
+
+
+def reduce_loop(dense, a, b, how):
+    """reduce_dense as a plain loop over the positions of every query, sums in exact Python integers reduced
+    modulo 2^64 to int64 at the end."""
+    dense = np.asarray(dense)
+    out = []
+    for s, e in zip(*clip_queries(a, b, dense.size)):
+        vals = [int(v) for v in dense[s:e]]
+        if not vals:
+            out.append(empty_value(how, dense.dtype))
+        elif how == "max":
+            out.append(max(vals))
+        elif how == "min":
+            out.append(min(vals))
+        elif how == "any":
+            out.append(any(v != 0 for v in vals))
+        else:
+            total = sum(vals)
+            wrapped = (total + 2 ** 63) % 2 ** 64 - 2 ** 63
+            out.append(wrapped if how == "sum" else float(np.float64(wrapped) / np.float64(len(vals))))
+    return out
+
+
 def merge_intervals(starts, stops, distance=0):
     """arithmetics/intervals.py:270-304 line by line, on one chromosome: (kept row indices, merged stops)."""
     starts, stops = np.asarray(starts, dtype=np.int64), np.asarray(stops, dtype=np.int64)

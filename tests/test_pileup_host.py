@@ -265,3 +265,103 @@ def test_run_length_values_must_not_be_floating_point():
     with pytest.raises(TypeError, match="integers or bool"):
         GenomicRunLengthArray(events, torch.tensor([0.5, 1.0]))
     assert GenomicRunLengthArray(events, torch.tensor([1, 0]), 5).dtype == torch.int64
+
+
+DTYPES = [np.int64, np.int32, np.int16, np.int8, np.uint8, np.bool_]
+HOWS = ("max", "min", "sum", "mean", "any")
+
+
+def _same(got, want):
+    got, want = np.asarray(got), np.asarray(want)
+    assert got.shape == want.shape
+    if got.dtype.kind == "f" or want.dtype.kind == "f":
+        np.testing.assert_array_equal(got.astype(np.float64), want.astype(np.float64))
+    else:
+        assert got.tolist() == want.tolist()
+
+
+def _queries(rng, size, n):
+    """Random queries reaching 3 positions past both ends, reversed, empty and duplicated ones included."""
+    a = rng.integers(-3, size + 4, n)
+    b = np.where(rng.random(n) < 0.8, a + rng.integers(0, size // 2 + 3, n), rng.integers(-3, size + 4, n))
+    a[: n // 8], b[: n // 8] = a[n // 8: 2 * (n // 8)], b[n // 8: 2 * (n // 8)]
+    return a, b
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_dense_of_inverts_runs_of(dtype):
+    rng = np.random.default_rng(30)
+    for size in (0, 1, 2, 7, 100):
+        dense = po.random_dense(rng, size, dtype)
+        s, e, v = po.runs_of(dense)
+        back = po.dense_of(s, e, v)
+        assert back.dtype == dense.dtype and back.tolist() == dense.tolist()
+        assert np.all(v[1:] != v[:-1]) and (size == 0 or (s[0] == 0 and e[-1] == size))
+        again = po.runs_of(back)
+        assert all(x.tolist() == y.tolist() for x, y in zip((s, e, v), again))
+    assert po.dense_of([0, 2, 5], [2, 5, 6], [7, -1, 3], np.int8).tolist() == [7, 7, -1, -1, -1, 3]
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_dense_reducer_against_loop_and_runs(dtype):
+    """reduce_dense equals a plain loop over the positions of every query and, on the clipped queries, reduce_runs
+    (which works from the runs), for every dtype with its extreme values, empty rows following RaggedArray."""
+    rng = np.random.default_rng(31)
+    for size in (0, 1, 2, 5, 40, 300):
+        dense = po.random_dense(rng, size, dtype)
+        a, b = _queries(rng, size, 200)
+        a = np.concatenate([a, [0, size, -5, size + 5, 3, 0]])
+        b = np.concatenate([b, [size, size, -1, size + 9, 1, 0]])
+        for how in HOWS:
+            want = po.reduce_dense(dense, a, b, how)
+            _same(want, po.reduce_loop(dense, a, b, how))
+            if how in ("max", "min"):
+                assert want.dtype == dense.dtype
+            if size == 0 or how == "mean":
+                continue
+            s, e, v = po.runs_of(dense)
+            ca, cb = po.clip_queries(a, b, size)
+            runs = po.reduce_runs(s, e, v, ca, cb, how)
+            full = cb > ca
+            _same(want[full], runs[full].astype(want.dtype))
+            if dtype == np.int64 or how in ("sum", "any"):
+                _same(want, runs.astype(want.dtype))
+
+
+def test_dense_reducer_empty_rows():
+    dense = np.array([5, -3, 7], dtype=np.int16)
+    a, b = np.array([1, 2, 9, -4, 2]), np.array([1, 0, 12, -1, 3])
+    info = np.iinfo(np.int16)
+    assert po.reduce_dense(dense, a, b, "max").tolist() == [info.min] * 4 + [7]
+    assert po.reduce_dense(dense, a, b, "min").tolist() == [info.max] * 4 + [7]
+    assert po.reduce_dense(dense, a, b, "sum").tolist() == [0, 0, 0, 0, 7]
+    assert np.isnan(po.reduce_dense(dense, a, b, "mean")[:4]).all()
+    assert po.reduce_dense(dense, a, b, "any").tolist() == [False] * 4 + [True]
+    flags = np.array([True, False])
+    assert po.reduce_dense(flags, [0, 1, 1, 2], [0, 2, 1, 2], "max").tolist() == [False, False, False, False]
+    assert po.reduce_dense(flags, [0, 1, 1, 2], [0, 2, 1, 2], "min").tolist() == [True, False, True, True]
+    assert po.reduce_dense(flags, [0], [2], "max").tolist() == [True]
+
+
+def test_dense_reducer_wrapping_sums():
+    """Sums near and past 2^63 wrap modulo 2^64, as the kernels' uint64 arithmetic does: checked against exact Python
+    integers.  The mean is exact only where mean_is_exact says so."""
+    rng = np.random.default_rng(32)
+    lens = rng.integers(1, 50, 40)
+    vals = (1 << 62) + rng.integers(-1000, 1000, 40)
+    vals[::7] = -(1 << 62) - rng.integers(0, 1000, vals[::7].size)
+    dense = np.repeat(vals.astype(np.int64), lens)
+    a = rng.integers(0, dense.size, 300)
+    b = a + rng.integers(0, dense.size, 300)
+    got = po.reduce_dense(dense, a, b, "sum")
+    ca, cb = po.clip_queries(a, b, dense.size)
+    for g, s, e in zip(got, ca, cb):
+        exact = sum(int(v) for v in dense[s:e])
+        assert int(g) % 2 ** 64 == exact % 2 ** 64
+    assert (np.abs([sum(int(v) for v in dense[s:e]) for s, e in zip(ca, cb)]) >= 2 ** 63).any()   # some do wrap
+    _same(po.reduce_dense(dense, a, b, "mean"), po.reduce_loop(dense, a, b, "mean"))
+    exact = po.mean_is_exact(dense, a, b)
+    assert exact[cb - ca <= 0].all() and not exact[cb - ca > 2].any()
+    small = np.arange(-50, 50, dtype=np.int64)
+    assert po.mean_is_exact(small, [0, 10], [100, 90]).all()
+    assert po.reduce_dense(small, [0, 10], [100, 90], "mean").tolist() == [-0.5, -0.5]
