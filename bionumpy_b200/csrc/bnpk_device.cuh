@@ -10,6 +10,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "../../include/bnpk.h"
 
 namespace bnpk {
@@ -79,13 +80,60 @@ __device__ __forceinline__ uint64_t warp_sum_u64(uint64_t v) {
     return v;
 }
 
-// Decoupled look-back (single-pass chained scan).  Called by one full warp.  Publishes this
-// tile's aggregate, walks back over predecessors until an inclusive prefix is found, publishes
-// the tile's inclusive prefix and returns the exclusive one.  Tiles are handed out in
-// increasing order by an atomic ticket, so every predecessor is already running (or done).
-// The walk keeps kLookbackDepth windows of 32 predecessors in flight per round trip.
+// ---------------------------------------------------------------------------------------------
+// Single-pass scans: tiles of kScanTile items, handed out in increasing order by a ticket and chained by a decoupled
+// look-back.  A scan's workspace is kWsHeaderWords header words (the ticket) and one look-back state per tile,
+// zeroed before the launch (scan_workspace in bnpk_host.h).
+//
+// An operator is a type with `static uint64_t combine(uint64_t before, uint64_t after)`, associative and with
+// identity 0, on values of the 62-bit field of a look-back state.
+// ---------------------------------------------------------------------------------------------
+constexpr int kScanThreads = 256;
+constexpr int kScanItems = 8;
+constexpr int kScanTile = kScanThreads * kScanItems;
+constexpr int kScanWarps = kScanThreads / 32;
+
+struct Sum {
+    __device__ __forceinline__ static uint64_t combine(uint64_t before, uint64_t after) { return before + after; }
+};
+
+struct ScanSmem {
+    uint64_t warp[kScanWarps];
+    uint64_t base;
+    int64_t tile;
+};
+
+// The block's next tile, or -1 once the tiles [0, n_tiles) are all handed out.  Every thread of the block calls it,
+// and the loop body must pass a __syncthreads() before the next call (block_exclusive does).
+__device__ __forceinline__ int64_t next_tile(uint64_t *ws, int64_t n_tiles, ScanSmem &sm) {
+    if (threadIdx.x == 0) sm.tile = (int64_t)atomicAdd((unsigned long long *)(ws + kWsTicket), 1ull);
+    __syncthreads();
+    const int64_t tile = sm.tile;
+    return tile < n_tiles ? tile : -1;
+}
+
+// The words of the 32 lanes combined, a higher lane before a lower one, in every lane.
+template <class Op>
+__device__ __forceinline__ uint64_t warp_combine_down(uint64_t v, int lane) {
+    if constexpr (std::is_same<Op, Sum>::value) {
+        return warp_sum_u64(v);                             // a sum does not depend on the order
+    } else {
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint64_t t = __shfl_down_sync(0xffffffffu, v, o);
+            if (lane + o < 32) v = Op::combine(t, v);
+        }
+        return __shfl_sync(0xffffffffu, v, 0);
+    }
+}
+
+// Decoupled look-back.  Called by one full warp.  Publishes this tile's aggregate, walks back over predecessors until
+// an inclusive prefix is found, publishes the tile's inclusive prefix and returns the exclusive one.  Tiles are handed
+// out in increasing order by the ticket, so every predecessor is already running (or done).  The walk keeps
+// kLookbackDepth windows of 32 predecessors in flight per round trip; they are combined from the newest to the oldest.
 constexpr int kLookbackDepth = 4;
-__device__ __forceinline__ uint64_t lookback_exclusive(uint64_t *state, int64_t tile, uint64_t aggregate, int lane) {
+template <class Op>
+__device__ __forceinline__ uint64_t lookback(uint64_t *state, int64_t tile, uint64_t aggregate, int lane) {
     if (tile == 0) {
         if (lane == 0) st_relaxed(state, kFlagPrefix | aggregate);
         return 0;
@@ -128,14 +176,73 @@ __device__ __forceinline__ uint64_t lookback_exclusive(uint64_t *state, int64_t 
                     if (lane > first) v = 0;
                     done = true;
                 }
-                excl += warp_sum_u64(v);
+                excl = Op::combine(warp_combine_down<Op>(v, lane), excl);
             }
         }
         if (done) break;
         idx -= 32 * kLookbackDepth;
     }
-    if (lane == 0) st_relaxed(state + tile, kFlagPrefix | ((excl + aggregate) & kValueMask));
+    if (lane == 0) st_relaxed(state + tile, kFlagPrefix | (Op::combine(excl, aggregate) & kValueMask));
     return excl;
+}
+
+// The exclusive scan of one value per thread over the whole input: the block's scan, made global by look-back over
+// `state` (one word per tile).  Returns this thread's global exclusive prefix.  Every thread of the block calls it.
+template <class Op>
+__device__ __forceinline__ uint64_t block_exclusive(uint64_t v, int64_t tile, uint64_t *state, ScanSmem &sm) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint64_t inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint64_t t = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc = Op::combine(t, inc);
+    }
+    if (lane == 31) sm.warp[warp] = inc;
+    __syncthreads();
+    if (warp == 0) {
+        uint64_t winc = lane < kScanWarps ? sm.warp[lane] : 0;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint64_t t = __shfl_up_sync(0xffffffffu, winc, o);
+            if (lane >= o) winc = Op::combine(t, winc);
+        }
+        const uint64_t total = __shfl_sync(0xffffffffu, winc, kScanWarps - 1);
+        const uint64_t wex = __shfl_up_sync(0xffffffffu, winc, 1);
+        if (lane < kScanWarps) sm.warp[lane] = lane ? wex : 0;
+        const uint64_t excl = lookback<Op>(state, tile, total & kValueMask, lane);
+        if (lane == 0) sm.base = excl;
+    }
+    __syncthreads();
+    // an exclusive prefix is the inclusive one of the lane before: an operator need not have an inverse
+    const uint64_t lex = __shfl_up_sync(0xffffffffu, inc, 1);
+    const uint64_t r = Op::combine(Op::combine(sm.base, sm.warp[warp]), lane ? lex : 0);
+    __syncthreads();                                        // sm is free again
+    return r;
+}
+
+// offs[i] = size_of(0) + ... + size_of(i - 1) for i in [0, n], so offs[n] is the total, in one pass over a
+// one-scan workspace.  size_of(i) >= 0 is called once for every i < n.  Every thread of the block calls it.
+template <class F>
+__device__ __forceinline__ void exclusive_offsets(int64_t n, int64_t *offs, uint64_t *ws, F size_of) {
+    __shared__ ScanSmem sm;
+    const int64_t n_tiles = (n + kScanTile - 1) / kScanTile;
+    for (int64_t tile; (tile = next_tile(ws, n_tiles, sm)) >= 0;) {
+        const int64_t i0 = tile * kScanTile + (int64_t)threadIdx.x * kScanItems;
+        uint64_t v[kScanItems];
+        uint64_t sum = 0;
+#pragma unroll
+        for (int j = 0; j < kScanItems; ++j) {
+            v[j] = i0 + j < n ? size_of(i0 + j) : 0;
+            sum += v[j];
+        }
+        uint64_t o = block_exclusive<Sum>(sum, tile, ws + kWsHeaderWords, sm);
+#pragma unroll
+        for (int j = 0; j < kScanItems; ++j) {
+            if (i0 + j < n) offs[i0 + j] = (int64_t)o;
+            o += v[j];
+        }
+        if (tile == n_tiles - 1 && threadIdx.x == kScanThreads - 1) offs[n] = (int64_t)o;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -27,13 +27,6 @@ int ensure_dyn_smem(const void *kernel, int bytes);
         if (e__ != cudaSuccess) return ::bnpk::cuda_fail(e__, #expr); \
     } while (0)
 
-#define BNPK_LAUNCHED(name)                                         \
-    do {                                                            \
-        ::bnpk::g_launches.fetch_add(1, std::memory_order_relaxed); \
-        cudaError_t e__ = cudaGetLastError();                       \
-        if (e__ != cudaSuccess) return ::bnpk::cuda_fail(e__, name); \
-    } while (0)
-
 // optional per-launch timing of the dominant (tile) kernel, see bnpk_profile_* in bnpk.h
 void profile_before(cudaStream_t st);
 void profile_after(cudaStream_t st);
@@ -74,8 +67,9 @@ int launch(const char *name, void (*kern)(P...), unsigned grid, int block, size_
     if (profiled) profile_before(st);
     kern<<<grid, block, smem, st>>>(args...);
     if (profiled) profile_after(st);
-    BNPK_LAUNCHED(name);
-    return 0;
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_fail(e, name);
 }
 
 // A kernel that takes every CTA slot its shared memory leaves: raises its dynamic shared-memory limit to smem_max,
@@ -90,6 +84,17 @@ int launch_resident(const char *name, const char *misfit, void (*kern)(P...), si
     if (per_sm < 1) return set_err(BNPK_E_BINS, misfit);
     if (ctas_wanted == 0) return 0;
     return launch(name, kern, grid_cap(ctas_wanted, per_sm), block, smem, st, profiled, args...);
+}
+
+// The workspace of a single-pass scan of n items (bnpk_device.cuh) that runs n_scans look-backs: sets n_tiles (at
+// least one), refuses a workspace smaller than the header and n_scans states per tile, and zeroes that much on st.
+inline int scan_workspace(size_t n, int n_scans, void *workspace, size_t workspace_bytes, cudaStream_t st,
+                          size_t &n_tiles) {
+    n_tiles = std::max<size_t>((n + kScanTile - 1) / kScanTile, 1);
+    const size_t need = (kWsHeaderWords + n_scans * n_tiles) * sizeof(uint64_t);
+    if (workspace_bytes < need) return set_err(BNPK_E_WORKSPACE, "workspace too small");
+    BNPK_CUDA(cudaMemsetAsync(workspace, 0, need, st));
+    return 0;
 }
 
 size_t tile_workspace_bytes(size_t n);

@@ -101,66 +101,12 @@ __global__ void __launch_bounds__(256) count_byte_kernel(const uint8_t *chunk, s
 // ------------------------------------------------------------------------------------------
 // ragged offsets: exclusive prefix sum of max(len - shrink, 0), single pass (look-back)
 // ------------------------------------------------------------------------------------------
-constexpr int kScanThreads = 256;
-constexpr int kScanItems = 8;
-constexpr int kScanTile = kScanThreads * kScanItems;
-
 __global__ void __launch_bounds__(kScanThreads) row_offsets_kernel(const int32_t *lens, size_t n, int shrink,
                                                                    int64_t *offsets, uint64_t *ws) {
-    __shared__ uint64_t s_warp[kScanThreads / 32 + 1];
-    __shared__ int64_t s_tile;
-    __shared__ uint64_t s_base;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    uint64_t *state = ws + kWsHeaderWords;
-    const int64_t n_tiles = (int64_t)((n + kScanTile - 1) / kScanTile);
-    while (true) {
-        if (tid == 0) s_tile = (int64_t)atomicAdd((unsigned long long *)(ws + kWsTicket), 1ull);
-        __syncthreads();
-        const int64_t tile = s_tile;
-        if (tile >= n_tiles) break;
-        const size_t r0 = (size_t)tile * kScanTile + (size_t)tid * kScanItems;
-        uint64_t v[kScanItems];
-        uint64_t sum = 0;
-#pragma unroll
-        for (int i = 0; i < kScanItems; ++i) {
-            int64_t l = 0;
-            if (r0 + i < n) l = (int64_t)lens[r0 + i] - shrink;
-            v[i] = l > 0 ? (uint64_t)l : 0;
-            sum += v[i];
-        }
-        uint64_t inc = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint64_t t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
-        }
-        if (lane == 31) s_warp[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-            uint64_t w = lane < kScanThreads / 32 ? s_warp[lane] : 0;
-            uint64_t winc = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint64_t t = __shfl_up_sync(0xffffffffu, winc, o);
-                if (lane >= o) winc += t;
-            }
-            const uint64_t total = __shfl_sync(0xffffffffu, winc, kScanThreads / 32 - 1);
-            if (lane < kScanThreads / 32) s_warp[lane] = winc - w;
-            const uint64_t excl = lookback_exclusive(state, tile, total, lane);
-            if (lane == 0) {
-                s_base = excl;
-                if (tile == n_tiles - 1) offsets[n] = (int64_t)(excl + total);
-            }
-        }
-        __syncthreads();
-        uint64_t run = s_base + s_warp[warp] + inc - sum;
-#pragma unroll
-        for (int i = 0; i < kScanItems; ++i) {
-            if (r0 + i < n) offsets[r0 + i] = (int64_t)run;
-            run += v[i];
-        }
-        __syncthreads();
-    }
+    exclusive_offsets((int64_t)n, offsets, ws, [&](int64_t i) -> uint64_t {
+        const int64_t l = (int64_t)lens[i] - shrink;
+        return l > 0 ? (uint64_t)l : 0;
+    });
 }
 
 // ------------------------------------------------------------------------------------------
@@ -346,21 +292,16 @@ int bnpk_profile_read(double *total_ms, uint64_t *n_launches) {
 }
 
 int bnpk_status_init(int64_t *status, void *stream) {
-    status_init_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(status);
-    BNPK_LAUNCHED("status_init_kernel");
-    return 0;
+    return launch("status_init_kernel", status_init_kernel, 1, 32, 0, (cudaStream_t)stream, false, status);
 }
 
 int bnpk_count_byte(const uint8_t *chunk, size_t n, uint8_t value, int64_t *count_out, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     BNPK_CUDA(cudaMemsetAsync(count_out, 0, sizeof(int64_t), st));
     if (n == 0) return 0;
-    const size_t want = (n / 16 + 255) / 256;
-    const unsigned grid = grid_cap(want, 8);
     const uint32_t pattern = 0x01010101u * value;
-    count_byte_kernel<<<grid, 256, 0, st>>>(chunk, n, pattern, (unsigned long long *)count_out);
-    BNPK_LAUNCHED("count_byte_kernel");
-    return 0;
+    return launch("count_byte_kernel", count_byte_kernel, grid_cap((n / 16 + 255) / 256, 8), 256, 0, st, false, chunk, n,
+                  pattern, (unsigned long long *)count_out);
 }
 
 size_t bnpk_tile_workspace_bytes(size_t n) { return tile_workspace_bytes(n); }
@@ -393,14 +334,10 @@ int bnpk_row_offsets(const int32_t *lens, size_t n_rows, int shrink, int64_t *of
         BNPK_CUDA(cudaMemsetAsync(offsets, 0, sizeof(int64_t), st));
         return 0;
     }
-    const size_t n_tiles = (n_rows + kScanTile - 1) / kScanTile;
-    const size_t need = (kWsHeaderWords + n_tiles) * sizeof(uint64_t);
-    if (workspace_bytes < need) return set_err(BNPK_E_WORKSPACE, "workspace too small");
-    BNPK_CUDA(cudaMemsetAsync(workspace, 0, need, st));
-    const unsigned grid = grid_cap(n_tiles, 4);
-    row_offsets_kernel<<<grid, kScanThreads, 0, st>>>(lens, n_rows, shrink, offsets, (uint64_t *)workspace);
-    BNPK_LAUNCHED("row_offsets_kernel");
-    return 0;
+    size_t n_tiles;
+    if (int rc = scan_workspace(n_rows, 1, workspace, workspace_bytes, st, n_tiles)) return rc;
+    return launch("row_offsets_kernel", row_offsets_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st, false, lens,
+                  n_rows, shrink, offsets, (uint64_t *)workspace);
 }
 
 int bnpk_bincount(const int64_t *values, size_t n, int64_t n_bins, int hist_mode, int64_t *hist, int64_t *status,
@@ -416,76 +353,58 @@ int bnpk_bincount(const int64_t *values, size_t n, int64_t n_bins, int hist_mode
         const size_t smem = (size_t)n_bins * 4;
         int per_sm = 1;
         BNPK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bincount_kernel<true>, 512, smem));
-        const unsigned grid = grid_cap(want, std::max(per_sm, 1));
-        bincount_kernel<true><<<grid, 512, smem, st>>>(values, n, (uint64_t)n_bins, (unsigned long long *)hist, status);
-    } else {
-        const unsigned grid = grid_cap(want, 4);
-        bincount_kernel<false><<<grid, 512, 0, st>>>(values, n, (uint64_t)n_bins, (unsigned long long *)hist, status);
+        return launch("bincount_kernel", bincount_kernel<true>, grid_cap(want, std::max(per_sm, 1)), 512, smem, st,
+                      false, values, n, (uint64_t)n_bins, (unsigned long long *)hist, status);
     }
-    BNPK_LAUNCHED("bincount_kernel");
-    return 0;
+    return launch("bincount_kernel", bincount_kernel<false>, grid_cap(want, 4), 512, 0, st, false, values, n,
+                  (uint64_t)n_bins, (unsigned long long *)hist, status);
 }
 
 int bnpk_bincount_rows(const int64_t *values, const int64_t *offsets, size_t n_rows, int64_t n_bins, int64_t *out,
                        int64_t *status, void *stream) {
     if (n_bins < 1) return set_err(BNPK_E_BINS, "n_bins must be positive");
     if (n_rows == 0) return 0;
-    const size_t want = (n_rows + 7) / 8;
-    const unsigned grid = grid_cap(want, 8);
-    bincount_rows_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(values, offsets, n_rows, (uint64_t)n_bins,
-                                                                 (unsigned long long *)out, status);
-    BNPK_LAUNCHED("bincount_rows_kernel");
-    return 0;
+    return launch("bincount_rows_kernel", bincount_rows_kernel, grid_cap((n_rows + 7) / 8, 8), 256, 0,
+                  (cudaStream_t)stream, false, values, offsets, n_rows, (uint64_t)n_bins, (unsigned long long *)out,
+                  status);
 }
 
 int bnpk_multiline_flags(const uint8_t *chunk, size_t n, const int64_t *line_starts, const int32_t *line_lens, size_t n_lines,
                          int32_t *is_header, int64_t *out2, void *stream) {
     if (n_lines == 0 || n == 0) return 0;
-    const unsigned grid = grid_cap((n_lines + 255) / 256, 8);
-    multiline_flags_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(chunk, n, line_starts, line_lens, n_lines, is_header, out2);
-    BNPK_LAUNCHED("multiline_flags_kernel");
-    return 0;
+    return launch("multiline_flags_kernel", multiline_flags_kernel, grid_cap((n_lines + 255) / 256, 8), 256, 0,
+                  (cudaStream_t)stream, false, chunk, n, line_starts, line_lens, n_lines, is_header, out2);
 }
 
 int bnpk_multiline_entries(const uint8_t *chunk, const int64_t *line_starts, const int32_t *line_lens, const int32_t *is_header,
                            const int64_t *hdr_before, size_t keep, int trim_cr, int64_t *h_starts, int32_t *h_lens,
                            int64_t *s_starts, int32_t *s_lens, int64_t *entry_lens, void *stream) {
     if (keep == 0) return 0;
-    const unsigned grid = grid_cap((keep + 255) / 256, 8);
-    multiline_entries_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(chunk, line_starts, line_lens, is_header, hdr_before, keep, trim_cr,
-                                                                     h_starts, h_lens, s_starts, s_lens,
-                                                                     (unsigned long long *)entry_lens);
-    BNPK_LAUNCHED("multiline_entries_kernel");
-    return 0;
+    return launch("multiline_entries_kernel", multiline_entries_kernel, grid_cap((keep + 255) / 256, 8), 256, 0,
+                  (cudaStream_t)stream, false, chunk, line_starts, line_lens, is_header, hdr_before, keep, trim_cr,
+                  h_starts, h_lens, s_starts, s_lens, (unsigned long long *)entry_lens);
 }
 
 int bnpk_bloom_insert(const int64_t *values, size_t n, const int64_t *offsets, int n_hash, uint8_t *mask, size_t mask_size,
                       void *stream) {
     if (n_hash < 1 || mask_size == 0) return set_err(BNPK_E_BADARG, "bloom filter needs hash functions and a mask");
     if (n == 0) return 0;
-    const unsigned grid = grid_cap((n + 255) / 256, 16);
-    bloom_insert_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(values, n, offsets, n_hash, mask, (uint64_t)mask_size);
-    BNPK_LAUNCHED("bloom_insert_kernel");
-    return 0;
+    return launch("bloom_insert_kernel", bloom_insert_kernel, grid_cap((n + 255) / 256, 16), 256, 0,
+                  (cudaStream_t)stream, false, values, n, offsets, n_hash, mask, (uint64_t)mask_size);
 }
 
 int bnpk_bloom_query(const int64_t *values, size_t n, const int64_t *offsets, int n_hash, const uint8_t *mask, size_t mask_size,
                      uint8_t *out, void *stream) {
     if (n_hash < 1 || mask_size == 0) return set_err(BNPK_E_BADARG, "bloom filter needs hash functions and a mask");
     if (n == 0) return 0;
-    const unsigned grid = grid_cap((n + 255) / 256, 16);
-    bloom_query_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(values, n, offsets, n_hash, mask, (uint64_t)mask_size, out);
-    BNPK_LAUNCHED("bloom_query_kernel");
-    return 0;
+    return launch("bloom_query_kernel", bloom_query_kernel, grid_cap((n + 255) / 256, 16), 256, 0,
+                  (cudaStream_t)stream, false, values, n, offsets, n_hash, mask, (uint64_t)mask_size, out);
 }
 
 int bnpk_synth_fastq(uint8_t *out, uint64_t first_record, uint64_t n_records, uint64_t seed, void *stream) {
     if (n_records == 0) return 0;
-    const uint64_t want = (n_records + 7) / 8;
-    const unsigned grid = grid_cap(want, 16);
-    synth_fastq_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(out, first_record, n_records, seed);
-    BNPK_LAUNCHED("synth_fastq_kernel");
-    return 0;
+    return launch("synth_fastq_kernel", synth_fastq_kernel, grid_cap((n_records + 7) / 8, 16), 256, 0,
+                  (cudaStream_t)stream, false, out, first_record, n_records, seed);
 }
 
 }  // extern "C"

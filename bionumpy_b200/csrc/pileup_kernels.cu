@@ -22,9 +22,6 @@ namespace bnpk {
 
 namespace {
 
-constexpr int kScanThreads = 256;
-constexpr int kScanItems = 8;
-constexpr int kScanTile = kScanThreads * kScanItems;
 constexpr int kWalkItems = 16;
 constexpr uint64_t kBias = 1ull << 59;          // merge: stop + kBias in [0, 2^60)
 constexpr uint64_t kReset = 1ull << 61;         // merge: "a segment starts here" in the scanned word
@@ -55,41 +52,6 @@ __device__ __forceinline__ int64_t upper_bound(const int64_t *a, int64_t lo, int
         else hi = mid;
     }
     return lo;
-}
-
-// The block's exclusive sum of one value per thread, made global by look-back over `state`: returns this thread's
-// global exclusive prefix (mod 2^62) and leaves the tile's total in *s_total.  Every thread of the block calls it.
-__device__ __forceinline__ uint64_t tile_exclusive_sum(uint64_t v, int64_t tile, uint64_t *state, uint64_t *s_warp,
-                                                       uint64_t *s_base, uint64_t *s_total) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    uint64_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint64_t t = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += t;
-    }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-        const uint64_t w = lane < kScanThreads / 32 ? s_warp[lane] : 0;
-        uint64_t winc = w;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint64_t t = __shfl_up_sync(0xffffffffu, winc, o);
-            if (lane >= o) winc += t;
-        }
-        const uint64_t total = __shfl_sync(0xffffffffu, winc, kScanThreads / 32 - 1);
-        if (lane < kScanThreads / 32) s_warp[lane] = winc - w;
-        const uint64_t excl = lookback_exclusive(state, tile, total & kValueMask, lane);
-        if (lane == 0) {
-            *s_base = excl;
-            *s_total = total;
-        }
-    }
-    __syncthreads();
-    const uint64_t r = *s_base + s_warp[warp] + inc - v;
-    __syncthreads();                                   // s_warp and s_base are free again
-    return r;
 }
 
 // --------------------------------------------------------------------------------------------------------------------
@@ -135,18 +97,12 @@ __global__ void __launch_bounds__(256) interval_events_kernel(const __grid_const
 __global__ void __launch_bounds__(kScanThreads) pileup_runs_kernel(const int64_t *keys, int64_t n, int64_t size,
                                                                    int any_mode, int64_t *run_starts,
                                                                    int64_t *run_values, int64_t *n_runs, uint64_t *ws) {
-    __shared__ uint64_t s_warp[kScanThreads / 32];
-    __shared__ uint64_t s_base, s_total;
-    __shared__ int64_t s_tile;
+    __shared__ ScanSmem sm;
     const int tid = threadIdx.x;
     const int64_t n_tiles = n > 0 ? (n + kScanTile - 1) / kScanTile : 1;
     uint64_t *cov_state = ws + kWsHeaderWords;
     uint64_t *run_state = cov_state + n_tiles;
-    while (true) {
-        if (tid == 0) s_tile = (int64_t)atomicAdd((unsigned long long *)(ws + kWsTicket), 1ull);
-        __syncthreads();
-        const int64_t tile = s_tile;
-        if (tile >= n_tiles) break;
+    for (int64_t tile; (tile = next_tile(ws, n_tiles, sm)) >= 0;) {
         const int64_t i0 = tile * kScanTile + (int64_t)tid * kScanItems;
         int64_t k[kScanItems];
         int64_t dsum = 0;
@@ -157,7 +113,7 @@ __global__ void __launch_bounds__(kScanThreads) pileup_runs_kernel(const int64_t
         }
         const int64_t prev_pos = i0 > 0 && i0 <= n ? keys[i0 - 1] >> 1 : INT64_MIN;
         const int64_t next_pos = i0 + kScanItems < n ? keys[i0 + kScanItems] >> 1 : INT64_MAX;
-        int64_t cov = signed62(tile_exclusive_sum((uint64_t)dsum, tile, cov_state, s_warp, &s_base, &s_total));
+        int64_t cov = signed62(block_exclusive<Sum>((uint64_t)dsum, tile, cov_state, sm));
         // the runs of this thread: where the coverage after a position's last key differs from the coverage before
         // its first key; position 0 always starts a run, and when no key is at 0, the run (0, 0) is the first
         int64_t val[kScanItems];
@@ -191,7 +147,7 @@ __global__ void __launch_bounds__(kScanThreads) pileup_runs_kernel(const int64_t
             }
         }
         const uint64_t n_emit = (uint64_t)__popc(emit) + lead_zero;
-        uint64_t o = tile_exclusive_sum(n_emit, tile, run_state, s_warp, &s_base, &s_total);
+        uint64_t o = block_exclusive<Sum>(n_emit, tile, run_state, sm);
         if (lead_zero) {
             run_starts[o] = 0;
             run_values[o] = 0;
@@ -251,32 +207,7 @@ __global__ void __launch_bounds__(256) runs_locate_kernel(const __grid_constant_
 
 __global__ void __launch_bounds__(kScanThreads) count_scan_kernel(const int64_t *count, int64_t n, int64_t *offs,
                                                                   uint64_t *ws) {
-    __shared__ uint64_t s_warp[kScanThreads / 32];
-    __shared__ uint64_t s_base, s_total;
-    __shared__ int64_t s_tile;
-    const int tid = threadIdx.x;
-    const int64_t n_tiles = (n + kScanTile - 1) / kScanTile;
-    while (true) {
-        if (tid == 0) s_tile = (int64_t)atomicAdd((unsigned long long *)(ws + kWsTicket), 1ull);
-        __syncthreads();
-        const int64_t tile = s_tile;
-        if (tile >= n_tiles) break;
-        const int64_t i0 = tile * kScanTile + (int64_t)tid * kScanItems;
-        int64_t c[kScanItems];
-        uint64_t sum = 0;
-#pragma unroll
-        for (int j = 0; j < kScanItems; ++j) {
-            c[j] = i0 + j < n ? count[i0 + j] : 0;
-            sum += (uint64_t)c[j];
-        }
-        uint64_t o = tile_exclusive_sum(sum, tile, ws + kWsHeaderWords, s_warp, &s_base, &s_total);
-#pragma unroll
-        for (int j = 0; j < kScanItems; ++j) {
-            if (i0 + j < n) offs[i0 + j] = (int64_t)o;
-            o += (uint64_t)c[j];
-        }
-        if (tile == n_tiles - 1 && tid == kScanThreads - 1) offs[n] = (int64_t)o;
-    }
+    exclusive_offsets(n, offs, ws, [&](int64_t i) { return (uint64_t)count[i]; });
 }
 
 __device__ __forceinline__ int64_t combine(int mode, int64_t acc, int64_t v, int64_t overlap) {
@@ -378,47 +309,12 @@ __global__ void __launch_bounds__(256) runs_extract_kernel(const __grid_constant
 // --------------------------------------------------------------------------------------------------------------------
 // merge
 // --------------------------------------------------------------------------------------------------------------------
-// The ordered segmented maximum of two scanned words, `x` before `y`: y alone when a segment starts in y.
-__device__ __forceinline__ uint64_t seg_max(uint64_t x, uint64_t y) {
-    return (y & kReset) ? y : (x & kReset) | max(x & ~kReset, y);
-}
-
-// lookback_exclusive with seg_max for the sum: the words of the tiles before `tile`, combined in order.  Called by one
-// full warp; `aggregate` is the tile's own combined word.
-__device__ __forceinline__ uint64_t lookback_seg_max(uint64_t *state, int64_t tile, uint64_t aggregate, int lane) {
-    if (tile == 0) {
-        if (lane == 0) st_relaxed(state, kFlagPrefix | aggregate);
-        return 0;
+// The ordered segmented maximum of two scanned words, `before` and `after`: `after` alone when a segment starts in it.
+struct SegMax {
+    __device__ __forceinline__ static uint64_t combine(uint64_t before, uint64_t after) {
+        return (after & kReset) ? after : (before & kReset) | max(before & ~kReset, after);
     }
-    if (lane == 0) st_relaxed(state + tile, kFlagAgg | aggregate);
-    uint64_t excl = 0;                 // the identity: no segment start, the lowest biased stop
-    int64_t idx = tile - 1;
-    while (true) {
-        uint64_t s;
-        unsigned pref;
-        do {
-            const int64_t j = idx - lane;
-            s = j >= 0 ? ld_relaxed(state + j) : kFlagPrefix;
-            const unsigned zero = __ballot_sync(0xffffffffu, (s >> 62) == 0);
-            pref = __ballot_sync(0xffffffffu, (s >> 62) == 2);
-            const unsigned before = pref ? ((pref & (0u - pref)) - 1u) : 0xffffffffu;
-            if (!(zero & before)) break;
-        } while (true);
-        const int first = pref ? __ffs(pref) - 1 : 32;
-        uint64_t v = lane <= first ? (s & kValueMask) : 0;
-        // lane l + o lies before lane l: combine in that order
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint64_t t = __shfl_down_sync(0xffffffffu, v, o);
-            if (lane + o < 32) v = seg_max(t, v);
-        }
-        excl = seg_max(__shfl_sync(0xffffffffu, v, 0), excl);
-        if (pref) break;
-        idx -= 32;
-    }
-    if (lane == 0) st_relaxed(state + tile, kFlagPrefix | (seg_max(excl, aggregate) & kValueMask));
-    return excl;
-}
+};
 
 struct MergeArgs {
     const int64_t *start, *stop;
@@ -429,19 +325,13 @@ struct MergeArgs {
 };
 
 __global__ void __launch_bounds__(kScanThreads) interval_merge_kernel(const __grid_constant__ MergeArgs a) {
-    __shared__ uint64_t s_warp[kScanThreads / 32];
-    __shared__ uint64_t s_base, s_total;
-    __shared__ int64_t s_tile;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    __shared__ ScanSmem sm;
+    const int tid = threadIdx.x;
     const int64_t n_tiles = (a.n + kScanTile - 1) / kScanTile;
     uint64_t *max_state = a.ws + kWsHeaderWords;
     uint64_t *grp_state = max_state + n_tiles;
     const int64_t d = a.distance;
-    while (true) {
-        if (tid == 0) s_tile = (int64_t)atomicAdd((unsigned long long *)(a.ws + kWsTicket), 1ull);
-        __syncthreads();
-        const int64_t tile = s_tile;
-        if (tile >= n_tiles) break;
+    for (int64_t tile; (tile = next_tile(a.ws, n_tiles, sm)) >= 0;) {
         const int64_t i0 = tile * kScanTile + (int64_t)tid * kScanItems;
         int64_t st[kScanItems + 1], sp[kScanItems];
         bool seg[kScanItems + 1];
@@ -453,36 +343,11 @@ __global__ void __launch_bounds__(kScanThreads) interval_merge_kernel(const __gr
             seg[j] = i >= a.n || i == 0 || (a.same_prev && !a.same_prev[i]);   // no flags: one segment
             if (j < kScanItems) {
                 sp[j] = i < a.n ? a.stop[i] : 0;
-                if (i < a.n) agg = seg_max(agg, (seg[j] ? kReset : 0) | (uint64_t)(sp[j] + (int64_t)kBias));
+                if (i < a.n) agg = SegMax::combine(agg, (seg[j] ? kReset : 0) | (uint64_t)(sp[j] + (int64_t)kBias));
             }
         }
-        // the segmented max of the threads before this one in the tile, then of the tiles before
-        uint64_t inc = agg;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint64_t t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc = seg_max(t, inc);
-        }
-        if (lane == 31) s_warp[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-            const uint64_t w = lane < kScanThreads / 32 ? s_warp[lane] : 0;
-            uint64_t winc = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint64_t t = __shfl_up_sync(0xffffffffu, winc, o);
-                if (lane >= o) winc = seg_max(t, winc);
-            }
-            const uint64_t total = __shfl_sync(0xffffffffu, winc, kScanThreads / 32 - 1);
-            const uint64_t wex = __shfl_up_sync(0xffffffffu, winc, 1);
-            if (lane < kScanThreads / 32) s_warp[lane] = lane ? wex : 0;
-            const uint64_t excl = lookback_seg_max(max_state, tile, total, lane);
-            if (lane == 0) s_base = excl;
-        }
-        __syncthreads();
-        const uint64_t lex = __shfl_up_sync(0xffffffffu, inc, 1);
-        uint64_t run = seg_max(seg_max(s_base, s_warp[warp]), lane ? lex : 0);
-        __syncthreads();
+        // the segmented max of the rows before this thread's first row
+        uint64_t run = block_exclusive<SegMax>(agg, tile, max_state, sm);
         // running max before each row (within its segment), the group starts and ends
         const int64_t prev_start = i0 > 0 && i0 <= a.n ? a.start[i0 - 1] : 0;
         int64_t incl[kScanItems];
@@ -494,7 +359,7 @@ __global__ void __launch_bounds__(kScanThreads) interval_merge_kernel(const __gr
             const int64_t before = (int64_t)(run & ~kReset) - (int64_t)kBias;
             if (seg[j] || st[j] > before + d) first |= 1u << j;
             if (!seg[j] && st[j] < (j ? st[j - 1] : prev_start)) report(a.status, i);
-            run = seg_max(run, (seg[j] ? kReset : 0) | (uint64_t)(sp[j] + (int64_t)kBias));
+            run = SegMax::combine(run, (seg[j] ? kReset : 0) | (uint64_t)(sp[j] + (int64_t)kBias));
             incl[j] = (int64_t)(run & ~kReset) - (int64_t)kBias;
         }
 #pragma unroll
@@ -503,7 +368,7 @@ __global__ void __launch_bounds__(kScanThreads) interval_merge_kernel(const __gr
             if (i >= a.n) break;
             if (seg[j + 1] || st[j + 1] > incl[j] + d) last |= 1u << j;
         }
-        uint64_t g = tile_exclusive_sum((uint64_t)__popc(first), tile, grp_state, s_warp, &s_base, &s_total);
+        uint64_t g = block_exclusive<Sum>((uint64_t)__popc(first), tile, grp_state, sm);
 #pragma unroll
         for (int j = 0; j < kScanItems; ++j) {
             if (first >> j & 1) a.out_rows[g++] = i0 + j;
@@ -554,11 +419,9 @@ int bnpk_pileup_runs(const int64_t *keys, size_t n_keys, int64_t size, int mode,
     if (size < 0 || size >= kMaxPos) return set_err(BNPK_E_BADARG, "size must be in [0, 2^59)");
     if ((n_keys && !keys) || !run_starts || !run_values || !n_runs || !workspace)
         return set_err(BNPK_E_BADARG, "keys, run_starts, run_values, n_runs and workspace are required");
-    const size_t n_tiles = std::max<size_t>((n_keys + kScanTile - 1) / kScanTile, 1);
-    const size_t need = (kWsHeaderWords + 2 * n_tiles) * sizeof(uint64_t);
-    if (workspace_bytes < need) return set_err(BNPK_E_WORKSPACE, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    BNPK_CUDA(cudaMemsetAsync(workspace, 0, need, st));
+    size_t n_tiles;
+    if (int rc = scan_workspace(n_keys, 2, workspace, workspace_bytes, st, n_tiles)) return rc;
     return launch("pileup_runs_kernel", pileup_runs_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st, false,
                   (const int64_t *)keys, (int64_t)n_keys, size, (int)(mode == BNPK_PILEUP_ANY), run_starts, run_values,
                   n_runs, (uint64_t *)workspace);
@@ -572,13 +435,11 @@ int bnpk_runs_reduce(const int64_t *run_starts, const int64_t *values, size_t n_
     if (n_q == 0) return 0;
     if (!q_start || !q_stop || !out || !scratch || !workspace)
         return set_err(BNPK_E_BADARG, "q_start, q_stop, out, scratch and workspace are required");
-    const size_t n_tiles = (n_q + kScanTile - 1) / kScanTile;
-    const size_t need = (kWsHeaderWords + n_tiles) * sizeof(uint64_t);
-    if (workspace_bytes < need) return set_err(BNPK_E_WORKSPACE, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
+    size_t n_tiles;
+    if (int rc = scan_workspace(n_q, 1, workspace, workspace_bytes, st, n_tiles)) return rc;
     RunArgs a{run_starts, values, (int64_t)n_runs, q_start, q_stop, (int64_t)n_q, mode,
               scratch, scratch + n_q, scratch + 2 * n_q, out};
-    BNPK_CUDA(cudaMemsetAsync(workspace, 0, need, st));
     int rc = launch("runs_locate_kernel", runs_locate_kernel, grid_cap((n_q + 255) / 256, 8), 256, 0, st, false, a);
     if (rc) return rc;
     rc = launch("count_scan_kernel", count_scan_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st, false,
@@ -610,10 +471,8 @@ int bnpk_interval_merge(const int64_t *start, const int64_t *stop, const uint8_t
     }
     if (!start || !stop || !out_rows || !out_stops || !status || !workspace)
         return set_err(BNPK_E_BADARG, "start, stop, out_rows, out_stops, status and workspace are required");
-    const size_t n_tiles = (n_rows + kScanTile - 1) / kScanTile;
-    const size_t need = (kWsHeaderWords + 2 * n_tiles) * sizeof(uint64_t);
-    if (workspace_bytes < need) return set_err(BNPK_E_WORKSPACE, "workspace too small");
-    BNPK_CUDA(cudaMemsetAsync(workspace, 0, need, st));
+    size_t n_tiles;
+    if (int rc = scan_workspace(n_rows, 2, workspace, workspace_bytes, st, n_tiles)) return rc;
     MergeArgs a{start, stop, same_prev, (int64_t)n_rows, distance, out_rows, out_stops, n_out, status,
                 (uint64_t *)workspace};
     return launch("interval_merge_kernel", interval_merge_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st, false, a);

@@ -743,11 +743,9 @@ static int launch_pwm(const uint8_t *base, size_t base_bytes, const int64_t *sta
     auto kern = rows_pwm_generic_kernel<SCORES>;
     const size_t smem = (size_t)alphabet_size * motif_len * sizeof(double) + 256;
     BNPK_DYN_SMEM(kern, kPwmMaxCells * sizeof(double) + 256);
-    kern<<<grid_cap((n_rows + 7) / 8, 8), 256, smem, st>>>(base, starts, lens, n_rows,
-                                                           enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size,
-                                                           matrix, motif_len, tail, offsets, out, status);
-    BNPK_LAUNCHED("rows_pwm_generic_kernel");
-    return 0;
+    return launch("rows_pwm_generic_kernel", kern, grid_cap((n_rows + 7) / 8, 8), 256, smem, st, false, base, starts,
+                  lens, n_rows, enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size, matrix, motif_len, tail,
+                  offsets, out, status);
 }
 
 // The limits of bnpk_rows_match*, and the kernels' view of the pattern in `m`.
@@ -792,11 +790,9 @@ static int launch_match(const uint8_t *base, size_t base_bytes, const int64_t *s
     auto kern = rows_match_generic_kernel<OUT>;
     const size_t smem = kMatchSmemHead + (size_t)m.n_words * 4 + 256;
     BNPK_DYN_SMEM(kern, kMatchSmemHead + kMatchMaxWords * 4 + 256);
-    kern<<<grid_cap((n_rows + 7) / 8, 8), 256, smem, st>>>(base, starts, lens, n_rows,
-                                                           enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size,
-                                                           m, offsets, out, status);
-    BNPK_LAUNCHED("rows_match_generic_kernel");
-    return 0;
+    return launch("rows_match_generic_kernel", kern, grid_cap((n_rows + 7) / 8, 8), 256, smem, st, false, base,
+                  starts, lens, n_rows, enc_mode == BNPK_ENC_LUT ? lut256 : nullptr, alphabet_size, m, offsets, out,
+                  status);
 }
 
 static uint64_t canon_pattern(int complement_xor) {
@@ -877,10 +873,9 @@ int bnpk_rows_generic_hash(const uint8_t *base, size_t base_bytes, const int64_t
     if (k < 1 || k > 63) return set_err(BNPK_E_K, "k must be in 1..63 for the generic hash");
     if (alphabet_size < 2 || alphabet_size > 255) return set_err(BNPK_E_BADARG, "alphabet_size must be in 2..255");
     if (n_rows == 0) return 0;
-    rows_generic_hash_kernel<<<grid_cap((n_rows + 7) / 8, 8), 256, 0, (cudaStream_t)stream>>>(
-        base, base_bytes, starts, lens, n_rows, lut256, alphabet_size, k, offsets, hashes_out, status);
-    BNPK_LAUNCHED("rows_generic_hash_kernel");
-    return 0;
+    return launch("rows_generic_hash_kernel", rows_generic_hash_kernel, grid_cap((n_rows + 7) / 8, 8), 256, 0,
+                  (cudaStream_t)stream, false, base, base_bytes, starts, lens, n_rows, lut256, alphabet_size, k,
+                  offsets, hashes_out, status);
 }
 
 int bnpk_rows_minimizers(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
@@ -937,10 +932,8 @@ int bnpk_kmer_table_rehash(const int64_t *keys, const int64_t *counts, size_t ca
     KmerTable t;
     t.keys = (unsigned long long *)new_keys; t.counts = (unsigned long long *)new_counts;
     t.mask = new_capacity - 1; t.n_used = (unsigned long long *)n_used;
-    table_rehash_kernel<<<grid_cap((capacity + 255) / 256, 8), 256, 0, (cudaStream_t)stream>>>(keys, counts, capacity, t,
-                                                                                               status);
-    BNPK_LAUNCHED("table_rehash_kernel");
-    return 0;
+    return launch("table_rehash_kernel", table_rehash_kernel, grid_cap((capacity + 255) / 256, 8), 256, 0,
+                  (cudaStream_t)stream, false, keys, counts, capacity, t, status);
 }
 
 int bnpk_rows_reverse_complement(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
@@ -948,11 +941,8 @@ int bnpk_rows_reverse_complement(const uint8_t *base, size_t base_bytes, const i
     (void)base_bytes;
     if (!lut256) return set_err(BNPK_E_BADARG, "lut256 required");
     if (n_rows == 0) return 0;
-    rows_reverse_complement_kernel<<<grid_cap((n_rows + 7) / 8, 8), 256, 0, (cudaStream_t)stream>>>(base, starts, lens,
-                                                                                                     n_rows, lut256,
-                                                                                                     offsets, out);
-    BNPK_LAUNCHED("rows_reverse_complement_kernel");
-    return 0;
+    return launch("rows_reverse_complement_kernel", rows_reverse_complement_kernel, grid_cap((n_rows + 7) / 8, 8), 256,
+                  0, (cudaStream_t)stream, false, base, starts, lens, n_rows, lut256, offsets, out);
 }
 
 int bnpk_rows_pwm_scores(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,

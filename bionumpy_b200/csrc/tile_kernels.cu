@@ -526,8 +526,9 @@ int chunk_kmer_count_impl(const uint8_t *chunk, size_t n, size_t slice_begin, si
     // and its halo): earlier calls count no tile, so no kernel reads the decision before it is taken.  Slices are
     // consecutive, so this is the only call with tile_begin == 0 that counts anything.
     if (a.tile_begin == 0 && a.tile_end > 0) {
-        cr_detect_kernel<<<1, 32, 0, st>>>(chunk, final_slice ? n : slice_end, lpe, trim_cr, status);
-        BNPK_LAUNCHED("cr_detect_kernel");
+        if (int rc = launch("cr_detect_kernel", cr_detect_kernel, 1, 32, 0, st, false, chunk,
+                            final_slice ? n : slice_end, lpe, trim_cr, status))
+            return rc;
     }
     BNPK_CUDA(cudaMemsetAsync(a.ws + kWsTicket, 0, sizeof(uint64_t), st));
     const bool smem_hist = use_smem_hist(n_bins, hist_mode);
@@ -540,12 +541,13 @@ int chunk_kmer_count_impl(const uint8_t *chunk, size_t n, size_t slice_begin, si
     int rc = launch_count(a, enc_mode, smem_hist, st);
     if (rc) return rc;
     if (final_slice && scratch32) {
-        widen_add_kernel<<<sm_count() * 8, 256, 0, st>>>(a.hist32, a.hist, (size_t)n_bins);
-        BNPK_LAUNCHED("widen_add_kernel");
+        rc = launch("widen_add_kernel", widen_add_kernel, sm_count() * 8, 256, 0, st, false, a.hist32, a.hist,
+                    (size_t)n_bins);
+        if (rc) return rc;
     }
     if (final_slice) {
-        finalize_status_kernel<<<1, 32, 0, st>>>(status, lpe);
-        BNPK_LAUNCHED("finalize_status_kernel");
+        rc = launch("finalize_status_kernel", finalize_status_kernel, 1, 32, 0, st, false, status, lpe);
+        if (rc) return rc;
         rc = count_fixups_impl(chunk, n, lpe, enc_mode, lut256, k, window, n_bins, hist, status,
                                (uint64_t *)workspace + kWsDeferred, a.deferred, a.deferred_cap, st);
     }
@@ -568,13 +570,11 @@ int line_split_impl(const uint8_t *chunk, size_t n, int lpe, int field_line, int
     a.starts = starts; a.lens = lens; a.max_rows = max_rows; a.n_bins = 1;
     if (max_rows) BNPK_CUDA(cudaMemsetAsync(lens, 0, max_rows * sizeof(int32_t), st));
     BNPK_CUDA(cudaMemsetAsync(workspace, 0, ws_lookback_words((size_t)a.n_tiles_total) * sizeof(uint64_t), st));
-    cr_detect_kernel<<<1, 32, 0, st>>>(chunk, n, lpe, trim_cr, status);
-    BNPK_LAUNCHED("cr_detect_kernel");
-    int rc = launch_tile<0, BNPK_ENC_ASCII_ACGT, false, false>(a, st);
+    int rc = launch("cr_detect_kernel", cr_detect_kernel, 1, 32, 0, st, false, chunk, n, lpe, trim_cr, status);
     if (rc) return rc;
-    finalize_status_kernel<<<1, 32, 0, st>>>(status, lpe);
-    BNPK_LAUNCHED("finalize_status_kernel");
-    return 0;
+    rc = launch_tile<0, BNPK_ENC_ASCII_ACGT, false, false>(a, st);
+    if (rc) return rc;
+    return launch("finalize_status_kernel", finalize_status_kernel, 1, 32, 0, st, false, status, lpe);
 }
 
 }  // namespace bnpk

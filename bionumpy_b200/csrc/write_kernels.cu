@@ -7,7 +7,7 @@
 //   two-line FASTA '>' name '\n' seq '\n'                                        Ln + Ls + 3
 //   wrapped FASTA  '>' name '\n', then ceil(Ls / W) lines of W bases (the last one shorter), each ending in '\n'
 //                                                                                Ln + 2 + Ls + ceil(Ls / W)
-// format_offsets_kernel is the exclusive prefix sum of those sizes (decoupled look-back, as bnpk_row_offsets).
+// format_offsets_kernel is the exclusive prefix sum of those sizes (the single-pass scan of bnpk_device.cuh, as bnpk_row_offsets).
 // format_kernel is output-driven: a CTA owns a tile of output bytes, finds the entry of each 16-byte unit by a binary
 // search of the offsets and builds the unit in registers -- one unaligned 16-byte gather when the unit lies inside one
 // field segment, byte by byte otherwise -- and writes it with one vector store.  The same kernel in CHECK mode walks
@@ -21,10 +21,6 @@ namespace {
 constexpr int kFmtThreads = 256;
 constexpr int kFmtUnitsPerThread = 4;
 constexpr int64_t kFmtTile = (int64_t)kFmtThreads * kFmtUnitsPerThread * 16;   // 16 KiB of output per tile
-
-constexpr int kOffThreads = 256;
-constexpr int kOffItems = 8;
-constexpr int kOffTile = kOffThreads * kOffItems;
 
 struct FmtArgs {
     const uint8_t *base[3];
@@ -52,64 +48,11 @@ __device__ __forceinline__ int64_t entry_size(int fmt, int width, int64_t ln, in
 }
 
 // exclusive prefix sum of the entry sizes; offs[n] = total
-__global__ void __launch_bounds__(kOffThreads) format_offsets_kernel(const __grid_constant__ FmtArgs a, int64_t *offs,
-                                                                     uint64_t *ws) {
-    __shared__ uint64_t s_warp[kOffThreads / 32 + 1];
-    __shared__ int64_t s_tile;
-    __shared__ uint64_t s_base;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    uint64_t *state = ws + kWsHeaderWords;
-    const int64_t n = a.n;
-    const int64_t n_tiles = (n + kOffTile - 1) / kOffTile;
-    while (true) {
-        if (tid == 0) s_tile = (int64_t)atomicAdd((unsigned long long *)(ws + kWsTicket), 1ull);
-        __syncthreads();
-        const int64_t tile = s_tile;
-        if (tile >= n_tiles) break;
-        const int64_t r0 = tile * kOffTile + (int64_t)tid * kOffItems;
-        uint64_t v[kOffItems];
-        uint64_t sum = 0;
-#pragma unroll
-        for (int i = 0; i < kOffItems; ++i) {
-            v[i] = 0;
-            if (r0 + i < n)
-                v[i] = (uint64_t)entry_size(a.fmt, a.width, len_of(a.lens[0], r0 + i), len_of(a.lens[1], r0 + i),
-                                            len_of(a.lens[2], r0 + i));
-            sum += v[i];
-        }
-        uint64_t inc = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint64_t t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
-        }
-        if (lane == 31) s_warp[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-            const uint64_t w = lane < kOffThreads / 32 ? s_warp[lane] : 0;
-            uint64_t winc = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint64_t t = __shfl_up_sync(0xffffffffu, winc, o);
-                if (lane >= o) winc += t;
-            }
-            const uint64_t total = __shfl_sync(0xffffffffu, winc, kOffThreads / 32 - 1);
-            if (lane < kOffThreads / 32) s_warp[lane] = winc - w;
-            const uint64_t excl = lookback_exclusive(state, tile, total, lane);
-            if (lane == 0) {
-                s_base = excl;
-                if (tile == n_tiles - 1) offs[n] = (int64_t)(excl + total);
-            }
-        }
-        __syncthreads();
-        uint64_t run = s_base + s_warp[warp] + inc - sum;
-#pragma unroll
-        for (int i = 0; i < kOffItems; ++i) {
-            if (r0 + i < n) offs[r0 + i] = (int64_t)run;
-            run += v[i];
-        }
-        __syncthreads();
-    }
+__global__ void __launch_bounds__(kScanThreads) format_offsets_kernel(const __grid_constant__ FmtArgs a, int64_t *offs,
+                                                                      uint64_t *ws) {
+    exclusive_offsets(a.n, offs, ws, [&](int64_t e) -> uint64_t {
+        return (uint64_t)entry_size(a.fmt, a.width, len_of(a.lens[0], e), len_of(a.lens[1], e), len_of(a.lens[2], e));
+    });
 }
 
 // the entry that holds output byte p: offs[e] <= p < offs[e + 1], searched in [lo, hi]
@@ -335,21 +278,17 @@ int bnpk_format_offsets(int format, int line_width, size_t n_entries, const bnpk
         BNPK_CUDA(cudaMemsetAsync(out_offsets, 0, sizeof(int64_t), st));
         return 0;
     }
-    const size_t n_tiles = (n_entries + kOffTile - 1) / kOffTile;
-    const size_t need = (kWsHeaderWords + n_tiles) * sizeof(uint64_t);
-    if (workspace_bytes < need) return set_err(BNPK_E_WORKSPACE, "workspace too small");
-    BNPK_CUDA(cudaMemsetAsync(workspace, 0, need, st));
-    const unsigned grid = grid_cap(n_tiles, 4);
-    format_offsets_kernel<<<grid, kOffThreads, 0, st>>>(a, out_offsets, (uint64_t *)workspace);
-    BNPK_LAUNCHED("format_offsets_kernel");
+    size_t n_tiles;
+    if (int rc = scan_workspace(n_entries, 1, workspace, workspace_bytes, st, n_tiles)) return rc;
+    if (int rc = launch("format_offsets_kernel", format_offsets_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st, false,
+                        a, out_offsets, (uint64_t *)workspace))
+        return rc;
     if (!a.lut[1]) return 0;                 // raw text: every byte is written as it is
     if (!status) return set_err(BNPK_E_BADARG, "a sequence LUT needs a status block for the bad-base report");
     a.offs = out_offsets;
     a.status = status;
     // the total is on the device: a grid for the average case, every CTA loops over tiles up to offs[n]
-    format_kernel<true><<<(unsigned)sm_count() * 8, kFmtThreads, 0, st>>>(a);
-    BNPK_LAUNCHED("format_kernel<check>");
-    return 0;
+    return launch("format_kernel<check>", format_kernel<true>, (unsigned)sm_count() * 8, kFmtThreads, 0, st, false, a);
 }
 
 int bnpk_format_records(int format, int line_width, size_t n_entries, const bnpk_field *fields,
@@ -364,9 +303,8 @@ int bnpk_format_records(int format, int line_width, size_t n_entries, const bnpk
     a.out_begin = out_begin;
     a.out_end = out_end;
     a.out = out;
-    format_kernel<false><<<fmt_grid(out_end - out_begin), kFmtThreads, 0, (cudaStream_t)stream>>>(a);
-    BNPK_LAUNCHED("format_kernel");
-    return 0;
+    return launch("format_kernel", format_kernel<false>, fmt_grid(out_end - out_begin), kFmtThreads, 0,
+                  (cudaStream_t)stream, false, a);
 }
 
 }  // extern "C"
