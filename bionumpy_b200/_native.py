@@ -26,6 +26,8 @@ COL_SKIP, COL_TEXT, COL_INT, COL_INT_OR_DOT, COL_STRAND = 0, 1, 2, 3, 4
 BAD_TABS, BAD_COLUMNS, BAD_INT, BAD_STRAND = 1, 2, 3, 4
 PILEUP_COUNT, PILEUP_ANY = 0, 1
 RUNS_MAX, RUNS_MIN, RUNS_SUM, RUNS_ANY = 0, 1, 2, 3
+(OP_ADD, OP_SUB, OP_MUL, OP_AND, OP_OR, OP_XOR, OP_MIN, OP_MAX, OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT,
+ OP_GE) = range(14)
 INT64_MAX = (1 << 63) - 1
 SMEM_MAX_BINS = 32768
 
@@ -85,6 +87,8 @@ SIGNATURES = {
     "bnpk_runs_extract": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _vp, _vp]),
     "bnpk_interval_merge": (_i, [_vp, _vp, _vp, _sz, _i64, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "bnpk_rows_equal_prev": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp]),
+    "bnpk_runs_combine": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "bnpk_interval_intersect": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
 

@@ -15,7 +15,7 @@ import torch
 from .. import _native as nv
 from .. import config, ops
 from ..datatypes import replace
-from ..encoded_array import EncodedRaggedArray, as_encoded_array
+from ..encoded_array import BaseEncoding, EncodedArray, EncodedRaggedArray, as_encoded_array
 from ..ragged import LazyRaggedArray
 from ..rows import RowView
 
@@ -25,6 +25,11 @@ def _device():
     if dev.type != "cuda":
         raise nv.NativeLibraryError("pileups need a CUDA device: bionumpy_b200 has no CPU fallback")
     return dev
+
+
+def to_device(array, device):
+    """A host NumPy array on the device through pinned memory, without waiting for the copy."""
+    return torch.from_numpy(np.array(array, copy=True)).pin_memory().to(device, non_blocking=True)
 
 
 def _int64(values, device):
@@ -258,6 +263,116 @@ class GenomicRunLengthArray:
 
     __str__ = __repr__
 
+    def __array_ufunc__(self, ufunc, method, *inputs, **kwargs):
+        """The ufuncs of TRACK_UFUNCS between tracks of one size and integer or bool scalars run on the runs
+        (bnpk_runs_combine, one synchronisation); any other call gets the dense arrays."""
+        out = track_ufunc(ufunc, method, inputs, kwargs)
+        if out is not None:
+            return out
+        return getattr(ufunc, method)(*[np.asarray(x) if isinstance(x, GenomicRunLengthArray) else x
+                                        for x in inputs], **kwargs)
+
+
+def _binary(ufunc):
+    return (lambda self, other: ufunc(self, other)), (lambda self, other: ufunc(other, self))
+
+
+def _add_operators(cls):
+    """The Python operators of a track class as the ufuncs its __array_ufunc__ serves."""
+    for name, ufunc in (("and", np.bitwise_and), ("or", np.bitwise_or), ("xor", np.bitwise_xor), ("add", np.add),
+                        ("sub", np.subtract), ("mul", np.multiply)):
+        forward, reflected = _binary(ufunc)
+        setattr(cls, f"__{name}__", forward)
+        setattr(cls, f"__r{name}__", reflected)
+    for name, ufunc in (("eq", np.equal), ("ne", np.not_equal), ("lt", np.less), ("le", np.less_equal),
+                        ("gt", np.greater), ("ge", np.greater_equal)):
+        setattr(cls, f"__{name}__", _binary(ufunc)[0])
+    cls.__invert__ = lambda self: np.invert(self)
+    cls.__neg__ = lambda self: np.negative(self)
+    cls.__hash__ = None
+    return cls
+
+
+_add_operators(GenomicRunLengthArray)
+
+# ufunc -> the kernel's operator; the logical ones first map each value to (value != 0)
+TRACK_UFUNCS = {np.add: nv.OP_ADD, np.subtract: nv.OP_SUB, np.multiply: nv.OP_MUL, np.bitwise_and: nv.OP_AND,
+                np.bitwise_or: nv.OP_OR, np.bitwise_xor: nv.OP_XOR, np.minimum: nv.OP_MIN, np.maximum: nv.OP_MAX,
+                np.equal: nv.OP_EQ, np.not_equal: nv.OP_NE, np.less: nv.OP_LT, np.less_equal: nv.OP_LE,
+                np.greater: nv.OP_GT, np.greater_equal: nv.OP_GE, np.logical_and: nv.OP_AND,
+                np.logical_or: nv.OP_OR, np.logical_xor: nv.OP_XOR}
+_LOGICAL = (np.logical_and, np.logical_or, np.logical_xor)
+
+
+def _is_int_scalar(x):
+    return isinstance(x, (bool, int, np.bool_, np.integer))
+
+
+def _probe(x):
+    """What NumPy's type rules see of an operand: a one-element array of the track's computed dtype (bool, or int64 for
+    every integer track), or the scalar itself."""
+    if isinstance(x, GenomicRunLengthArray):
+        return np.zeros(1, dtype=np.bool_ if x.dtype == torch.bool else np.int64)
+    return x
+
+
+def track_ufunc(ufunc, method, inputs, kwargs):
+    """``ufunc(*inputs)`` on run-length tracks, or None when the call is not one the runs serve (another ufunc or
+    method, keyword arguments, a float or non-scalar operand).  Unary ufuncs are binary ones with a scalar: ~x is
+    x ^ -1 (x ^ True for bool), -x is 0 - x and logical_not(x) is x == 0.  The result dtype is NumPy's on the dense
+    arrays, except that integer tracks narrower than int64 are computed, and returned, as int64.  Tracks of different
+    sizes raise ValueError; what NumPy refuses (bool - bool, -bool) raises its TypeError."""
+    if method != "__call__" or kwargs:
+        return None
+    if len(inputs) == 1:
+        (x,) = inputs
+        if not isinstance(x, GenomicRunLengthArray):
+            return None
+        if ufunc is np.invert:
+            np.invert(_probe(x))
+            return track_ufunc(np.bitwise_xor, method, (x, True if x.dtype == torch.bool else -1), kwargs)
+        if ufunc is np.negative:
+            np.negative(_probe(x))
+            return track_ufunc(np.subtract, method, (0, x), kwargs)
+        if ufunc is np.logical_not:
+            return track_ufunc(np.equal, method, (x, False if x.dtype == torch.bool else 0), kwargs)
+        return None
+    if len(inputs) != 2 or ufunc not in TRACK_UFUNCS:
+        return None
+    if not all(isinstance(x, GenomicRunLengthArray) or _is_int_scalar(x) for x in inputs):
+        return None
+    tracks = [x for x in inputs if isinstance(x, GenomicRunLengthArray)]
+    size = len(tracks[0])
+    if any(len(t) != size for t in tracks):
+        raise ValueError(f"tracks of sizes {len(tracks[0])} and {len(tracks[1])} cannot be combined")
+    dtype = ufunc(*[_probe(x) for x in inputs]).dtype
+    if dtype.kind not in "biu":
+        return None
+    op = TRACK_UFUNCS[ufunc]
+    if dtype == np.bool_ and ufunc in (np.add, np.multiply):
+        op = nv.OP_OR if ufunc is np.add else nv.OP_AND          # NumPy's bool + and *
+    dev = tracks[0]._events.device
+    runs = []
+    for x in inputs:
+        if isinstance(x, GenomicRunLengthArray):
+            values = x._values64() if ufunc not in _LOGICAL or x.dtype == torch.bool else (x._values != 0).to(torch.int64)
+            runs.append((x._events, values))
+        else:
+            v = int(bool(x)) if ufunc in _LOGICAL else int(x)
+            runs.append((torch.arange(2, dtype=torch.int64, device=dev) * size,      # made on the device: no copy
+                         torch.full((1,), v, dtype=torch.int64, device=dev)))
+    (a_starts, a_values), (b_starts, b_values) = runs
+    if size == 0:          # a size-0 track has one empty run; the kernel needs both sides alike
+        a_starts, a_values = a_starts[:1], a_values[:0]
+        b_starts, b_values = b_starts[:1], b_values[:0]
+    starts, values, n_runs = ops.runs_combine(a_starts.contiguous(), a_values.contiguous(), b_starts.contiguous(),
+                                              b_values.contiguous(), op)
+    n = int(n_runs.item())
+    if size == 0:
+        starts, values, n = torch.zeros(2, dtype=torch.int64, device=dev), torch.zeros(1, dtype=torch.int64, device=dev), 1
+    values = values[:n] != 0 if dtype == np.bool_ else values[:n]
+    return GenomicRunLengthArray(starts[:n + 1], values, size)
+
 
 class RunsRaggedArray(LazyRaggedArray):
     """``track[intervals]``: one row per interval, the track's values over [start, stop) clipped to [0, len(track)),
@@ -311,3 +426,175 @@ class RunsRaggedArray(LazyRaggedArray):
     @property
     def dtype(self):
         return self._track.dtype
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# interval sets (arithmetics/intervals.py:235-342)
+# --------------------------------------------------------------------------------------------------------------------
+NAME_SLOTS, NAME_BYTES = 4096, 1 << 16      # the distinct-name runs read back in the one synchronisation
+
+
+def _text_column(intervals):
+    chrom = intervals.chromosome
+    if isinstance(chrom, (np.ndarray, tuple, list)):
+        chrom = as_encoded_array([str(c) for c in chrom])
+    if not isinstance(chrom, EncodedRaggedArray):
+        raise TypeError(f"chromosome names must be text, not {type(chrom).__name__}")
+    return chrom
+
+
+def _name_runs(rows, slots=NAME_SLOTS, nbytes=NAME_BYTES):
+    """The first ``slots`` rows that start a run of equal names, packed for the host: [count, bytes] as int64, each
+    slot's length as int64 and the slots' bytes end to end (``nbytes``), all uint8; no synchronisation."""
+    dev, n = rows.base.device, rows.lens.numel()
+    first = ops.rows_equal_prev(rows.base, rows.starts, rows.lens) == 0
+    pos = torch.cumsum(first, 0) - 1
+    slot = torch.where(first & (pos < slots), pos, torch.full_like(pos, slots))
+    row = torch.zeros(slots + 1, dtype=torch.int64, device=dev).scatter_(
+        0, slot, torch.arange(n, dtype=torch.int64, device=dev))[:slots]
+    count = first.sum().reshape(1)
+    total = torch.where(first, rows.lens.to(torch.int64), 0).sum().reshape(1)       # of every run, not only the slots'
+    lens = torch.where(torch.arange(slots, device=dev) < count, rows.lens[row].to(torch.int64), 0)
+    ends = torch.cumsum(lens, 0)
+    j = torch.arange(nbytes, dtype=torch.int64, device=dev)
+    r = torch.searchsorted(ends, j, right=True).clamp_(max=slots - 1)
+    src = (rows.starts[row[r]] + j - (ends[r] - lens[r])).clamp_(0, max(rows.base.numel() - 1, 0))
+    data = torch.where(j < ends[-1], rows.base[src], 0).to(torch.uint8)
+    return torch.cat([torch.cat([count, total, lens]).view(torch.uint8), data])
+
+
+def _unpack_names(packed, rows):
+    """The distinct names of _name_runs' packing; more runs or bytes than it holds are read again, exactly (one more
+    synchronisation)."""
+    count, total = np.frombuffer(packed[:16].tobytes(), dtype=np.int64).tolist()
+    slots = NAME_SLOTS
+    if count > NAME_SLOTS or total > NAME_BYTES:
+        slots = count
+        packed = _name_runs(rows, count, total).cpu().numpy()
+    lens = np.frombuffer(packed[16:16 + 8 * count].tobytes(), dtype=np.int64).tolist()
+    data = packed[16 + 8 * slots:].tobytes()
+    ends = np.cumsum(lens).tolist()
+    return {data[e - n:e].decode() for e, n in zip(ends, lens)}
+
+
+def chromosome_ranks(columns, key=None, sort_order=None):
+    """The rank of every row's chromosome name in each text column (int64 device tensors), in one synchronisation:
+    the rows that start a run of equal names (bnpk_rows_equal_prev) are the only names copied to the host, where the
+    distinct names are ranked by ``key(name)`` (equal keys share a rank), by their position in ``sort_order`` (a name
+    missing from it raises KeyError) or, by default, as bytes; a byte-sorted table of them maps every row to its rank on
+    the device (bnpk_name_lookup)."""
+    views = [RowView(c) for c in columns]
+    live = [v for v in views if v.lens.numel()]
+    if not live:
+        return [torch.zeros(0, dtype=torch.int64, device=v.base.device) for v in views]
+    packed = torch.cat([_name_runs(v) for v in live]).cpu().numpy()
+    size = packed.size // len(live)
+    names = set()
+    for i, v in enumerate(live):
+        names |= _unpack_names(packed[i * size:(i + 1) * size], v)
+    if sort_order is not None:
+        order = {name: i for i, name in enumerate(sort_order)}
+        missing = sorted(names - set(order))
+        if missing:
+            raise KeyError(missing[0])
+        rank = {n: order[n] for n in names}
+    else:
+        key = key or (lambda n: n.encode())
+        keys = {n: key(n) for n in names}
+        rank, r, prev = {}, -1, object()
+        for n in sorted(names, key=keys.__getitem__):
+            if r < 0 or keys[n] != prev:
+                r, prev = r + 1, keys[n]
+            rank[n] = r
+    table = sorted(names, key=str.encode)
+    raw = [n.encode() for n in table]
+    dev = views[0].base.device
+    text = to_device(np.frombuffer(b"".join(raw) or b"\0", dtype=np.uint8), dev)
+    offsets = to_device(np.cumsum([0] + [len(b) for b in raw]).astype(np.int64), dev)
+    of_table = to_device(np.array([rank[n] for n in table], dtype=np.int64), dev)
+    out = []
+    for v in views:
+        if v.lens.numel() == 0:
+            out.append(torch.zeros(0, dtype=torch.int64, device=dev))
+            continue
+        ids, _ = ops.name_lookup(v.base, v.starts, v.lens, text, offsets)
+        out.append(of_table[ids.to(torch.int64)])
+    return out
+
+
+def lexsort_order(*keys):
+    """np.lexsort(keys) (the last key is the primary one) as stable torch.sort passes on the device."""
+    order = torch.sort(keys[0], stable=True).indices
+    for k in keys[1:]:
+        order = order[torch.sort(k[order], stable=True).indices]
+    return order
+
+
+def sort_intervals(intervals, chromosome_key_function=lambda x: x, sort_order=None):
+    """Intervals ordered by (chromosome_key_function(chromosome), start, stop), stably (arithmetics/intervals.py:
+    235-256); with ``sort_order`` the chromosomes come in that order and a chromosome missing from it raises KeyError.
+    One synchronisation, for the distinct chromosome names."""
+    if len(intervals) == 0:
+        return intervals
+    dev = _device()
+    start, stop = _start_stop(intervals, dev)
+    (rank,) = chromosome_ranks([_text_column(intervals)], chromosome_key_function, sort_order)
+    return intervals[lexsort_order(stop, start, rank)]
+
+
+def _sweep(a, b, start, stop, same=None):
+    """Rows of concatenate(a, b) ordered by ``start`` (the device order over the concatenated rows) paired with
+    ``stop`` by bnpk_interval_intersect: the emitted rows with their stops replaced, one synchronisation."""
+    from ..datatypes import concatenate
+    rows, stops, n_out, _ = ops.interval_intersect(start[0], stop, same)
+    both, (k,) = concatenate(a, b, extra=[n_out])
+    return replace(both[start[1][rows[:k]]], stop=stops[:k])
+
+
+def intersect(intervals_a, intervals_b):
+    """The reference's sorted sweep (arithmetics/intervals.py:317-325), which ignores the chromosome: the rows of both
+    sets ordered by start (stably), every row whose start lies before the previous sorted stop, with that stop.  Both
+    sets must be records of one type.  One synchronisation."""
+    dev = _device()
+    sa, ea = _start_stop(intervals_a, dev)
+    sb, eb = _start_stop(intervals_b, dev)
+    start, stop = torch.cat([sa, sb]), torch.cat([ea, eb])
+    order = torch.sort(start, stable=True).indices
+    return _sweep(intervals_a, intervals_b, (start[order], order), torch.sort(stop).values)
+
+
+def global_intersect(intervals_b, intervals_a):
+    """intersect on every chromosome (arithmetics/intervals.py:328-335, argument order kept: the rows of intervals_a
+    come first): rows ordered by (chromosome name as bytes, start), stably, stops by (name, stop).  Unlike the
+    reference, the last stop of one chromosome is never compared with the first start of the next, so a = chr1:100-200
+    and b = chr2:10-20 intersect to nothing (the reference gives chr2:10-200).  Two synchronisations."""
+    dev = _device()
+    sa, ea = _start_stop(intervals_a, dev)
+    sb, eb = _start_stop(intervals_b, dev)
+    ra, rb = chromosome_ranks([_text_column(intervals_a), _text_column(intervals_b)])
+    start, stop, rank = torch.cat([sa, sb]), torch.cat([ea, eb]), torch.cat([ra, rb])
+    order = lexsort_order(start, rank)
+    stops = stop[lexsort_order(stop, rank)]
+    r = rank[order]
+    same = torch.cat([torch.zeros(1, dtype=torch.bool, device=dev), r[1:] == r[:-1]]).to(torch.uint8)
+    return _sweep(intervals_a, intervals_b, (start[order], order), stops, same)
+
+
+def count_overlap(intervals_a, intervals_b) -> int:
+    """The sum over the sorted sweep of both sets of max(previous stop - start, 0) (arithmetics/intervals.py:307-314),
+    on one contig: one kernel launch that writes no rows, one synchronisation."""
+    dev = _device()
+    sa, ea = _start_stop(intervals_a, dev)
+    sb, eb = _start_stop(intervals_b, dev)
+    start = torch.sort(torch.cat([sa, sb])).values
+    stop = torch.sort(torch.cat([ea, eb])).values
+    _, _, _, overlap = ops.interval_intersect(start, stop, rows=False)
+    return int(overlap.item())
+
+
+def unique_intersect(intervals_a, intervals_b, genome_size):
+    """The rows of intervals_a that overlap any interval of intervals_b (arithmetics/intervals.py:338-342): the mask of
+    b, then the fused any() of a's rows over it.  Two synchronisations."""
+    mask = get_boolean_mask(intervals_b, genome_size)
+    rows = torch.nonzero(mask[intervals_a].any(axis=-1)).reshape(-1)      # one read, then every field by index
+    return intervals_a[rows]

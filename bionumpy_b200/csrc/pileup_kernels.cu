@@ -16,6 +16,11 @@
 // interval_merge_kernel: a segmented inclusive max-scan of stop (look-back 1 with an ordered segmented-max operator)
 //   and the compaction of the first row of every group (look-back 2).
 // rows_equal_prev_kernel: one thread per row, a full byte compare with the previous row.
+// runs_combine_kernel: a merge path over the run starts of two tracks, 2048 merged starts per tile, each thread's first
+//   split between the tracks found by binary search on its diagonal; every start decides alone whether a run of
+//   op(a, b) begins there, and the runs are compacted in order (one look-back).
+// interval_intersect_kernel: row r > 0 of a segment pairs with row r - 1 when stop[r - 1] > start[r]; the pairs are
+//   compacted in order (one look-back) and their overlaps summed (one atomic per block and tile).
 #include "bnpk_host.h"
 
 namespace bnpk {
@@ -393,6 +398,159 @@ __global__ void __launch_bounds__(256) rows_equal_prev_kernel(const uint8_t *bas
     }
 }
 
+// --------------------------------------------------------------------------------------------------------------------
+// two tracks into one
+// --------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ int64_t apply_op(int op, int64_t a, int64_t b) {
+    const uint64_t x = (uint64_t)a, y = (uint64_t)b;
+    switch (op) {
+        case BNPK_OP_ADD: return (int64_t)(x + y);
+        case BNPK_OP_SUB: return (int64_t)(x - y);
+        case BNPK_OP_MUL: return (int64_t)(x * y);
+        case BNPK_OP_AND: return a & b;
+        case BNPK_OP_OR: return a | b;
+        case BNPK_OP_XOR: return a ^ b;
+        case BNPK_OP_MIN: return min(a, b);
+        case BNPK_OP_MAX: return max(a, b);
+        case BNPK_OP_EQ: return a == b;
+        case BNPK_OP_NE: return a != b;
+        case BNPK_OP_LT: return a < b;
+        case BNPK_OP_LE: return a <= b;
+        case BNPK_OP_GT: return a > b;
+        default: return a >= b;
+    }
+}
+
+struct CombineArgs {
+    const int64_t *a_starts, *a_values;     // a_starts[n_a] = b_starts[n_b] = the size
+    const int64_t *b_starts, *b_values;
+    int64_t n_a, n_b;
+    int op;
+    int64_t *out_starts, *out_values, *n_out;
+    uint64_t *ws;
+};
+
+__global__ void __launch_bounds__(kScanThreads) runs_combine_kernel(const __grid_constant__ CombineArgs a) {
+    __shared__ ScanSmem sm;
+    const int64_t n = a.n_a + a.n_b;
+    const int64_t n_tiles = (n + kScanTile - 1) / kScanTile;
+    const int64_t *as = a.a_starts, *bs = a.b_starts;
+    for (int64_t tile; (tile = next_tile(a.ws, n_tiles, sm)) >= 0;) {
+        const int64_t i0 = tile * kScanTile + (int64_t)threadIdx.x * kScanItems;
+        // the merged starts before i0: ia of A's and i0 - ia of B's, an A start before a B start at the same position
+        const int64_t d = min(i0, n);
+        int64_t lo = max(d - a.n_b, (int64_t)0), hi = min(d, a.n_a);
+        while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (as[mid] <= bs[d - 1 - mid]) lo = mid + 1;
+            else hi = mid;
+        }
+        int64_t ia = lo, ib = d - lo;
+        int64_t pos[kScanItems], val[kScanItems];
+        uint32_t emit = 0;
+#pragma unroll
+        for (int j = 0; j < kScanItems; ++j) {
+            if (i0 + j >= n) break;
+            // the sizes at as[n_a] and bs[n_b] sort after every start, so neither track is read past its end
+            int64_t p, ja, jb;
+            bool last;
+            if (as[ia] <= bs[ib]) {
+                p = as[ia++];
+                last = bs[ib] != p;                   // a B start at p comes next and closes the group
+                ja = ia - 1;
+                jb = ib;
+            } else {
+                p = bs[ib++];
+                last = true;
+                ja = ia - (ia > 0 && as[ia - 1] == p);
+                jb = ib - 1;
+            }
+            if (!last) continue;
+            // the value from p on, and the value at the previous start position (every track has a start at 0)
+            const int64_t v = apply_op(a.op, a.a_values[ia - 1], a.b_values[ib - 1]);
+            if (p == 0 || v != apply_op(a.op, a.a_values[ja - 1], a.b_values[jb - 1])) {
+                emit |= 1u << j;
+                pos[j] = p;
+                val[j] = v;
+            }
+        }
+        uint64_t o = block_exclusive<Sum>((uint64_t)__popc(emit), tile, a.ws + kWsHeaderWords, sm);
+#pragma unroll
+        for (int j = 0; j < kScanItems; ++j) {
+            if (emit >> j & 1) {
+                a.out_starts[o] = pos[j];
+                a.out_values[o] = val[j];
+                ++o;
+            }
+        }
+        if (tile == n_tiles - 1 && threadIdx.x == kScanThreads - 1) {
+            a.n_out[0] = (int64_t)o;
+            a.out_starts[o] = as[a.n_a];
+        }
+    }
+}
+
+// --------------------------------------------------------------------------------------------------------------------
+// intersect
+// --------------------------------------------------------------------------------------------------------------------
+struct IntersectArgs {
+    const int64_t *start, *stop;
+    const uint8_t *same_prev;
+    int64_t n;
+    int64_t *out_rows, *out_stops, *n_out, *overlap;
+    uint64_t *ws;
+};
+
+__global__ void __launch_bounds__(kScanThreads) interval_intersect_kernel(const __grid_constant__ IntersectArgs a) {
+    __shared__ ScanSmem sm;
+    __shared__ uint64_t warp_overlap[kScanWarps];
+    const int64_t n_tiles = (a.n + kScanTile - 1) / kScanTile;
+    for (int64_t tile; (tile = next_tile(a.ws, n_tiles, sm)) >= 0;) {
+        const int64_t i0 = tile * kScanTile + (int64_t)threadIdx.x * kScanItems;
+        int64_t prev_stop = i0 > 0 && i0 <= a.n ? a.stop[i0 - 1] : 0;
+        int64_t stops[kScanItems];
+        uint32_t emit = 0;
+        uint64_t over = 0;
+#pragma unroll
+        for (int j = 0; j < kScanItems; ++j) {
+            const int64_t i = i0 + j;
+            if (i >= a.n) break;
+            const int64_t s = a.start[i];
+            // row i pairs with row i - 1 of its segment when that row's (sorted) stop is past its start
+            if (i > 0 && (!a.same_prev || a.same_prev[i]) && prev_stop > s) {
+                emit |= 1u << j;
+                stops[j] = prev_stop;
+                over += (uint64_t)(prev_stop - s);
+            }
+            prev_stop = a.stop[i];
+        }
+        if (a.overlap) {
+            over = warp_sum_u64(over);
+            if ((threadIdx.x & 31) == 0) warp_overlap[threadIdx.x >> 5] = over;
+        }
+        uint64_t g = block_exclusive<Sum>((uint64_t)__popc(emit), tile, a.ws + kWsHeaderWords, sm);
+        if (a.overlap && threadIdx.x == 0) {
+            uint64_t total = 0;
+#pragma unroll
+            for (int w = 0; w < kScanWarps; ++w) total += warp_overlap[w];
+            if (total) atomicAdd((unsigned long long *)a.overlap, (unsigned long long)total);
+        }
+        if (a.out_rows) {
+#pragma unroll
+            for (int j = 0; j < kScanItems; ++j) {
+                if (emit >> j & 1) {
+                    a.out_rows[g] = i0 + j;
+                    a.out_stops[g] = stops[j];
+                    ++g;
+                }
+            }
+        } else {
+            g += __popc(emit);
+        }
+        if (tile == n_tiles - 1 && threadIdx.x == kScanThreads - 1) a.n_out[0] = (int64_t)g;
+    }
+}
+
 }  // namespace
 }  // namespace bnpk
 
@@ -485,6 +643,50 @@ int bnpk_rows_equal_prev(const uint8_t *base, size_t base_bytes, const int64_t *
     if (!base || !starts || !lens || !flag) return set_err(BNPK_E_BADARG, "base, starts, lens and flag are required");
     return launch("rows_equal_prev_kernel", rows_equal_prev_kernel, grid_cap((n_rows + 255) / 256, 8), 256, 0,
                   (cudaStream_t)stream, false, base, starts, lens, (int64_t)n_rows, flag);
+}
+
+int bnpk_runs_combine(const int64_t *a_starts, const int64_t *a_values, size_t n_a, const int64_t *b_starts,
+                      const int64_t *b_values, size_t n_b, int op, int64_t *out_starts, int64_t *out_values,
+                      int64_t *n_out, void *workspace, size_t workspace_bytes, void *stream) {
+    if (op < BNPK_OP_ADD || op > BNPK_OP_GE) return set_err(BNPK_E_BADARG, "unknown track operator");
+    if (!a_starts || !b_starts || !out_starts || !n_out || !workspace)
+        return set_err(BNPK_E_BADARG, "a_starts, b_starts, out_starts, n_out and workspace are required");
+    if ((n_a == 0) != (n_b == 0)) return set_err(BNPK_E_BADARG, "a track without runs is empty: both must be");
+    if (n_a && (!a_values || !b_values || !out_values))
+        return set_err(BNPK_E_BADARG, "a_values, b_values and out_values are required");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_a == 0) {
+        // two tracks of size 0 without runs: no run, and the end of the last run is 0
+        BNPK_CUDA(cudaMemsetAsync(n_out, 0, sizeof(int64_t), st));
+        BNPK_CUDA(cudaMemsetAsync(out_starts, 0, sizeof(int64_t), st));
+        return 0;
+    }
+    size_t n_tiles;
+    if (int rc = scan_workspace(n_a + n_b, 1, workspace, workspace_bytes, st, n_tiles)) return rc;
+    CombineArgs a{a_starts, a_values, b_starts, b_values, (int64_t)n_a, (int64_t)n_b, op,
+                  out_starts, out_values, n_out, (uint64_t *)workspace};
+    return launch("runs_combine_kernel", runs_combine_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st, false, a);
+}
+
+int bnpk_interval_intersect(const int64_t *start, const int64_t *stop, const uint8_t *same_prev, size_t n,
+                            int64_t *out_rows, int64_t *out_stops, int64_t *n_out, int64_t *overlap, void *workspace,
+                            size_t workspace_bytes, void *stream) {
+    if (!n_out) return set_err(BNPK_E_BADARG, "n_out is required");
+    if (out_rows && !out_stops) return set_err(BNPK_E_BADARG, "out_rows needs out_stops");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n && (!start || !stop || !workspace)) return set_err(BNPK_E_BADARG, "start, stop and workspace are required");
+    size_t n_tiles = 0;
+    if (n) {
+        if (int rc = scan_workspace(n, 1, workspace, workspace_bytes, st, n_tiles)) return rc;
+    }
+    if (overlap) BNPK_CUDA(cudaMemsetAsync(overlap, 0, sizeof(int64_t), st));
+    if (n == 0) {
+        BNPK_CUDA(cudaMemsetAsync(n_out, 0, sizeof(int64_t), st));
+        return 0;
+    }
+    IntersectArgs a{start, stop, same_prev, (int64_t)n, out_rows, out_stops, n_out, overlap, (uint64_t *)workspace};
+    return launch("interval_intersect_kernel", interval_intersect_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st,
+                  false, a);
 }
 
 }  // extern "C"

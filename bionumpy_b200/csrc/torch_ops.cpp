@@ -545,6 +545,58 @@ Tensor rows_equal_prev(const Tensor &base, const Tensor &starts, const Tensor &l
     return flag;
 }
 
+// op(A, B) of two tracks: (run_starts int64[Ra + Rb + 1], run_values int64[max(Ra + Rb, 1)], n_runs int64[1])
+std::tuple<Tensor, Tensor, Tensor> runs_combine(const Tensor &a_starts, const Tensor &a_values, const Tensor &b_starts,
+                                                const Tensor &b_values, int64_t op) {
+    need(a_starts, torch::kInt64, "a_starts");
+    need(a_values, torch::kInt64, "a_values", a_starts);
+    need(b_starts, torch::kInt64, "b_starts", a_starts);
+    need(b_values, torch::kInt64, "b_values", a_starts);
+    TORCH_CHECK(a_starts.numel() == a_values.numel() + 1 && b_starts.numel() == b_values.numel() + 1,
+                "bnpk: a track is R values and R + 1 run starts");
+    c10::cuda::CUDAGuard guard(a_starts.device());
+    const int64_t n = a_values.numel() + b_values.numel();
+    Tensor starts = torch::empty({n + 1}, a_starts.options());
+    Tensor values = torch::empty({std::max<int64_t>(n, 1)}, a_starts.options());
+    Tensor n_runs = torch::empty({1}, a_starts.options());
+    Tensor ws = new_workspace(a_starts, (size_t)std::max<int64_t>(n, 1));
+    check(bnpk_runs_combine(a_starts.data_ptr<int64_t>(), a_values.data_ptr<int64_t>(), (size_t)a_values.numel(),
+                            b_starts.data_ptr<int64_t>(), b_values.data_ptr<int64_t>(), (size_t)b_values.numel(),
+                            (int)op, starts.data_ptr<int64_t>(), values.data_ptr<int64_t>(), n_runs.data_ptr<int64_t>(),
+                            ws.data_ptr<uint8_t>(), (size_t)ws.numel(), cur_stream(a_starts)),
+          "runs_combine");
+    return {starts, values, n_runs};
+}
+
+// intersect: (out_rows int64[R], out_stops int64[R], n_out int64[1], overlap int64[1]); rows=False leaves the first
+// two empty and counts only
+std::tuple<Tensor, Tensor, Tensor, Tensor> interval_intersect(const Tensor &start, const Tensor &stop,
+                                                              const c10::optional<Tensor> &same_prev, bool rows) {
+    need(start, torch::kInt64, "start");
+    need(stop, torch::kInt64, "stop", start);
+    TORCH_CHECK(start.numel() == stop.numel(), "bnpk: start and stop differ in length");
+    const uint8_t *sp = nullptr;
+    if (same_prev) {
+        need(*same_prev, torch::kUInt8, "same_prev", start);
+        TORCH_CHECK(same_prev->numel() == start.numel(), "bnpk: one same_prev flag per row");
+        sp = u8(*same_prev);
+    }
+    c10::cuda::CUDAGuard guard(start.device());
+    const int64_t n = start.numel();
+    Tensor out_rows = torch::empty({rows ? n : 0}, start.options());
+    Tensor out_stops = torch::empty({rows ? n : 0}, start.options());
+    Tensor n_out = torch::empty({1}, start.options());
+    Tensor overlap = torch::empty({1}, start.options());
+    Tensor ws = new_workspace(start, (size_t)std::max<int64_t>(n, 1));
+    check(bnpk_interval_intersect(start.data_ptr<int64_t>(), stop.data_ptr<int64_t>(), sp, (size_t)n,
+                                  rows ? out_rows.data_ptr<int64_t>() : nullptr,
+                                  rows ? out_stops.data_ptr<int64_t>() : nullptr, n_out.data_ptr<int64_t>(),
+                                  overlap.data_ptr<int64_t>(), ws.data_ptr<uint8_t>(), (size_t)ws.numel(),
+                                  cur_stream(start)),
+          "interval_intersect");
+    return {out_rows, out_stops, n_out, overlap};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bnpk, m) {
@@ -583,6 +635,10 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("runs_extract(Tensor run_starts, Tensor values, Tensor q_start, Tensor offsets, int total) -> Tensor");
     m.def("interval_merge(Tensor start, Tensor stop, Tensor? same_prev, int distance) -> (Tensor, Tensor, Tensor, Tensor)");
     m.def("rows_equal_prev(Tensor base, Tensor starts, Tensor lens) -> Tensor");
+    m.def("runs_combine(Tensor a_starts, Tensor a_values, Tensor b_starts, Tensor b_values, int op) "
+          "-> (Tensor, Tensor, Tensor)");
+    m.def("interval_intersect(Tensor start, Tensor stop, Tensor? same_prev, bool rows) "
+          "-> (Tensor, Tensor, Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
@@ -609,4 +665,6 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("runs_extract", &runs_extract);
     m.impl("interval_merge", &interval_merge);
     m.impl("rows_equal_prev", &rows_equal_prev);
+    m.impl("runs_combine", &runs_combine);
+    m.impl("interval_intersect", &interval_intersect);
 }

@@ -67,6 +67,41 @@ def replace(entries, **fields):
     return type(entries)(*[fields[f] if f in fields else getattr(entries, f) for f in entries._fields])
 
 
+def concatenate(a, b, extra=()):
+    """The entries of ``a`` followed by those of ``b`` (np.concatenate of two records of one type), and the host values
+    of ``extra`` (one-word device tensors, e.g. a kernel's output count), all read in one synchronisation.  Text
+    fields are copied row by row (the flat mode of bnpk_interval_gather), so only the bytes of the rows, not the whole
+    chunks they may be views of, are copied.  Returns (record, [extra values])."""
+    if type(a) is not type(b):
+        raise TypeError(f"cannot concatenate {type(a).__name__} and {type(b).__name__}")
+    from . import ops
+    from .encoded_array import EncodedArray, EncodedRaggedArray
+    from .rows import RowView
+    fields, texts, words = {}, {}, []
+    for f in a._fields:
+        x, y = getattr(a, f), getattr(b, f)
+        if isinstance(x, EncodedRaggedArray) and isinstance(y, EncodedRaggedArray):
+            if x.encoding != y.encoding:
+                raise TypeError(f"the {f} fields have different encodings")
+            texts[f] = [(RowView(v), ops.row_offsets(v._lens.contiguous())) for v in (x, y)]
+            words += [offsets[-1:] for _, offsets in texts[f]]
+        elif isinstance(x, EncodedArray) and isinstance(y, EncodedArray):
+            fields[f] = EncodedArray(torch.cat([x.raw(), y.raw()]), x.encoding)
+        elif isinstance(x, torch.Tensor) and isinstance(y, torch.Tensor):
+            fields[f] = torch.cat([x, y])
+        else:
+            raise TypeError(f"cannot concatenate the {f} fields ({type(x).__name__}, {type(y).__name__})")
+    values = torch.cat([w.to(torch.int64).reshape(1) for w in words + list(extra)]).cpu().tolist() if words or extra \
+        else []
+    for i, (f, parts) in enumerate(texts.items()):
+        flat = [ops.interval_copy(rows.base, rows.starts, rows.starts + rows.lens.to(torch.int64), offsets, total)
+                for (rows, offsets), total in zip(parts, values[2 * i:2 * i + 2])]
+        x = getattr(a, f)
+        fields[f] = EncodedRaggedArray(EncodedArray(torch.cat(flat), x.encoding),
+                                       torch.cat([rows.lens for rows, _ in parts]))
+    return type(a)(*[fields[f] for f in a._fields]), values[len(words):]
+
+
 class SequenceEntry(_Entries):
     _fields = ("name", "sequence")
 

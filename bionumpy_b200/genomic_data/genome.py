@@ -12,7 +12,8 @@ import torch
 
 from .. import _native as nv
 from .. import ops
-from ..arithmetics.intervals import GenomicRunLengthArray, RunsRaggedArray, _device, _int64, coverage_runs
+from ..arithmetics.intervals import (GenomicRunLengthArray, RunsRaggedArray, _add_operators, _device, _int64,
+                                     coverage_runs, to_device, track_ufunc)
 from ..datatypes import replace
 from ..rows import RowView
 
@@ -28,13 +29,13 @@ def keep_all(name):
 
 class Genome:
     """Contig names and sizes in file order (genome.py:19-37).  Contigs the filter rejects are known but left out:
-    intervals on them are dropped."""
+    intervals on them are dropped.  ``filter_function=None`` keeps every contig (genome_context.py:92-93)."""
 
     def __init__(self, chrom_sizes, fasta_filename=None, sort_names=False, filter_function=keep_all):
         if sort_names:
             chrom_sizes = {key: chrom_sizes[key] for key in sorted(chrom_sizes)}
         self._all = {str(k): int(v) for k, v in chrom_sizes.items()}
-        self._sizes = {k: v for k, v in self._all.items() if filter_function(k)}
+        self._sizes = {k: v for k, v in self._all.items() if filter_function is None or filter_function(k)}
         ends = np.cumsum([0] + list(self._sizes.values())).astype(np.int64)
         self._offsets = dict(zip(self._sizes, ends[:-1].tolist()))
         self.size = int(ends[-1])
@@ -86,10 +87,10 @@ class Genome:
             names = sorted(self._all, key=lambda n: n.encode())
             raw = [n.encode() for n in names]
             ends = np.cumsum([0] + [len(b) for b in raw]).astype(np.int64)
-            text = torch.frombuffer(bytearray(b"".join(raw) or b"\0"), dtype=torch.uint8).to(dev)
-            offset = torch.tensor([self._offsets.get(n, -1) for n in names], dtype=torch.int64, device=dev)
-            size = torch.tensor([self._all[n] for n in names], dtype=torch.int64, device=dev)
-            self._table = (names, text, torch.from_numpy(ends).to(dev), offset, size)
+            text = to_device(np.frombuffer(b"".join(raw) or b"\0", dtype=np.uint8), dev)
+            offset = to_device(np.array([self._offsets.get(n, -1) for n in names], dtype=np.int64), dev)
+            size = to_device(np.array([self._all[n] for n in names], dtype=np.int64), dev)
+            self._table = (names, text, to_device(ends, dev), offset, size)
         return self._table
 
     def get_intervals(self, intervals, stranded=False) -> "GenomicIntervals":
@@ -193,6 +194,15 @@ class GenomicIntervals:
         """Where any interval covers the genome (bool)."""
         return self._runs(nv.PILEUP_ANY)
 
+    def sorted(self) -> "GenomicIntervals":
+        """The intervals in genome order, then by start, then by stop, stably (genomic_intervals.py:691-699); on the
+        device, no synchronisation."""
+        from ..arithmetics.intervals import lexsort_order
+        names = self._genome._name_table()[0]
+        order = {n: i for i, n in enumerate(self._genome._sizes)}
+        rank = to_device(np.array([order.get(n, -1) for n in names], dtype=np.int64), self._ids.device)
+        return self[lexsort_order(self._g_stop, self._g_start, rank[self._ids.to(torch.int64)])]
+
     def merged(self, distance=0) -> "GenomicIntervals":
         """merge_intervals on every contig, in genome order: the rows are sorted by global start on the device, a
         merge never crosses a contig, one synchronisation."""
@@ -216,6 +226,31 @@ class GenomicArray:
     def __init__(self, events, values, genome):
         self._global = GenomicRunLengthArray(events, values, genome.size)
         self._genome = genome
+
+    @classmethod
+    def _of(cls, track, genome):
+        out = cls.__new__(cls)
+        out._global, out._genome = track, genome
+        return out
+
+    @property
+    def dtype(self):
+        return self._global.dtype
+
+    def __array_ufunc__(self, ufunc, method, *inputs, **kwargs):
+        """Track operators and the ufuncs of arithmetics.intervals.TRACK_UFUNCS between tracks on genomes with the
+        same contigs and sizes (else ValueError) and integer or bool scalars, on the runs (one synchronisation); any
+        other call gets the dense arrays of the whole genome."""
+        genomes = [x._genome for x in inputs if isinstance(x, GenomicArray)]
+        for g in genomes[1:]:
+            if list(g._sizes.items()) != list(genomes[0]._sizes.items()):
+                raise ValueError("the tracks are on genomes with different contigs or sizes")
+        args = [x._global if isinstance(x, GenomicArray) else x for x in inputs]
+        out = track_ufunc(ufunc, method, args, kwargs)
+        if out is None:
+            return getattr(ufunc, method)(*[np.asarray(x) if isinstance(x, GenomicRunLengthArray) else x
+                                            for x in args], **kwargs)
+        return GenomicArray._of(out, genomes[0])
 
     def __getitem__(self, idx):
         """``track["chr1"]``: one contig's runs.  ``track[intervals]`` (GenomicIntervals, or a record placed on the
@@ -258,5 +293,7 @@ class GenomicArray:
             lines.append("...")
         return "\n".join(lines)
 
+
+_add_operators(GenomicArray)
 
 __all__ = ["Genome", "GenomicIntervals", "GenomicArray", "ignore_underscores", "keep_all"]

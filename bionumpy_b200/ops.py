@@ -696,3 +696,41 @@ def rows_equal_prev(base, starts, lens):
     flag = torch.empty(lens.numel(), dtype=torch.uint8, device=base.device)
     check(lib().bnpk_rows_equal_prev(*args, ptr(flag), stream_ptr()))
     return flag
+
+
+@_on_device
+def runs_combine(a_starts, a_values, b_starts, b_values, op):
+    """bnpk_runs_combine: (run_starts int64[Ra + Rb + 1], run_values int64[Ra + Rb], n_runs int64[1]), the canonical
+    runs of op(A, B) (nv.OP_*) of two tracks of one size, the first n_runs + 1 starts and n_runs values valid (nothing
+    is read back)."""
+    _int64_args((a_starts, "a_starts"), (a_values, "a_values"), (b_starts, "b_starts"), (b_values, "b_values"))
+    if a_starts.numel() != a_values.numel() + 1 or b_starts.numel() != b_values.numel() + 1:
+        raise ValueError("a track is R values and R + 1 run starts")
+    n, dev = a_values.numel() + b_values.numel(), a_starts.device
+    starts = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    values = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+    n_runs = torch.empty(1, dtype=torch.int64, device=dev)
+    ws = nv.workspace(max(n, 1), dev)
+    check(lib().bnpk_runs_combine(ptr(a_starts), ptr(a_values), a_values.numel(), ptr(b_starts), ptr(b_values),
+                                  b_values.numel(), op, ptr(starts), ptr(values), ptr(n_runs), ptr(ws), ws.numel(),
+                                  stream_ptr()))
+    return starts, values, n_runs
+
+
+@_on_device
+def interval_intersect(start, stop, same_prev=None, rows=True):
+    """bnpk_interval_intersect over rows sorted by start and, separately, their stops sorted (inside each segment of
+    ``same_prev``, uint8): (out_rows int64[R] or None, out_stops int64[R] or None, n_out int64[1], overlap int64[1]),
+    the first n_out rows valid.  ``rows=False`` counts the pairs and sums their overlaps only."""
+    _int64_args((start, "start"), (stop, "stop"))
+    n, dev = start.numel(), start.device
+    if stop.numel() != n or (same_prev is not None and (same_prev.numel() != n or same_prev.dtype != torch.uint8)):
+        raise ValueError("start, stop and same_prev (uint8) differ in length")
+    if same_prev is not None:
+        _need_cuda(same_prev, "same_prev")
+    out_rows, out_stops = (torch.empty(n, dtype=torch.int64, device=dev) for _ in range(2)) if rows else (None, None)
+    n_out, overlap = (torch.empty(1, dtype=torch.int64, device=dev) for _ in range(2))
+    ws = nv.workspace(max(n, 1), dev)
+    check(lib().bnpk_interval_intersect(ptr(start), ptr(stop), ptr(same_prev), n, ptr(out_rows), ptr(out_stops),
+                                        ptr(n_out), ptr(overlap), ptr(ws), ws.numel(), stream_ptr()))
+    return out_rows, out_stops, n_out, overlap

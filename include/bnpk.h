@@ -395,8 +395,22 @@ int bnpk_interval_gather(const uint8_t *file, size_t file_bytes, size_t n_rows, 
  *   same segment is atomicMin-ed into status[BNPK_ST_BAD_BASE].  workspace as for bnpk_row_offsets with n := n_rows.
  * bnpk_rows_equal_prev: flag[r] = 1 iff r > 0 and the bytes of row r equal those of row r - 1 (same length, every
  *   byte), else 0.
- * BNPK_E_BADARG before any device work for an unknown mode, a size or distance outside [0, 2^59), and a missing
- * pointer the call needs.
+ * bnpk_runs_combine: op(A, B) of two tracks of one size S (a_starts[n_a] == b_starts[n_b] == S, checked by the caller)
+ *   whose runs are non-empty but whose neighbouring runs may have equal values.  P is the union of both tracks' run
+ *   starts; the value on [p, the next point of P) is op(A(p), B(p)) in int64, and a run starts at p where p == 0 or
+ *   the value differs from the value at the previous point of P, so the output is canonical.  Writes *n_out = R
+ *   (<= n_a + n_b), out_starts[0 .. R] (capacity n_a + n_b + 1, out_starts[R] = S) and out_values[0 .. R).  BNPK_OP_ADD,
+ *   SUB and MUL wrap, AND / OR / XOR are bitwise, MIN / MAX as named, and EQ, NE, LT, LE, GT and GE give 0 or 1.  An
+ *   empty track may have no runs: n_a == n_b == 0 writes *n_out = 0 and out_starts[0] = 0; one of them 0 is
+ *   BNPK_E_BADARG.  workspace as for bnpk_row_offsets with n := n_a + n_b.
+ * bnpk_interval_intersect: the reference's sorted sweep (intersect / count_overlap, arithmetics/intervals.py:307-335).
+ *   start[0 .. n) is sorted inside each segment (segments as for bnpk_interval_merge; same_prev NULL: one segment) and
+ *   stop[0 .. n) is the same rows' stops sorted on their own inside each segment.  For every row r + 1 of r's segment
+ *   with stop[r] > start[r + 1], in order: out_rows[g] = r + 1, out_stops[g] = stop[r]; *n_out = the number of such
+ *   rows.  overlap (int64[1], may be NULL) = the sum of stop[r] - start[r + 1] over them (int64, wrapping).  out_rows
+ *   NULL writes only n_out and overlap.  workspace as for bnpk_row_offsets with n := n.
+ * BNPK_E_BADARG before any device work for an unknown mode or operator, a size or distance outside [0, 2^59), and a
+ * missing pointer the call needs.
  * ------------------------------------------------------------------------------------- */
 #define BNPK_PILEUP_COUNT 0
 #define BNPK_PILEUP_ANY   1
@@ -404,6 +418,20 @@ int bnpk_interval_gather(const uint8_t *file, size_t file_bytes, size_t n_rows, 
 #define BNPK_RUNS_MIN 1
 #define BNPK_RUNS_SUM 2
 #define BNPK_RUNS_ANY 3
+#define BNPK_OP_ADD 0
+#define BNPK_OP_SUB 1
+#define BNPK_OP_MUL 2
+#define BNPK_OP_AND 3
+#define BNPK_OP_OR  4
+#define BNPK_OP_XOR 5
+#define BNPK_OP_MIN 6
+#define BNPK_OP_MAX 7
+#define BNPK_OP_EQ  8
+#define BNPK_OP_NE  9
+#define BNPK_OP_LT  10
+#define BNPK_OP_LE  11
+#define BNPK_OP_GT  12
+#define BNPK_OP_GE  13
 
 int bnpk_interval_events(const int64_t *start, const int64_t *stop, const int32_t *ids, const int64_t *contig_offset,
                          const int64_t *contig_len, size_t n_contigs, int64_t size, size_t n_rows, int64_t *keys,
@@ -420,6 +448,12 @@ int bnpk_interval_merge(const int64_t *start, const int64_t *stop, const uint8_t
                         void *workspace, size_t workspace_bytes, void *stream);
 int bnpk_rows_equal_prev(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
                          size_t n_rows, uint8_t *flag, void *stream);
+int bnpk_runs_combine(const int64_t *a_starts, const int64_t *a_values, size_t n_a, const int64_t *b_starts,
+                      const int64_t *b_values, size_t n_b, int op, int64_t *out_starts, int64_t *out_values,
+                      int64_t *n_out, void *workspace, size_t workspace_bytes, void *stream);
+int bnpk_interval_intersect(const int64_t *start, const int64_t *stop, const uint8_t *same_prev, size_t n,
+                            int64_t *out_rows, int64_t *out_stops, int64_t *n_out, int64_t *overlap, void *workspace,
+                            size_t workspace_bytes, void *stream);
 
 /* Bloom filter over k-mer hashes (sequence/bloom_filter.py:15-42): hash function i is v ^ offsets[i]; the filter is
  * one byte per position (the reference's bool mask).  insert: mask[(v ^ offsets[i]) % mask_size] = 1 for every value and
