@@ -320,7 +320,8 @@ def track_ufunc(ufunc, method, inputs, kwargs):
     """``ufunc(*inputs)`` on run-length tracks, or None when the call is not one the runs serve (another ufunc or
     method, keyword arguments, a float or non-scalar operand).  Unary ufuncs are binary ones with a scalar: ~x is
     x ^ -1 (x ^ True for bool), -x is 0 - x and logical_not(x) is x == 0.  The result dtype is NumPy's on the dense
-    arrays, except that integer tracks narrower than int64 are computed, and returned, as int64.  Tracks of different
+    arrays, except that integer tracks narrower than int64 are computed, and returned, as int64; a result NumPy gives
+    as float or as an unsigned type wider than uint8 takes the dense path (None).  Tracks of different
     sizes raise ValueError; what NumPy refuses (bool - bool, -bool) raises its TypeError."""
     if method != "__call__" or kwargs:
         return None
@@ -346,12 +347,18 @@ def track_ufunc(ufunc, method, inputs, kwargs):
     if any(len(t) != size for t in tracks):
         raise ValueError(f"tracks of sizes {len(tracks[0])} and {len(tracks[1])} cannot be combined")
     dtype = ufunc(*[_probe(x) for x in inputs]).dtype
-    if dtype.kind not in "biu":
-        return None
+    if dtype.kind not in "biu" or (dtype.kind == "u" and dtype.itemsize > 1):
+        return None              # float, and uint16 / 32 / 64 (a bool track with such a scalar): the dense path
+    dev = tracks[0]._events.device
+    if ufunc not in _LOGICAL and any(_is_int_scalar(x) and not -2 ** 63 <= int(x) < 2 ** 63 for x in inputs):
+        if dtype != np.bool_:
+            return None
+        # a comparison with an integer that no int64 equals has one result at every position, NumPy's
+        value = torch.full((1,), bool(ufunc(*[_probe(x) for x in inputs])[0]), dtype=torch.bool, device=dev)
+        return GenomicRunLengthArray(torch.arange(2, dtype=torch.int64, device=dev) * size, value, size)
     op = TRACK_UFUNCS[ufunc]
     if dtype == np.bool_ and ufunc in (np.add, np.multiply):
         op = nv.OP_OR if ufunc is np.add else nv.OP_AND          # NumPy's bool + and *
-    dev = tracks[0]._events.device
     runs = []
     for x in inputs:
         if isinstance(x, GenomicRunLengthArray):
@@ -370,7 +377,14 @@ def track_ufunc(ufunc, method, inputs, kwargs):
     n = int(n_runs.item())
     if size == 0:
         starts, values, n = torch.zeros(2, dtype=torch.int64, device=dev), torch.zeros(1, dtype=torch.int64, device=dev), 1
-    values = values[:n] != 0 if dtype == np.bool_ else values[:n]
+    if dtype == np.bool_:
+        values = values[:n] != 0
+    elif dtype.itemsize < 8:
+        # only a bool track with a narrower NumPy integer scalar gets here (True + np.int8(127)): NumPy's dtype, and
+        # the int64 result wrapped into it as NumPy wraps; the two values of such a track stay distinct
+        values = values[:n].to(torch.from_numpy(np.zeros(0, dtype=dtype)).dtype)
+    else:
+        values = values[:n]
     return GenomicRunLengthArray(starts[:n + 1], values, size)
 
 

@@ -127,3 +127,88 @@ def dense_op(ufunc, *operands):
     with np.errstate(over="ignore"):
         out = ufunc(*[widen(x) for x in operands])
     return out, po.runs_of(out)
+
+
+ITEMS = {"a": 1, "b": 1, "ab": 2}
+
+
+def event_tracks(events, at, m, after=0, seed=0):
+    """Two tracks A and B laid out by events, the first merged run start of ``events[at]`` at merged index ``m``.
+
+    Merged order is the combine kernel's: run starts by position, an A start before a B start at one position.  Each
+    event is (side, a, b) at a position of its own: side "a", "b" or "ab" starts a run of A, of B or of both there, and
+    a and b are the values from there on (the value of a side that starts no run is ignored; a value equal to the one
+    before gives equal neighbouring runs, as astype does).  Position 0 holds both first runs (merged indices 0 and 1),
+    filler events of random sides and changing values take the merged indices up to the events, and filler events of
+    exactly ``after`` merged run starts follow them.  Gaps between positions are 1 to 3.  The placement is asserted
+    against a plain sort of the starts.  Returns ((a_starts, a_ends, a_values), (b_starts, b_ends, b_values), size),
+    int64, and the event's position."""
+    rng = np.random.default_rng(seed)
+    before = m - 2 - sum(ITEMS[e[0]] for e in events[:at])
+    assert before >= 0, (m, events[:at])
+    code = {"a": 1, "b": 2, "ab": 3}                 # bit 0: A starts a run, bit 1: B does
+
+    def filler(n_items):
+        """Random sides whose run starts number exactly n_items (a last tie that would overshoot becomes an A)."""
+        sides = rng.integers(1, 4, n_items + 1)
+        items = np.cumsum(np.where(sides == 3, 2, 1))
+        k = int(np.searchsorted(items, n_items))
+        sides = sides[:k + 1] if n_items else sides[:0]
+        if n_items and items[k] > n_items:
+            sides[k] = 1
+        return sides
+
+    head, tail = filler(before), filler(after)
+    sides = np.concatenate([[3], head, [code[e[0]] for e in events], tail]).astype(np.int64)
+    n, first = sides.size, 1 + head.size
+    pos = np.concatenate([[0], np.cumsum(rng.integers(1, 4, n - 1))]).astype(np.int64)
+    size = int(pos[-1]) + int(rng.integers(1, 4))
+    out = []
+    for k in range(2):
+        # filler values change by 1..3 modulo 7 at every start, so filler runs are canonical; the events' values
+        # are set as given and the fillers after them go on from the last one
+        step = np.where(sides >> k & 1 == 1, rng.integers(1, 4, n), 0)
+        vals = np.zeros(n, dtype=np.int64)
+        vals[:first] = (int(rng.integers(0, 7)) + np.cumsum(step[:first])) % 7
+        mine = sides[:first] >> k & 1 == 1
+        last = int(vals[:first][mine][-1])
+        for i, e in enumerate(events):
+            vals[first + i] = e[1 + k] if sides[first + i] >> k & 1 else last
+            last = int(vals[first + i])
+        vals[first + len(events):] = (last + np.cumsum(step[first + len(events):])) % 7
+        sel = sides >> k & 1 == 1
+        starts = pos[sel]
+        out.append((starts, np.append(starts[1:], size).astype(np.int64), vals[sel]))
+    mp = np.concatenate([out[0][0], out[1][0]])
+    side = np.concatenate([np.zeros(out[0][0].size, np.int64), np.ones(out[1][0].size, np.int64)])
+    order = np.lexsort((side, mp))
+    p = int(pos[first + at])
+    assert (mp[order[m]], side[order[m]]) == (p, 0 if "a" in events[at][0] else 1), (m, p)
+    assert mp.size == m + sum(ITEMS[e[0]] for e in events[at:]) + after
+    return out[0], out[1], size, p
+
+
+def sweep_loop(start, stop, same_prev=None):
+    """bnpk_interval_intersect as a loop over the rows as given: row i is emitted iff i > 0, same_prev[i] (when given)
+    and stop[i - 1] > start[i], with stop[i - 1] as its stop.  Returns (rows, stops, overlap): overlap is the sum of
+    stop[i - 1] - start[i] over the emitted rows in exact integers, wrapped to int64 as NumPy's int64 sum wraps."""
+    rows, stops, total = [], [], 0
+    for i in range(1, len(start)):
+        if (same_prev is None or same_prev[i]) and int(stop[i - 1]) > int(start[i]):
+            rows.append(i)
+            stops.append(int(stop[i - 1]))
+            total += int(stop[i - 1]) - int(start[i])
+    return np.array(rows, dtype=np.int64), np.array(stops, dtype=np.int64), (total + 2 ** 63) % 2 ** 64 - 2 ** 63
+
+
+def mask_intersect(a, b):
+    """The true intersection of two interval sets from dense masks, never the sweep: {name: (starts, stops)}, the
+    runs where both sets cover, on every chromosome of either set (each as long as its largest stop)."""
+    out = {}
+    for name in sorted(set(a[0]) | set(b[0])):
+        sel = [(np.asarray(x[0], dtype=object) == name) for x in (a, b)]
+        size = max([int(np.max(x[2][s])) for x, s in zip((a, b), sel) if s.any()] + [0])
+        both = po.dense_mask(a[1][sel[0]], a[2][sel[0]], size) & po.dense_mask(b[1][sel[1]], b[2][sel[1]], size)
+        s, e, v = po.runs_of(both)
+        out[name] = (s[v], e[v])
+    return out

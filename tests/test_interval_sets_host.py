@@ -155,3 +155,66 @@ def test_new_kernels_are_sm90a_code_without_stack_or_spills():
     for block in re.split(r"\n\s+Function : ", sass):
         if any(n in block.split("\n", 1)[0] for n in names):
             assert "STL" not in block and "LDL" not in block          # no local-memory spills
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# the helpers of tests/test_gpu_track_ops.py
+# --------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("m", [8, 16, 2040, 2047, 2048, 2049, 4096, 2048 * 40])
+@pytest.mark.parametrize("side", ["a", "b", "ab"])
+def test_event_tracks_placement(m, side):
+    """The placed event is the m-th run start of a plain merge of both tracks, A before B at one position, and both
+    tracks are well-formed runs of one size holding the event's values."""
+    a, b, size, p = so.event_tracks([("ab", 1, 2), (side, 5, 6)], 1, m, after=9, seed=m)
+    merged = sorted([(int(x), "A") for x in a[0]] + [(int(x), "B") for x in b[0]])
+    assert merged[m] == (p, "A" if "a" in side else "B")
+    if side == "ab":
+        assert merged[m + 1] == (p, "B")
+    assert len(merged) == m + len(side) + 9
+    for starts, ends, values in (a, b):
+        assert starts[0] == 0 and ends[-1] == size and np.all(starts[1:] == ends[:-1]) and np.all(ends > starts)
+    da, db = po.dense_of(*a), po.dense_of(*b)
+    assert (da[p], db[p]) == (5 if "a" in side else da[p - 1], 6 if "b" in side else db[p - 1])
+    assert (da[p - 1], db[p - 1]) == (1, 2)
+
+
+def test_event_tracks_exact_ends():
+    for total in (2049, 2056, 4097):
+        a, b, size, p = so.event_tracks([("a", 3, 0)], 0, total - 1, after=0, seed=total)
+        assert a[0].size + b[0].size == total and a[0][-1] == p
+
+
+def test_sweep_loop_matches_intersect():
+    rng = np.random.default_rng(1)
+    for n in (1, 2, 50, 700):
+        a = (["chr1"] * n, rng.integers(0, 3 * n, n), None)
+        a = (a[0], a[1], a[1] + rng.integers(0, 10, n))
+        b = (["chr1"] * (n // 2 + 1), rng.integers(0, 3 * n, n // 2 + 1), None)
+        b = (b[0], b[1], b[1] + rng.integers(0, 10, b[1].size))
+        s, e = np.concatenate([a[1], b[1]]), np.concatenate([a[2], b[2]])
+        order = np.argsort(s, kind="mergesort")
+        rows, stops, over = so.sweep_loop(s[order], np.sort(e))
+        want_rows, want_stops = so.intersect(a, b)
+        assert order[rows].tolist() == want_rows.tolist() and stops.tolist() == want_stops.tolist()
+        assert over == so.count_overlap(a, b)
+    same = np.array([0, 1, 0, 1], dtype=np.uint8)
+    rows, stops, over = so.sweep_loop(np.array([0, 1, 2, 3]), np.array([9, 9, 9, 9]), same)
+    assert rows.tolist() == [1, 3] and stops.tolist() == [9, 9] and over == 8 + 6
+    top = np.array([0, 1, 2], dtype=np.int64), np.array([2 ** 62, 2 ** 62 + 2 ** 61, 2 ** 62], dtype=np.int64)
+    assert so.sweep_loop(*top)[2] == (2 ** 62 - 1) + (2 ** 62 + 2 ** 61 - 2) - 2 ** 64       # past 2^63: wraps
+
+
+def test_mask_intersect_matches_intersect_on_merged_sets():
+    rng = np.random.default_rng(2)
+    for n in (1, 30, 400):
+        sets = []
+        for _ in range(2):
+            s = np.sort(rng.integers(0, 10 * n, n))
+            rows, stops = po.merge_intervals(s, s + rng.integers(1, 25, n))
+            sets.append((["chr1"] * rows.size, s[rows], stops))
+        a, b = sets
+        rows, stops = so.intersect(a, b)
+        starts = np.concatenate([a[1], b[1]])[rows]
+        ws, we = so.mask_intersect(a, b)["chr1"]
+        assert sorted(zip(starts.tolist(), stops.tolist())) == list(zip(ws.tolist(), we.tolist()))
+        assert int((we - ws).sum()) == so.count_overlap(a, b)
