@@ -28,6 +28,8 @@ PILEUP_COUNT, PILEUP_ANY = 0, 1
 RUNS_MAX, RUNS_MIN, RUNS_SUM, RUNS_ANY = 0, 1, 2, 3
 (OP_ADD, OP_SUB, OP_MUL, OP_AND, OP_OR, OP_XOR, OP_MIN, OP_MAX, OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT,
  OP_GE) = range(14)
+RUNS_TO_NONZERO, RUNS_TO_ALL = 0, 1
+MAX_OUT_COLUMNS = 8
 INT64_MAX = (1 << 63) - 1
 SMEM_MAX_BINS = 32768
 
@@ -89,6 +91,9 @@ SIGNATURES = {
     "bnpk_rows_equal_prev": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp]),
     "bnpk_runs_combine": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "bnpk_interval_intersect": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "bnpk_runs_to_intervals": (_i, [_vp, _vp, _sz, _vp, _sz, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "bnpk_delimited_offsets": (_i, [_vp, _i, _sz, _vp, _vp, _vp, _sz, _vp]),
+    "bnpk_delimited_format": (_i, [_vp, _i, _sz, _vp, _i64, _i64, _vp, _vp]),
 }
 
 
@@ -100,6 +105,11 @@ class Field(ctypes.Structure):
 class Column(ctypes.Structure):
     """bnpk_column: how one tab-separated column is written (COL_*), its output and, for text, its lengths."""
     _fields_ = [("kind", _i), ("out", _vp), ("lens", _vp)]
+
+
+class OutColumn(ctypes.Structure):
+    """bnpk_out_column: one written column (COL_TEXT, COL_INT or COL_STRAND), its data and, for text, its rows."""
+    _fields_ = [("kind", _i), ("data", _vp), ("base_bytes", _sz), ("starts", _vp), ("lens", _vp)]
 
 
 class NativeLibraryError(RuntimeError):

@@ -256,6 +256,27 @@ class GenomicRunLengthArray:
         events = (self._events[i0:i1 + 1] - a).clamp_(0, b - a)
         return GenomicRunLengthArray(events, self._values[i0:i1], b - a)
 
+    def to_bedgraph(self, sequence_name):
+        """The runs as BedGraph rows on contig ``sequence_name`` (arithmetics/intervals.py:119-121): every run as it
+        is stored, the value in the track's dtype (bool as 0 / 1 when written, where the reference writes True /
+        False).  The chromosome column is the name's bytes, viewed by every row; one synchronisation."""
+        from ..datatypes import BedGraph
+        dev = self._events.device
+        n = len(self)
+        if n == 0:
+            empty = torch.zeros(0, dtype=torch.int64, device=dev)
+            no_names = EncodedRaggedArray(EncodedArray(torch.zeros(0, dtype=torch.uint8, device=dev), BaseEncoding),
+                                          torch.zeros(0, dtype=torch.int32, device=dev))
+            return BedGraph(no_names, empty, empty, self._values[:0])
+        ends = torch.tensor([0, n], dtype=torch.int64, device=dev)
+        _, start, stop, value, n_out = ops.runs_to_intervals(self._events, self._values64(), ends, nv.RUNS_TO_ALL)
+        k = int(n_out.cpu()[0])
+        name = torch.frombuffer(bytearray(str(sequence_name).encode()), dtype=torch.uint8).to(dev)
+        chrom = EncodedRaggedArray(EncodedArray(name, BaseEncoding), torch.full((k,), name.numel(), dtype=torch.int32,
+                                                                                 device=dev),
+                                   starts=torch.zeros(k, dtype=torch.int64, device=dev))
+        return BedGraph(chrom, start[:k], stop[:k], self._cast(value[:k]))
+
     def __repr__(self):
         if len(self) <= 20:
             return _format(self.to_array().cpu().numpy())

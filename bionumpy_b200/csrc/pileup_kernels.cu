@@ -21,6 +21,8 @@
 //   op(a, b) begins there, and the runs are compacted in order (one look-back).
 // interval_intersect_kernel: row r > 0 of a segment pairs with row r - 1 when stop[r - 1] > start[r]; the pairs are
 //   compacted in order (one look-back) and their overlaps summed (one atomic per block and tile).
+// runs_to_intervals_kernel: 8 runs per thread; two binary searches of the contig ends (in shared memory when they fit)
+//   give each run's pieces, and the rows they open are compacted in order (one look-back).
 #include "bnpk_host.h"
 
 namespace bnpk {
@@ -551,6 +553,84 @@ __global__ void __launch_bounds__(kScanThreads) interval_intersect_kernel(const 
     }
 }
 
+// --------------------------------------------------------------------------------------------------------------------
+// runs -> interval rows
+// --------------------------------------------------------------------------------------------------------------------
+constexpr int kEndsSmem = 2048;     // contig ends staged in shared memory (16 KiB) when all C + 1 fit
+
+struct ToIntervalsArgs {
+    const int64_t *starts, *values;     // starts[n_runs] = the size = ends[n_contigs]
+    int64_t n_runs;
+    const int64_t *ends;                // int64[n_contigs + 1], strictly increasing from 0
+    int64_t n_contigs;
+    int all;
+    int32_t *out_contig;
+    int64_t *out_start, *out_stop, *out_value, *n_out;
+    uint64_t *ws;
+};
+
+// Run i = [s, e) lies in contigs c .. c + pieces - 1, and the contig borders inside it cut it into `pieces` pieces.  In
+// ALL mode every piece is a row.  In NONZERO mode a zero run has no piece, and a non-zero run's first piece continues
+// the row of the run before unless s is a border or that run is zero ("opens"), its last piece leaves its row open
+// for the next run unless e is a border or that run is zero ("closes").  So the rows are counted by the pieces that
+// open one, and the k-th row's start and stop are written by whichever pieces open and close it.
+struct RunPieces {
+    int64_t s, e, v, c;
+    int64_t pieces;             // 0: the run gives no row
+    bool open, close;
+};
+
+__device__ __forceinline__ RunPieces run_pieces(const ToIntervalsArgs &a, const int64_t *ends, int64_t i) {
+    RunPieces r{a.starts[i], a.starts[i + 1], a.values[i], 0, 0, false, false};
+    if (!a.all && r.v == 0) return r;
+    const int64_t nc = a.n_contigs;
+    r.c = upper_bound(ends, 0, nc + 1, r.s) - 1;                 // ends[c] <= s < ends[c + 1]
+    const int64_t c1 = lower_bound(ends, r.c + 1, nc + 1, r.e);   // ends[c1 - 1] < e <= ends[c1]
+    r.pieces = c1 - r.c;
+    r.open = a.all || i == 0 || ends[r.c] == r.s || a.values[i - 1] == 0;
+    r.close = a.all || i == a.n_runs - 1 || (c1 <= nc && ends[c1] == r.e) || a.values[i + 1] == 0;
+    return r;
+}
+
+__global__ void __launch_bounds__(kScanThreads) runs_to_intervals_kernel(const __grid_constant__ ToIntervalsArgs a) {
+    __shared__ ScanSmem sm;
+    __shared__ int64_t s_ends[kEndsSmem];
+    const int64_t n = a.n_runs, nc = a.n_contigs;
+    const bool staged = nc < kEndsSmem;
+    if (staged)
+        for (int64_t c = threadIdx.x; c <= nc; c += kScanThreads) s_ends[c] = a.ends[c];
+    // next_tile's barrier orders the staging before the first search
+    const int64_t *ends = staged ? s_ends : a.ends;
+    const int64_t n_tiles = (n + kScanTile - 1) / kScanTile;
+    for (int64_t tile; (tile = next_tile(a.ws, n_tiles, sm)) >= 0;) {
+        const int64_t i0 = tile * kScanTile + (int64_t)threadIdx.x * kScanItems;
+        const int64_t i1 = min(i0 + kScanItems, n);
+        uint64_t count = 0;
+        for (int64_t i = i0; i < i1; ++i) {
+            const RunPieces r = run_pieces(a, ends, i);
+            if (r.pieces) count += (uint64_t)r.pieces - 1 + r.open;
+        }
+        uint64_t o = block_exclusive<Sum>(count, tile, a.ws + kWsHeaderWords, sm);
+        // the same pieces again (the runs are in L1): keeping eight runs' pieces in registers would spill
+        for (int64_t i = i0; i < i1; ++i) {
+            const RunPieces r = run_pieces(a, ends, i);
+            if (!r.pieces) continue;
+            int64_t row = (int64_t)o - !r.open;
+            for (int64_t p = 0; p < r.pieces; ++p, ++row) {
+                const bool last = p + 1 == r.pieces;
+                if (p || r.open) {
+                    a.out_contig[row] = (int32_t)(r.c + p);
+                    a.out_start[row] = p ? ends[r.c + p] : r.s;
+                    if (a.all) a.out_value[row] = r.v;
+                }
+                if (!last || r.close) a.out_stop[row] = last ? r.e : ends[r.c + p + 1];
+            }
+            o += (uint64_t)r.pieces - 1 + r.open;
+        }
+        if (tile == n_tiles - 1 && threadIdx.x == kScanThreads - 1) a.n_out[0] = (int64_t)o;
+    }
+}
+
 }  // namespace
 }  // namespace bnpk
 
@@ -686,6 +766,29 @@ int bnpk_interval_intersect(const int64_t *start, const int64_t *stop, const uin
     }
     IntersectArgs a{start, stop, same_prev, (int64_t)n, out_rows, out_stops, n_out, overlap, (uint64_t *)workspace};
     return launch("interval_intersect_kernel", interval_intersect_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st,
+                  false, a);
+}
+
+int bnpk_runs_to_intervals(const int64_t *run_starts, const int64_t *values, size_t n_runs, const int64_t *contig_ends,
+                           size_t n_contigs, int mode, int32_t *out_contig, int64_t *out_start, int64_t *out_stop,
+                           int64_t *out_value, int64_t *n_out, void *workspace, size_t workspace_bytes, void *stream) {
+    if (mode != BNPK_RUNS_TO_NONZERO && mode != BNPK_RUNS_TO_ALL) return set_err(BNPK_E_BADARG, "unknown rows mode");
+    if (!n_out) return set_err(BNPK_E_BADARG, "n_out is required");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_runs == 0) {
+        BNPK_CUDA(cudaMemsetAsync(n_out, 0, sizeof(int64_t), st));
+        return 0;
+    }
+    if (n_contigs < 1 || n_contigs >= (size_t)INT32_MAX) return set_err(BNPK_E_BADARG, "n_contigs must be in [1, 2^31 - 1)");
+    if (!run_starts || !values || !contig_ends || !out_contig || !out_start || !out_stop || !workspace ||
+        (mode == BNPK_RUNS_TO_ALL && !out_value))
+        return set_err(BNPK_E_BADARG, "run_starts, values, contig_ends, the outputs and workspace are required");
+    size_t n_tiles;
+    if (int rc = scan_workspace(n_runs, 1, workspace, workspace_bytes, st, n_tiles)) return rc;
+    ToIntervalsArgs a{run_starts, values, (int64_t)n_runs, contig_ends, (int64_t)n_contigs,
+                      (int)(mode == BNPK_RUNS_TO_ALL), out_contig, out_start, out_stop, out_value, n_out,
+                      (uint64_t *)workspace};
+    return launch("runs_to_intervals_kernel", runs_to_intervals_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st,
                   false, a);
 }
 

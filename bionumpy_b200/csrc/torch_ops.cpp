@@ -597,6 +597,101 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> interval_intersect(const Tensor &star
     return {out_rows, out_stops, n_out, overlap};
 }
 
+// a track's rows: (contig int32[R + C], start, stop, value int64[R + C], n_out int64[1]), the first n_out valid
+std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor> runs_to_intervals(const Tensor &run_starts, const Tensor &values,
+                                                                     const Tensor &contig_ends, int64_t mode) {
+    need(run_starts, torch::kInt64, "run_starts");
+    need(values, torch::kInt64, "values", run_starts);
+    need(contig_ends, torch::kInt64, "contig_ends", run_starts);
+    TORCH_CHECK(run_starts.numel() == values.numel() + 1, "bnpk: a track is R values and R + 1 run starts");
+    TORCH_CHECK(contig_ends.numel() >= 2, "bnpk: contig_ends holds 0 and the end of every contig");
+    c10::cuda::CUDAGuard guard(run_starts.device());
+    const int64_t n = values.numel(), c = contig_ends.numel() - 1;
+    Tensor contig = torch::empty({n + c}, run_starts.options().dtype(torch::kInt32));
+    Tensor start = torch::empty({n + c}, run_starts.options());
+    Tensor stop = torch::empty({n + c}, run_starts.options());
+    Tensor value = torch::empty({n + c}, run_starts.options());
+    Tensor n_out = torch::empty({1}, run_starts.options());
+    Tensor ws = new_workspace(run_starts, (size_t)std::max<int64_t>(n, 1));
+    check(bnpk_runs_to_intervals(run_starts.data_ptr<int64_t>(), values.data_ptr<int64_t>(), (size_t)n,
+                                 contig_ends.data_ptr<int64_t>(), (size_t)c, (int)mode, contig.data_ptr<int32_t>(),
+                                 start.data_ptr<int64_t>(), stop.data_ptr<int64_t>(), value.data_ptr<int64_t>(),
+                                 n_out.data_ptr<int64_t>(), ws.data_ptr<uint8_t>(), (size_t)ws.numel(),
+                                 cur_stream(run_starts)),
+          "runs_to_intervals");
+    return {contig, start, stop, value, n_out};
+}
+
+// delimited columns: `kinds` names each column's kind; a TEXT column takes three tensors of `columns` (base uint8,
+// starts int64, lens int32), an INT column one int64 and a STRAND column one uint8 tensor, each with one row per line
+struct OutColumns {
+    bnpk_out_column col[BNPK_MAX_OUT_COLUMNS];
+    int n_cols;
+    size_t n_lines;
+};
+
+OutColumns need_out_columns(const std::vector<Tensor> &columns, const std::vector<int64_t> &kinds) {
+    TORCH_CHECK(!kinds.empty() && kinds.size() <= BNPK_MAX_OUT_COLUMNS, "bnpk: 1 to 8 columns");
+    OutColumns oc{};
+    oc.n_cols = (int)kinds.size();
+    size_t t = 0;
+    int64_t rows = -1;
+    for (size_t k = 0; k < kinds.size(); ++k) {
+        bnpk_out_column &c = oc.col[k];
+        c.kind = (int)kinds[k];
+        int64_t n = 0;
+        if (c.kind == BNPK_COL_TEXT) {
+            TORCH_CHECK(t + 3 <= columns.size(), "bnpk: a text column is three tensors");
+            const Rows r = need_rows(columns[t], columns[t + 1], columns[t + 2], c10::nullopt, columns[0]);
+            c.data = r.base;
+            c.base_bytes = r.base_bytes;
+            c.starts = r.starts;
+            c.lens = r.lens;
+            n = (int64_t)r.n_rows;
+            t += 3;
+        } else {
+            TORCH_CHECK(c.kind == BNPK_COL_INT || c.kind == BNPK_COL_STRAND, "bnpk: a column is TEXT, INT or STRAND");
+            TORCH_CHECK(t < columns.size(), "bnpk: a column misses its tensor");
+            need(columns[t], c.kind == BNPK_COL_INT ? torch::kInt64 : torch::kUInt8, "column", columns[0]);
+            c.data = columns[t].data_ptr();
+            n = columns[t].numel();
+            t += 1;
+        }
+        TORCH_CHECK(rows < 0 || n == rows, "bnpk: the columns differ in length");
+        rows = n;
+    }
+    TORCH_CHECK(t == columns.size(), "bnpk: more tensors than the kinds name");
+    oc.n_lines = (size_t)rows;
+    return oc;
+}
+
+std::tuple<Tensor, Tensor> delimited_offsets(const std::vector<Tensor> &columns, const std::vector<int64_t> &kinds) {
+    const OutColumns oc = need_out_columns(columns, kinds);
+    const Tensor &like = columns[0];
+    c10::cuda::CUDAGuard guard(like.device());
+    Tensor offsets = torch::empty({(int64_t)oc.n_lines + 1}, like.options().dtype(torch::kInt64));
+    Tensor status = new_status(like);
+    Tensor ws = new_workspace(like, std::max<size_t>(oc.n_lines, 1));
+    check(bnpk_delimited_offsets(oc.col, oc.n_cols, oc.n_lines, offsets.data_ptr<int64_t>(), status.data_ptr<int64_t>(),
+                                 ws.data_ptr<uint8_t>(), (size_t)ws.numel(), cur_stream(like)),
+          "delimited_offsets");
+    return {offsets, status};
+}
+
+Tensor delimited_format(const std::vector<Tensor> &columns, const std::vector<int64_t> &kinds, const Tensor &offsets,
+                        int64_t out_begin, int64_t out_end) {
+    const OutColumns oc = need_out_columns(columns, kinds);
+    const int64_t *offs = need_offsets(offsets, oc.n_lines, columns[0]);
+    TORCH_CHECK(0 <= out_begin && out_begin <= out_end, "bnpk: need 0 <= out_begin <= out_end");
+    c10::cuda::CUDAGuard guard(offsets.device());
+    Tensor out = torch::empty({out_end - out_begin}, offsets.options().dtype(torch::kUInt8));
+    if (out_end > out_begin)
+        check(bnpk_delimited_format(oc.col, oc.n_cols, oc.n_lines, offs, out_begin, out_end, out.data_ptr<uint8_t>(),
+                                    cur_stream(offsets)),
+              "delimited_format");
+    return out;
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bnpk, m) {
@@ -639,6 +734,10 @@ TORCH_LIBRARY(bnpk, m) {
           "-> (Tensor, Tensor, Tensor)");
     m.def("interval_intersect(Tensor start, Tensor stop, Tensor? same_prev, bool rows) "
           "-> (Tensor, Tensor, Tensor, Tensor)");
+    m.def("runs_to_intervals(Tensor run_starts, Tensor values, Tensor contig_ends, int mode) "
+          "-> (Tensor, Tensor, Tensor, Tensor, Tensor)");
+    m.def("delimited_offsets(Tensor[] columns, int[] kinds) -> (Tensor, Tensor)");
+    m.def("delimited_format(Tensor[] columns, int[] kinds, Tensor offsets, int out_begin, int out_end) -> Tensor");
 }
 
 TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
@@ -667,4 +766,7 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("rows_equal_prev", &rows_equal_prev);
     m.impl("runs_combine", &runs_combine);
     m.impl("interval_intersect", &interval_intersect);
+    m.impl("runs_to_intervals", &runs_to_intervals);
+    m.impl("delimited_offsets", &delimited_offsets);
+    m.impl("delimited_format", &delimited_format);
 }

@@ -12,6 +12,11 @@
 // search of the offsets and builds the unit in registers -- one unaligned 16-byte gather when the unit lies inside one
 // field segment, byte by byte otherwise -- and writes it with one vector store.  The same kernel in CHECK mode walks
 // the whole text without writing it and reports the first sequence byte whose LUT entry is 0.
+//
+// Delimited lines (BED, bedGraph; dump_csv io/dump_csv.py, join_columns io/strops.py:186-215): line e is its columns
+// joined by '\t' and ended by '\n'.  delimited_offsets_kernel is the exclusive prefix sum of the line sizes;
+// delimited_text_kernel is output-driven: a CTA owns a 16 KiB window of output, finds its lines by a binary search of
+// the offsets, builds them one line per thread in shared memory and stores the window with 16-byte stores.
 #include "bnpk_host.h"
 
 namespace bnpk {
@@ -262,6 +267,159 @@ unsigned fmt_grid(int64_t span_bytes) {
     return grid_cap((size_t)((span_bytes + kFmtTile - 1) / kFmtTile), 8);
 }
 
+// --------------------------------------------------------------------------------------------------------------------
+// delimited lines (K14)
+// --------------------------------------------------------------------------------------------------------------------
+constexpr int kDelimThreads = 256;
+constexpr int64_t kDelimWindow = 16384;         // output bytes a CTA builds in shared memory at a time
+
+struct DelimColumn {
+    int kind;
+    const uint8_t *data;
+    uint64_t base_bytes;
+    const int64_t *starts;
+    const int32_t *lens;
+};
+
+struct DelimArgs {
+    DelimColumn col[BNPK_MAX_OUT_COLUMNS];
+    int n_cols;
+    int64_t n;                      // lines
+    const int64_t *offs;            // int64[n + 1]
+    int64_t out_begin, out_end;
+    uint8_t *out;
+    int64_t *status;
+};
+
+// |v| and the number of characters of v in decimal ('-' included); INT64_MIN's magnitude is 2^63
+__device__ __forceinline__ int int_width(int64_t v, uint64_t &mag) {
+    mag = v < 0 ? 0ull - (uint64_t)v : (uint64_t)v;
+    int d = 1;
+    uint64_t p = 10;
+#pragma unroll
+    for (int k = 1; k < 20; ++k, p *= 10) d += mag >= p;
+    return d + (v < 0);
+}
+
+__device__ __forceinline__ int64_t field_width(const DelimColumn &c, int64_t e) {
+    if (c.kind == BNPK_COL_TEXT) return (int64_t)max(c.lens[e], 0);
+    if (c.kind == BNPK_COL_STRAND) return 1;
+    uint64_t mag;
+    return int_width(((const int64_t *)c.data)[e], mag);
+}
+
+// exclusive prefix sum of the line sizes (every column, a tab between two, '\n'); offs[n] = total
+__global__ void __launch_bounds__(kScanThreads) delimited_offsets_kernel(const __grid_constant__ DelimArgs a,
+                                                                         int64_t *offs, uint64_t *ws) {
+    exclusive_offsets(a.n, offs, ws, [&](int64_t e) -> uint64_t {
+        int64_t size = a.n_cols;
+        for (int k = 0; k < a.n_cols; ++k) {
+            const DelimColumn &c = a.col[k];
+            size += field_width(c, e);
+            if (c.kind == BNPK_COL_STRAND && c.data[e] > 2)
+                atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE], (long long)(e << 8 | k << 3 | BNPK_BAD_STRAND));
+        }
+        return (uint64_t)size;
+    });
+}
+
+// The digits of mag < 10^9 that end at window index `last` (inclusive), `n_digits` of them (leading zeros when the
+// part is not the top one); only the indices in [0, kDelimWindow) are written.
+__device__ __forceinline__ void put_digits(uint8_t *win, int64_t last, uint32_t part, int n_digits) {
+    for (int i = 0; i < n_digits; ++i) {
+        const int64_t q = last - i;
+        const uint32_t next = part / 10;
+        if (q >= 0 && q < kDelimWindow) win[q] = (uint8_t)('0' + (part - next * 10));
+        part = next;
+    }
+}
+
+// A CTA owns the output window [w0, w0 + kDelimWindow) (out-relative, aligned so that out + w0 is 16-byte aligned) and
+// builds, one line per thread, the bytes of every line that overlaps it into shared memory; a line that straddles two
+// windows is built by both CTAs, each keeping its own bytes.  The window is then stored with 16-byte stores.
+__global__ void __launch_bounds__(kDelimThreads) delimited_text_kernel(const __grid_constant__ DelimArgs a) {
+    __shared__ __align__(16) uint8_t win[kDelimWindow];
+    const int64_t begin = a.out_begin, span = a.out_end - a.out_begin;
+    const int mis = (int)(reinterpret_cast<uintptr_t>(a.out) & 15);
+    const int64_t n_windows = (span + mis + kDelimWindow - 1) / kDelimWindow;
+    for (int64_t w = blockIdx.x; w < n_windows; w += gridDim.x) {
+        const int64_t w0 = w * kDelimWindow - mis;                          // out-relative index of win[0]
+        const int64_t lo_j = max(w0, (int64_t)0), hi_j = min(w0 + kDelimWindow, span);
+        const int64_t lo = find_entry(a.offs, 0, a.n - 1, begin + lo_j);
+        const int64_t hi = find_entry(a.offs, lo, a.n - 1, begin + hi_j - 1);
+        for (int64_t e = lo + threadIdx.x; e <= hi; e += kDelimThreads) {
+            int64_t q = a.offs[e] - begin - w0;                             // window index of the line's next byte
+            for (int k = 0; k < a.n_cols; ++k) {
+                const DelimColumn &c = a.col[k];
+                if (k) {
+                    if (q >= 0 && q < kDelimWindow) win[q] = '\t';
+                    ++q;
+                }
+                if (c.kind == BNPK_COL_TEXT) {
+                    const int64_t len = max(c.lens[e], 0);
+                    const int64_t src = len ? c.starts[e] : 0;
+                    for (int64_t i = max(-q, (int64_t)0), i1 = min(len, kDelimWindow - q); i < i1; ++i) {
+                        const int64_t b = src + i;
+                        win[q + i] = b >= 0 && (uint64_t)b < c.base_bytes ? c.data[b] : 0;
+                    }
+                    q += len;
+                } else if (c.kind == BNPK_COL_STRAND) {
+                    const uint8_t code = c.data[e];
+                    if (q >= 0 && q < kDelimWindow) win[q] = code == 0 ? '+' : code == 1 ? '-' : '.';
+                    ++q;
+                } else {
+                    const int64_t v = ((const int64_t *)c.data)[e];
+                    uint64_t mag;
+                    const int width = int_width(v, mag);
+                    if (q + width > 0 && q < kDelimWindow) {
+                        if (v < 0 && q >= 0) win[q] = '-';
+                        // split once at 10^9 and 10^18, then every digit comes from 32-bit arithmetic
+                        const uint64_t top = mag / 1000000000ull;
+                        const uint32_t low = (uint32_t)(mag - top * 1000000000ull);
+                        const uint32_t mid = (uint32_t)(top % 1000000000ull), high = (uint32_t)(top / 1000000000ull);
+                        const int n_digits = width - (v < 0);
+                        const int64_t last = q + width - 1;
+                        put_digits(win, last, low, min(n_digits, 9));
+                        if (n_digits > 9) put_digits(win, last - 9, mid, min(n_digits - 9, 9));
+                        if (n_digits > 18) put_digits(win, last - 18, high, n_digits - 18);
+                    }
+                    q += width;
+                }
+            }
+            if (q >= 0 && q < kDelimWindow) win[q] = '\n';
+        }
+        __syncthreads();
+        for (int64_t u = threadIdx.x; u < kDelimWindow / 16; u += kDelimThreads) {
+            const int64_t j0 = w0 + 16 * u;
+            if (j0 + 16 <= lo_j || j0 >= hi_j) continue;
+            if (j0 >= lo_j && j0 + 16 <= hi_j) {
+                *reinterpret_cast<uint4 *>(a.out + j0) = *reinterpret_cast<const uint4 *>(win + 16 * u);
+            } else {
+                for (int i = 0; i < 16; ++i)
+                    if (j0 + i >= lo_j && j0 + i < hi_j) a.out[j0 + i] = win[16 * u + i];
+            }
+        }
+        __syncthreads();                                                    // the window is free again
+    }
+}
+
+int fill_delim(DelimArgs &a, const bnpk_out_column *columns, int n_columns, size_t n_lines) {
+    if (!columns || n_columns < 1 || n_columns > BNPK_MAX_OUT_COLUMNS)
+        return set_err(BNPK_E_BADARG, "1 to BNPK_MAX_OUT_COLUMNS columns are required");
+    memset(&a, 0, sizeof(a));
+    for (int k = 0; k < n_columns; ++k) {
+        const bnpk_out_column &c = columns[k];
+        if (c.kind != BNPK_COL_TEXT && c.kind != BNPK_COL_INT && c.kind != BNPK_COL_STRAND)
+            return set_err(BNPK_E_BADARG, "a written column is BNPK_COL_TEXT, BNPK_COL_INT or BNPK_COL_STRAND");
+        if (n_lines && (!c.data || (c.kind == BNPK_COL_TEXT && (!c.starts || !c.lens))))
+            return set_err(BNPK_E_BADARG, "a column misses its data, starts or lens");
+        a.col[k] = DelimColumn{c.kind, (const uint8_t *)c.data, (uint64_t)c.base_bytes, c.starts, c.lens};
+    }
+    a.n_cols = n_columns;
+    a.n = (int64_t)n_lines;
+    return 0;
+}
+
 }  // namespace
 }  // namespace bnpk
 
@@ -304,6 +462,41 @@ int bnpk_format_records(int format, int line_width, size_t n_entries, const bnpk
     a.out_end = out_end;
     a.out = out;
     return launch("format_kernel", format_kernel<false>, fmt_grid(out_end - out_begin), kFmtThreads, 0,
+                  (cudaStream_t)stream, false, a);
+}
+
+int bnpk_delimited_offsets(const bnpk_out_column *columns, int n_columns, size_t n_lines, int64_t *out_offsets,
+                           int64_t *status, void *workspace, size_t workspace_bytes, void *stream) {
+    DelimArgs a;
+    if (int rc = fill_delim(a, columns, n_columns, n_lines)) return rc;
+    if (!out_offsets) return set_err(BNPK_E_BADARG, "out_offsets is required");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_lines == 0) {
+        BNPK_CUDA(cudaMemsetAsync(out_offsets, 0, sizeof(int64_t), st));
+        return 0;
+    }
+    if (!status || !workspace) return set_err(BNPK_E_BADARG, "status and workspace are required");
+    a.status = status;
+    size_t n_tiles;
+    if (int rc = scan_workspace(n_lines, 1, workspace, workspace_bytes, st, n_tiles)) return rc;
+    return launch("delimited_offsets_kernel", delimited_offsets_kernel, grid_cap(n_tiles, 4), kScanThreads, 0, st,
+                  false, a, out_offsets, (uint64_t *)workspace);
+}
+
+int bnpk_delimited_format(const bnpk_out_column *columns, int n_columns, size_t n_lines, const int64_t *out_offsets,
+                          int64_t out_begin, int64_t out_end, uint8_t *out, void *stream) {
+    DelimArgs a;
+    if (int rc = fill_delim(a, columns, n_columns, n_lines)) return rc;
+    if (out_end < out_begin || out_begin < 0) return set_err(BNPK_E_BADARG, "need 0 <= out_begin <= out_end");
+    if (out_end == out_begin) return 0;
+    if (!out) return set_err(BNPK_E_BADARG, "out is NULL for a non-empty range");
+    if (n_lines == 0 || !out_offsets) return set_err(BNPK_E_BADARG, "a non-empty range needs lines and their offsets");
+    a.offs = out_offsets;
+    a.out_begin = out_begin;
+    a.out_end = out_end;
+    a.out = out;
+    const int64_t windows = (out_end - out_begin + 15 + kDelimWindow - 1) / kDelimWindow;
+    return launch("delimited_text_kernel", delimited_text_kernel, grid_cap((size_t)windows, 8), kDelimThreads, 0,
                   (cudaStream_t)stream, false, a);
 }
 

@@ -111,8 +111,8 @@ class SequenceEntryWithQuality(_Entries):
 
 
 def _interval_field(field, value):
-    """Interval and Bed6 fields: text columns (chromosome, name) as text, integer columns (start, stop, score) as int64
-    CUDA tensors and strand as StrandEncoding codes."""
+    """Interval, Bed6 and BedGraph fields: text columns (chromosome, name) as text, integer columns (start, stop, score)
+    as int64 CUDA tensors, a bedGraph value as a CUDA tensor of its own dtype and strand as StrandEncoding codes."""
     if field in ("chromosome", "name"):
         return _from_strings(field, value)
     from . import config
@@ -127,6 +127,8 @@ def _interval_field(field, value):
         return EncodedArray(torch.from_numpy(codes).to(config.default_device()), StrandEncoding)
     if isinstance(value, torch.Tensor):
         return value
+    if field == "value":
+        return torch.as_tensor(np.asarray(value)).to(config.default_device())     # kept in its dtype
     if field == "score" and isinstance(value, list):
         value = [0 if v == "." else int(v) for v in value]        # Optional[int]: "." is 0 (io/strops.py:69-83)
     return torch.as_tensor(np.asarray(value, dtype=np.int64)).to(config.default_device())
@@ -166,3 +168,9 @@ class StrandedInterval(_IntervalEntries):
 class Bed6(_IntervalEntries):
     """datatypes/__init__.py:67-70: Interval + name, score (Optional[int]) and strand."""
     _fields = ("chromosome", "start", "stop", "name", "score", "strand")
+
+
+class BedGraph(_IntervalEntries):
+    """datatypes/__init__.py:27-31: chromosome, start, stop and value.  The value is an integer (or bool) tensor here:
+    the tracks it comes from hold integers, and a float value cannot be written."""
+    _fields = ("chromosome", "start", "stop", "value")

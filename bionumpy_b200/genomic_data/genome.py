@@ -14,7 +14,8 @@ from .. import _native as nv
 from .. import ops
 from ..arithmetics.intervals import (GenomicRunLengthArray, RunsRaggedArray, _add_operators, _device, _int64,
                                      coverage_runs, to_device, track_ufunc)
-from ..datatypes import replace
+from ..datatypes import BedGraph, Interval, replace
+from ..encoded_array import BaseEncoding, EncodedArray, EncodedRaggedArray
 from ..rows import RowView
 
 
@@ -41,6 +42,7 @@ class Genome:
         self.size = int(ends[-1])
         self._fasta_filename = fasta_filename
         self._table = None
+        self._layout_cache = None
 
     @classmethod
     def from_dict(cls, chrom_sizes, *args, **kwargs) -> "Genome":
@@ -92,6 +94,37 @@ class Genome:
             size = to_device(np.array([self._all[n] for n in names], dtype=np.int64), dev)
             self._table = (names, text, to_device(ends, dev), offset, size)
         return self._table
+
+    def _layout(self):
+        """The contigs a track's rows can lie on: the kept contigs of size > 0 in genome order, as their global ends
+        (int64[C + 1], from 0) and their indices in the name table (int64[C]); built once on the device."""
+        if self._layout_cache is None:
+            names = self._name_table()[0]
+            index = {n: i for i, n in enumerate(names)}
+            kept = [n for n, size in self._sizes.items() if size > 0]
+            ends = np.cumsum([0] + [self._sizes[n] for n in kept]).astype(np.int64)
+            dev = self._name_table()[1].device
+            self._layout_cache = (to_device(ends, dev), to_device(np.array([index[n] for n in kept], dtype=np.int64), dev))
+        return self._layout_cache
+
+    def _rows(self, track, mode):
+        """The rows of a global track (bnpk_runs_to_intervals, one synchronisation): (name table index int64, global
+        start, global stop, value or None), each cut at the contig borders."""
+        ends, name_ids = self._layout()
+        dev = ends.device
+        if name_ids.numel() == 0:
+            empty = torch.zeros(0, dtype=torch.int64, device=dev)
+            return empty, empty, empty, empty if mode == nv.RUNS_TO_ALL else None
+        contig, start, stop, value, n_out = ops.runs_to_intervals(track._events, track._values64(), ends, mode)
+        k = int(n_out.cpu()[0])
+        value = None if value is None else value[:k]
+        return name_ids[contig[:k].to(torch.int64)], start[:k], stop[:k], value
+
+    def _names_of(self, ids):
+        """The names of name-table rows ``ids`` (int64) as text views into the device name table, no copy."""
+        _, text, name_offsets, _, _ = self._name_table()
+        lens = (name_offsets[1:] - name_offsets[:-1])[ids].to(torch.int32)
+        return EncodedRaggedArray(EncodedArray(text, BaseEncoding), lens, starts=name_offsets[ids])
 
     def get_intervals(self, intervals, stranded=False) -> "GenomicIntervals":
         """genome.py:181-209: the intervals of a record (Interval, Bed6, ...) placed on this genome."""
@@ -149,6 +182,18 @@ class GenomicIntervals:
         if n_keep < len(ids):
             out = out[torch.nonzero(keep).reshape(-1)]
         return out
+
+    @classmethod
+    def from_track(cls, track) -> "GenomicIntervals":
+        """The intervals where a GenomicArray is not 0 (genomic_intervals.py:529-543), in genome order, cut at contig
+        borders; one synchronisation.  Neighbouring non-zero runs are one interval whatever their values.  The
+        reference returns every run of an integer track as a bedGraph here, against its own docstring; this follows
+        the docstring."""
+        genome = track._genome
+        ids, g_start, g_stop, _ = genome._rows(track._global, nv.RUNS_TO_NONZERO)
+        offset = genome._name_table()[3]
+        record = Interval(genome._names_of(ids), g_start - offset[ids], g_stop - offset[ids])
+        return cls(record, ids.to(torch.int32), g_start, g_stop, genome)
 
     @property
     def chromosome(self):
@@ -282,6 +327,17 @@ class GenomicArray:
 
     def to_dict(self):
         return {name: self._contig(name) for name in self._genome._sizes}
+
+    def get_data(self):
+        """genomic_track.py:199-218: a bool track as the Interval rows where it is True (GenomicIntervals.from_track),
+        any other track as a BedGraph of every run, cut at contig borders, with the track's values; one
+        synchronisation."""
+        if self.dtype == torch.bool:
+            return GenomicIntervals.from_track(self).get_data()
+        genome = self._genome
+        ids, g_start, g_stop, value = genome._rows(self._global, nv.RUNS_TO_ALL)
+        offset = genome._name_table()[3]
+        return BedGraph(genome._names_of(ids), g_start - offset[ids], g_stop - offset[ids], self._global._cast(value))
 
     def sum(self, axis=None, **kwargs):
         return self._global.sum()

@@ -7,5 +7,5 @@ from .write import NpBufferedWriter
 from .parser import CudaFileReader, NpDataclassReader
 from .multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
 from .indexed_fasta import IndexedFasta, read_index, create_index, open_indexed
-from .delimited import DelimitedBuffer, BedBuffer, Bed6Buffer
+from .delimited import DelimitedBuffer, BedBuffer, Bed6Buffer, BdgBuffer
 from .motifs import read_motif

@@ -132,6 +132,11 @@ class CudaOneLineBuffer:
         return cls._write_format_id, 1
 
     @classmethod
+    def formatted(cls, entries):
+        from .write import formatted_entries
+        return formatted_entries(entries, *cls._write_format())
+
+    @classmethod
     def from_data(cls, entries):
         """The records as this format's text: a device EncodedArray (csrc/write_kernels.cu)."""
         from .write import format_entries

@@ -4,13 +4,15 @@
                     record type names via bnpk_delimited_columns: text columns as (chunk, starts, lens) views, integers
                     as int64, strand as StrandEncoding codes.  The chunk is cut after its last newline; the first fault
                     of the chunk is raised as the reference's FormatException(line_number).
-  get_data        : the record type, built lazily from those columns."""
+  get_data        : the record type, built lazily from those columns.
+  from_data       : the record's own fields as tab-separated lines, formatted on the device (bnpk_delimited_offsets /
+                    bnpk_delimited_format): text as it is, integers in decimal, strand as '+', '-' or '.'."""
 import torch
 
 from .. import _native as nv
 from .. import ops
-from ..datatypes import Bed6, Interval
-from ..encoded_array import EncodedArray, BaseEncoding
+from ..datatypes import Bed6, BedGraph, Interval, StrandedInterval
+from ..encoded_array import EncodedArray, EncodedRaggedArray, BaseEncoding
 from ..encodings import StrandEncoding
 from .buffers import FieldView, _to_device_bytes
 from .exceptions import FormatException, IncompleteEntryException
@@ -108,8 +110,16 @@ class DelimitedBuffer:
         return self.dataclass.lazy(self)
 
     @classmethod
+    def formatted(cls, entries):
+        """The text of a record chunk, its size known and any byte range formatted on demand (the writer's protocol)."""
+        return DelimitedText(entries)
+
+    @classmethod
     def from_data(cls, entries):
-        raise NotImplementedError("writing BED is not supported")
+        """The records as tab-separated lines of their own fields (delimited_buffers.py:150-160): a device
+        EncodedArray.  Bed6 records give six columns whatever the buffer type."""
+        text = DelimitedText(entries)
+        return EncodedArray(text.slice(0, text.size), BaseEncoding)
 
 
 class BedBuffer(DelimitedBuffer):
@@ -122,3 +132,58 @@ class Bed6Buffer(DelimitedBuffer):
     """delimited_buffers.py Bed6Buffer: chromosome, start, stop, name, score (. = 0), strand."""
     dataclass = Bed6
     _kinds = (nv.COL_TEXT, nv.COL_INT, nv.COL_INT, nv.COL_TEXT, nv.COL_INT_OR_DOT, nv.COL_STRAND)
+
+
+class BdgBuffer(DelimitedBuffer):
+    """bedGraph: chromosome, start, stop and an integer value.  Written only: the reference reads bedGraph values as
+    floats, and this package has no float tracks."""
+    dataclass = BedGraph
+
+    @classmethod
+    def from_raw_buffer(cls, chunk, header_data=None):
+        raise NotImplementedError("reading bedGraph is not supported: its values are floats")
+
+
+_WRITTEN = (Interval, StrandedInterval, Bed6, BedGraph)
+
+
+def _column(entries, field):
+    """(nv.COL_*, tensors) of one field of a record chunk."""
+    from .write import _view
+    value = getattr(entries, field)
+    if isinstance(value, EncodedRaggedArray):
+        if not value.encoding.is_base_encoding():
+            raise TypeError(f"the {field} column must be text, got {value.encoding}")
+        return nv.COL_TEXT, _view(value)
+    if isinstance(value, EncodedArray):
+        if value.encoding != StrandEncoding:
+            raise TypeError(f"the {field} column must be text or strand codes, got {value.encoding}")
+        return nv.COL_STRAND, value.raw().reshape(-1).to(torch.uint8).contiguous()
+    if not isinstance(value, torch.Tensor):
+        raise TypeError(f"the {field} column must be a tensor, got {type(value).__name__}")
+    if value.is_floating_point() or value.is_complex():
+        raise TypeError(f"the {field} column holds {value.dtype}: only integer values are written")
+    if not value.is_cuda:
+        raise nv.NativeLibraryError("writing needs CUDA tensors: bionumpy_b200 has no CPU fallback")
+    return nv.COL_INT, value.reshape(-1).to(torch.int64).contiguous()
+
+
+class DelimitedText:
+    """The tab-separated text of a record chunk: line offsets on the device and the size, read with the first bad
+    strand code in one synchronisation; ``slice(a, b, out)`` formats bytes [a, b)."""
+
+    def __init__(self, entries):
+        if not isinstance(entries, _WRITTEN):
+            raise TypeError(f"cannot write {type(entries).__name__} as delimited text: "
+                            f"{', '.join(t.__name__ for t in _WRITTEN)} are written")
+        self.columns = [_column(entries, f) for f in entries._fields]
+        self.offsets, status = ops.delimited_offsets(self.columns)
+        self.size, fault = (int(x) for x in torch.cat([self.offsets[-1:],
+                                                       status[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]).cpu().tolist())
+        if fault != nv.INT64_MAX:
+            line, col = fault >> 8, (fault >> 3) & 31
+            raise ValueError(f"line {line}: the {entries._fields[col]} column holds a strand code that is not "
+                             "'+', '-' or '.'")
+
+    def slice(self, begin, end, out=None):
+        return ops.delimited_format(self.columns, self.offsets, begin, end, out)

@@ -28,8 +28,11 @@ def _buffer_type_for(suffix):
     if suffix == ".bed":
         from .delimited import BedBuffer
         return BedBuffer
+    if suffix == ".bdg":
+        from .delimited import BdgBuffer
+        return BdgBuffer
     raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
-                       f"(supported: .fq .fastq .fa .fasta .bed and their .gz forms); pass buffer_type=")
+                       f"(supported: .fq .fastq .fa .fasta .bed .bdg and their .gz forms); pass buffer_type=")
 
 
 def _suffix(path):
@@ -42,17 +45,20 @@ def _suffix(path):
 
 def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
     """files.py:85-182.  Reading ("r", "rb") gives an NpDataclassReader; writing ("w", "wb", "write") or appending
-    ("a", "ab", "append") gives an NpBufferedWriter, which writes ``.gz`` files as BGZF."""
+    ("a", "ab", "append") gives an NpBufferedWriter, which writes ``.gz`` files as BGZF.  ``.bdg`` (bedGraph) is
+    written only.  BED is written with the buffer type named: ``bnp.open("x.bed", "w", buffer_type=BedBuffer)`` (or
+    Bed6Buffer; either writes a record's own fields).  Opening ``.bed`` for writing by its suffix alone raises
+    NotImplementedError, as it did before BED could be written, so code that relies on that keeps working."""
     if mode not in (None, "r", "rb") and mode not in WRITE_MODES:
         raise NotImplementedError(f"mode {mode!r}: use r/rb to read, w/wb/write or a/ab/append to write")
     path = str(filename)
     suffix, is_gzip = _suffix(path)
+    if mode in WRITE_MODES and buffer_type is None and suffix == ".bed":
+        raise NotImplementedError("writing .bed by its suffix alone is not supported: name the format with "
+                                  "buffer_type=bnp.io.BedBuffer (or Bed6Buffer)")
     if buffer_type is None:
         buffer_type = _buffer_type_for(suffix)
     if mode in WRITE_MODES:
-        from .delimited import DelimitedBuffer
-        if isinstance(buffer_type, type) and issubclass(buffer_type, DelimitedBuffer):
-            raise NotImplementedError(f"writing {suffix} files is not supported")
         from .write import NpBufferedWriter
         raw = open(path, WRITE_MODES[mode])
         if is_gzip:

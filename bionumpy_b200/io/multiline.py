@@ -140,6 +140,11 @@ class CudaMultiLineFastaBuffer:
         return nv.FMT_FASTA_WRAPPED, int(cls.n_characters_per_line)
 
     @classmethod
+    def formatted(cls, entries):
+        from .write import formatted_entries
+        return formatted_entries(entries, *cls._write_format())
+
+    @classmethod
     def from_data(cls, entries):
         """The records as FASTA with n_characters_per_line bases per line: a device EncodedArray.  An entry with an
         empty sequence is its header line alone."""

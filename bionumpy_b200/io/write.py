@@ -136,10 +136,14 @@ class Formatted:
         return ops.format_records(self.fmt, self.line_width, self.fields, self.offsets, begin, end, out)
 
 
+def formatted_entries(entries, fmt, line_width=1):
+    """The text of a record chunk in a sequence format (the buffers' ``formatted``, which the writer calls)."""
+    return Formatted(entry_fields(entries, fmt), fmt, line_width)
+
+
 def format_entries(entries, fmt, line_width=1):
     """All of a chunk's text as one device tensor (the buffers' from_data)."""
-    fields = entry_fields(entries, fmt)
-    f = Formatted(fields, fmt, line_width)
+    f = formatted_entries(entries, fmt, line_width)
     return EncodedArray(f.slice(0, f.size), BaseEncoding)
 
 
@@ -222,7 +226,9 @@ class _HostSink:
 
 
 class NpBufferedWriter:
-    """parser.py:209-273: writes record chunks to a file object in the format of ``buffer_type``."""
+    """parser.py:209-273: writes record chunks to a file object in the format of ``buffer_type``, whose
+    ``formatted(chunk)`` gives the chunk's text: its ``size``, its line ``offsets`` on the device and
+    ``slice(a, b, out)``, which formats bytes [a, b) into ``out``."""
 
     def __init__(self, file_obj, buffer_type):
         self._file_obj = file_obj
@@ -260,8 +266,7 @@ class NpBufferedWriter:
             return
         if len(data) == 0:
             return
-        fmt, width = self._buffer_type._write_format()
-        f = Formatted(entry_fields(data, fmt), fmt, width)
+        f = self._buffer_type.formatted(data)
         dev = f.offsets.device
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream()

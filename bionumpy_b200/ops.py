@@ -734,3 +734,89 @@ def interval_intersect(start, stop, same_prev=None, rows=True):
     check(lib().bnpk_interval_intersect(ptr(start), ptr(stop), ptr(same_prev), n, ptr(out_rows), ptr(out_stops),
                                         ptr(n_out), ptr(overlap), ptr(ws), ws.numel(), stream_ptr()))
     return out_rows, out_stops, n_out, overlap
+
+
+@_on_device
+def runs_to_intervals(run_starts, values, contig_ends, mode=nv.RUNS_TO_NONZERO):
+    """bnpk_runs_to_intervals: the rows of a global track cut at the contig ends (int64[C + 1], strictly increasing
+    from 0 to the size): (contig int32, start int64, stop int64, value int64 or None, n_out int64[1]), each of capacity
+    R + C, the first n_out rows valid (nothing is read back).  nv.RUNS_TO_NONZERO: the stretches of non-zero value;
+    nv.RUNS_TO_ALL: every run, with its value."""
+    _int64_args((run_starts, "run_starts"), (values, "values"), (contig_ends, "contig_ends"))
+    if run_starts.numel() != values.numel() + 1:
+        raise ValueError("a track is R values and R + 1 run starts")
+    if contig_ends.numel() < 2:
+        raise ValueError("contig_ends holds 0 and the end of every contig")
+    n, c, dev = values.numel(), contig_ends.numel() - 1, run_starts.device
+    contig = torch.empty(n + c, dtype=torch.int32, device=dev)
+    start, stop = (torch.empty(n + c, dtype=torch.int64, device=dev) for _ in range(2))
+    value = torch.empty(n + c, dtype=torch.int64, device=dev) if mode == nv.RUNS_TO_ALL else None
+    n_out = torch.empty(1, dtype=torch.int64, device=dev)
+    ws = nv.workspace(max(n, 1), dev)
+    check(lib().bnpk_runs_to_intervals(ptr(run_starts), ptr(values), n, ptr(contig_ends), c, mode, ptr(contig),
+                                       ptr(start), ptr(stop), ptr(value), ptr(n_out), ptr(ws), ws.numel(),
+                                       stream_ptr()))
+    return contig, start, stop, value, n_out
+
+
+def _out_columns(columns):
+    """A host bnpk_out_column[k] of columns given as (nv.COL_TEXT, (base uint8, starts int64, lens int32)),
+    (nv.COL_INT, int64) or (nv.COL_STRAND, uint8) CUDA tensors of one row count.  Returns (array, rows, device)."""
+    if not 1 <= len(columns) <= nv.MAX_OUT_COLUMNS:
+        raise ValueError(f"1 to {nv.MAX_OUT_COLUMNS} columns")
+    arr = (nv.OutColumn * len(columns))()
+    rows, dev = None, None
+    for i, (kind, data) in enumerate(columns):
+        if kind == nv.COL_TEXT:
+            base_p, base_bytes, starts_p, lens_p, n = _rows_args(*data)
+            arr[i] = nv.OutColumn(kind, base_p.value, base_bytes, starts_p.value, lens_p.value)
+            d = data[0].device
+        elif kind in (nv.COL_INT, nv.COL_STRAND):
+            _need_cuda(data, "column")
+            want = torch.int64 if kind == nv.COL_INT else torch.uint8
+            if data.dtype != want:
+                raise TypeError(f"an {'INT' if kind == nv.COL_INT else 'STRAND'} column must be {want}")
+            arr[i] = nv.OutColumn(kind, data.data_ptr() or None, 0, None, None)
+            n, d = data.numel(), data.device
+        else:
+            raise ValueError(f"unknown column kind {kind}")
+        if rows is None:
+            rows, dev = n, d
+        if n != rows:
+            raise ValueError(f"the columns differ in length ({rows} and {n} rows)")
+        if d != dev:
+            raise ValueError("the columns are on different devices")
+    return arr, rows, dev
+
+
+def delimited_offsets(columns, status=None):
+    """bnpk_delimited_offsets: (int64[E + 1] line offsets, status); a strand code above 2 is reported in
+    status[ST_BAD_BASE] as (line << 8 | column << 3 | nv.BAD_STRAND)."""
+    arr, n, dev = _out_columns(columns)
+    with torch.cuda.device(dev):
+        offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        if status is None:
+            status = nv.new_status(dev)
+        ws = nv.workspace(max(n, 1), dev)
+        check(lib().bnpk_delimited_offsets(ctypes.cast(arr, ctypes.c_void_p), len(columns), n, ptr(offsets),
+                                           ptr(status), ptr(ws), ws.numel(), stream_ptr()))
+    return offsets, status
+
+
+@_on_device
+def delimited_format(columns, offsets, out_begin=0, out_end=None, out=None):
+    """Bytes [out_begin, out_end) of the lines (default: all, offsets[-1] read back) into ``out`` (uint8, at least
+    out_end - out_begin bytes; allocated when None).  Returns ``out``."""
+    _need_cuda(offsets, "offsets")
+    arr, n, _ = _out_columns(columns)
+    if offsets.dtype != torch.int64 or offsets.numel() != n + 1:
+        raise ValueError("offsets must be int64[E + 1]")
+    if out_end is None:
+        out_end = int(offsets[-1].item())
+    if out is None:
+        out = torch.empty(max(out_end - out_begin, 0), dtype=torch.uint8, device=offsets.device)
+    elif out.numel() < out_end - out_begin:
+        raise ValueError("out is smaller than the range")
+    check(lib().bnpk_delimited_format(ctypes.cast(arr, ctypes.c_void_p), len(columns), n, ptr(offsets), out_begin,
+                                      out_end, ptr(out) if out.numel() else None, stream_ptr()))
+    return out

@@ -455,6 +455,25 @@ int bnpk_interval_intersect(const int64_t *start, const int64_t *stop, const uin
                             int64_t *out_rows, int64_t *out_stops, int64_t *n_out, int64_t *overlap, void *workspace,
                             size_t workspace_bytes, void *stream);
 
+/* K13  a track back into interval rows (GenomicIntervals.from_track, genomic_data/genomic_intervals.py:529-543;
+ *   GenomicArray.get_data / _get_intervals_from_data, genomic_data/genomic_track.py:84-91,199-218).
+ *   The track is n_runs runs of a global layout (run_starts int64[R + 1], values int64[R], every run non-empty) and
+ *   contig_ends int64[C + 1] are the ends of the contigs in it: contig_ends[0] = 0, strictly increasing (a contig of
+ *   size 0 has no positions: leave it out), contig_ends[C] = run_starts[R].  A row is one piece of the track inside one
+ *   contig, in order: out_contig[g] (int32, index into contig_ends), out_start[g], out_stop[g] (global) and, in
+ *   BNPK_RUNS_TO_ALL mode, out_value[g].
+ *     BNPK_RUNS_TO_NONZERO  the maximal stretches of non-zero value, cut at contig borders (out_value not written,
+ *                           may be NULL): neighbouring non-zero runs are one row whatever their values
+ *     BNPK_RUNS_TO_ALL      every run, cut at contig borders (bedGraph)
+ *   *n_out = the row count (int64).  Capacity of every output: n_runs + n_contigs rows.  workspace as for
+ *   bnpk_row_offsets with n := n_runs.  BNPK_E_BADARG for an unknown mode, n_contigs < 1 with n_runs > 0 and a
+ *   missing pointer. */
+#define BNPK_RUNS_TO_NONZERO 0
+#define BNPK_RUNS_TO_ALL     1
+int bnpk_runs_to_intervals(const int64_t *run_starts, const int64_t *values, size_t n_runs, const int64_t *contig_ends,
+                           size_t n_contigs, int mode, int32_t *out_contig, int64_t *out_start, int64_t *out_stop,
+                           int64_t *out_value, int64_t *n_out, void *workspace, size_t workspace_bytes, void *stream);
+
 /* Bloom filter over k-mer hashes (sequence/bloom_filter.py:15-42): hash function i is v ^ offsets[i]; the filter is
  * one byte per position (the reference's bool mask).  insert: mask[(v ^ offsets[i]) % mask_size] = 1 for every value and
  * function; query: out[j] = AND over the functions. */
@@ -504,6 +523,35 @@ int bnpk_format_offsets(int format, int line_width, size_t n_entries, const bnpk
  * out_begin).  Any range may be asked for, so a large text can be formatted in slices. */
 int bnpk_format_records(int format, int line_width, size_t n_entries, const bnpk_field *fields,
                         const int64_t *out_offsets, int64_t out_begin, int64_t out_end, uint8_t *out, void *stream);
+
+/* K14  delimited text from columns (dump_csv / join_columns, io/dump_csv.py, io/strops.py:186-215): line e is its
+ *   columns joined by '\t' and ended by '\n'.  `columns` is a HOST array of n_columns (1..BNPK_MAX_OUT_COLUMNS)
+ *   bnpk_out_column, each with E rows, written as its kind says (the reader's column kinds):
+ *     BNPK_COL_TEXT    the bytes base[starts[e] .. + lens[e]) (negative length = empty; a byte outside
+ *                      [base, base + base_bytes) is written as 0), copied as they are
+ *     BNPK_COL_INT     values[e] (int64) in decimal: '-' for a negative value, no leading zero, 0 as "0"
+ *     BNPK_COL_STRAND  codes[e] (uint8, StrandEncoding) as '+' (0), '-' (1), '.' (2); another code is written as '.'
+ *                      and reported by bnpk_delimited_offsets
+ *   bnpk_delimited_offsets: out_offsets int64[E + 1], the exclusive prefix sum of the line sizes (out_offsets[E] = the
+ *   text's size); the first bad strand code is atomicMin-ed into status[BNPK_ST_BAD_BASE] as (line << 8 | column << 3
+ *   | BNPK_BAD_STRAND) (status pre-initialised).  workspace as for bnpk_row_offsets with n := E.
+ *   bnpk_delimited_format: bytes [out_begin, out_end) of that text written to out[0 .. out_end - out_begin), as
+ *   bnpk_format_records.  BNPK_E_BADARG before any device work for a bad column count or kind, a missing pointer,
+ *   out_begin < 0 or out_end < out_begin. */
+#define BNPK_MAX_OUT_COLUMNS 8
+
+typedef struct bnpk_out_column {
+    int kind;
+    const void *data;          /* TEXT: base bytes; INT: int64[E]; STRAND: uint8[E] */
+    size_t base_bytes;         /* TEXT */
+    const int64_t *starts;     /* TEXT: int64[E] */
+    const int32_t *lens;       /* TEXT: int32[E] */
+} bnpk_out_column;
+
+int bnpk_delimited_offsets(const bnpk_out_column *columns, int n_columns, size_t n_lines, int64_t *out_offsets,
+                           int64_t *status, void *workspace, size_t workspace_bytes, void *stream);
+int bnpk_delimited_format(const bnpk_out_column *columns, int n_columns, size_t n_lines, const int64_t *out_offsets,
+                          int64_t out_begin, int64_t out_end, uint8_t *out, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * Host-buffer entry point (end-to-end): the call a reader loop makes with a chunk that is
