@@ -21,7 +21,8 @@ namespace bnpk {
 // -------------------------------------------------------------------------------------------
 // init: decide '\r' trimming like OneLineBuffer._modify_for_carriage_return
 // (io/one_line_buffer.py:175-182): trim iff the header line of one of the first
-// `lines_per_entry` entries ends in '\r'.
+// `lines_per_entry` complete entries ends in '\r'.  A header's '\r' counts only once the walk
+// has found the last newline of its entry: the incomplete tail does not decide.
 // -------------------------------------------------------------------------------------------
 __global__ void cr_detect_kernel(const uint8_t *chunk, size_t n, int lpe, int trim_cr, int64_t *status) {
     if (blockIdx.x != 0 || threadIdx.x >= 32) return;
@@ -30,10 +31,12 @@ __global__ void cr_detect_kernel(const uint8_t *chunk, size_t n, int lpe, int tr
     if (trim_cr == 1) cr = 1;
     if (trim_cr < 0) {
         int64_t pos = 0;
+        bool header_cr = false;
         for (int line = 0; line < lpe * lpe && pos < (int64_t)n; ++line) {
             const int64_t len = warp_line_len(chunk, n, pos, lane);
             if (len < 0) break;
-            if (line % lpe == 0 && len > 0 && chunk[pos + len - 1] == '\r') { cr = 1; break; }
+            if (line % lpe == 0) header_cr = len > 0 && chunk[pos + len - 1] == '\r';
+            if (line % lpe == lpe - 1 && header_cr) { cr = 1; break; }
             pos += len + 1;
         }
     }

@@ -214,6 +214,7 @@ class PinnedFileReader(CudaFileReader):
         self._source = source
         self._pending = None
         self._tail = None                              # device bytes that belong to the next chunk
+        self._tail_last = NEWLINE                      # the tail's last byte, known on the host
 
     def close(self):
         self._source.close()
@@ -250,14 +251,16 @@ class PinnedFileReader(CudaFileReader):
             if total == 0:
                 self._is_finished = True
                 return None
-            add_nl = last and nread > 0 and int(pinned[nread - 1]) != NEWLINE or (last and nread == 0 and tail_len > 0)
+            last_byte = int(pinned[nread - 1]) if nread else self._tail_last
+            add_nl = last and last_byte != NEWLINE                       # parser.py:183-186
             d = torch.empty(total + (1 if add_nl else 0), dtype=torch.uint8, device=dev)
             if tail_len:
                 d[:tail_len] = self._tail
             if nread:
                 d[tail_len:total].copy_(pinned[:nread], non_blocking=True)
             if add_nl:
-                d[total:] = NEWLINE                                      # parser.py:183-186
+                d[total:] = NEWLINE
+                last_byte = NEWLINE
             if max_chunk_size is not None and d.numel() > max_chunk_size:
                 raise Exception("No complete entry found")
             _, _, status = ops.line_split(d, lpe, 1, 0, ord(bt.HEADER), bt._check_plus, -1, max_rows=0)
@@ -266,7 +269,7 @@ class PinnedFileReader(CudaFileReader):
                 if last:
                     self._is_finished = True
                     return None
-                self._tail = d                                           # no complete entry yet: read more
+                self._tail, self._tail_last = d, last_byte               # no complete entry yet: read more
                 continue
             if st.bad_header_entry is not None:
                 raise FormatException(f"Expected header line to start with {bt.HEADER}",
@@ -277,6 +280,7 @@ class PinnedFileReader(CudaFileReader):
             size = st.n_complete_bytes
             buff = bt(d[:size], st.n_records, st.cr)
             self._tail = None if last or size == d.numel() else d[size:].clone()
+            self._tail_last = last_byte
             self._is_finished = last
             self.n_bytes_read += size
             self.n_lines_read += buff.n_lines
