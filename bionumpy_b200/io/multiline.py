@@ -73,13 +73,8 @@ class CudaMultiLineFastaBuffer:
         chunk = _to_device_bytes(chunk)
         assert chunk.numel() and int(chunk[0].item()) == ord(">"), "multi-line FASTA chunk must start with '>'"
         starts, lens = cls._lines(chunk)
-        n_lines = starts.numel()
         # header flags, the last newline that is followed by an entry start (multiline_buffer.py:93), '\r' probe: one kernel
-        is_header = torch.empty(n_lines, dtype=torch.int32, device=chunk.device)
-        out2 = torch.zeros(2, dtype=torch.int64, device=chunk.device)
-        with torch.cuda.device(chunk.device):
-            nv.check(nv.lib().bnpk_multiline_flags(nv.ptr(chunk), chunk.numel(), nv.ptr(starts), nv.ptr(lens), n_lines,
-                                                   nv.ptr(is_header), nv.ptr(out2), nv.stream_ptr()))
+        is_header, out2 = ops.multiline_flags(chunk, starts, lens)
         keep, has_cr = (int(x) for x in out2.cpu().tolist())          # the one synchronisation of this buffer
         if keep == 0:
             raise IncompleteEntryException("No complete entry found in multi-line FASTA buffer")
@@ -108,21 +103,10 @@ class CudaMultiLineFastaBuffer:
 
     def _materialise(self):
         if self._cache is None:
-            dev = self._data.device
-            keep, n_e = self._line_starts.numel(), self._n_entries
-            n_seq = keep - n_e
-            h_starts = torch.empty(n_e, dtype=torch.int64, device=dev)
-            h_lens = torch.empty(n_e, dtype=torch.int32, device=dev)
-            s_starts = torch.empty(n_seq, dtype=torch.int64, device=dev)
-            s_lens = torch.empty(n_seq, dtype=torch.int32, device=dev)
-            entry_lens = torch.zeros(n_e, dtype=torch.int64, device=dev)
-            starts, lens, hdr = self._line_starts.contiguous(), self._line_lens.contiguous(), self._is_header.contiguous()
-            with torch.cuda.device(dev):
-                nv.check(nv.lib().bnpk_multiline_entries(nv.ptr(self._data), nv.ptr(starts), nv.ptr(lens), nv.ptr(hdr),
-                                                         nv.ptr(self._hdr_before), keep, int(self._trim_cr), nv.ptr(h_starts),
-                                                         nv.ptr(h_lens), nv.ptr(s_starts), nv.ptr(s_lens), nv.ptr(entry_lens),
-                                                         nv.stream_ptr()))
-            flat, _, _ = ops.rows_encode(self._data, s_starts, s_lens, nv.ENC_LUT, _identity_lut(dev))
+            h_starts, h_lens, s_starts, s_lens, entry_lens = ops.multiline_entries(
+                self._data, self._line_starts, self._line_lens, self._is_header, self._hdr_before, self._n_entries,
+                self._trim_cr)
+            flat, _, _ = ops.rows_encode(self._data, s_starts, s_lens, nv.ENC_LUT, _identity_lut(self._data.device))
             names = FieldView(self._data, h_lens, h_starts)
             seqs = EncodedRaggedArray(EncodedArray(flat, BaseEncoding), entry_lens.to(torch.int32))
             self._cache = (names, seqs)

@@ -5,6 +5,7 @@ import numpy as np
 import torch
 
 from .. import _native as nv
+from .. import ops
 from ..encoded_array import EncodedArray
 from ..ragged import RaggedArray
 
@@ -48,16 +49,9 @@ class BloomFilter:
 
     def insert(self, sequences):
         """bloom_filter.py:37-39."""
-        v = _values(sequences).reshape(-1)
-        with torch.cuda.device(self._mask.device):
-            nv.check(nv.lib().bnpk_bloom_insert(nv.ptr(v), v.numel(), nv.ptr(self._offsets), self._offsets.numel(),
-                                                nv.ptr(self._mask), self._mask.numel(), nv.stream_ptr()))
+        ops.bloom_insert(_values(sequences).reshape(-1), self._offsets, self._mask)
 
     def __getitem__(self, idx):
         """bloom_filter.py:41-42: membership of every value (bool tensor of the same shape)."""
         v = _values(idx)
-        out = torch.empty(v.numel(), dtype=torch.uint8, device=self._mask.device)
-        with torch.cuda.device(self._mask.device):
-            nv.check(nv.lib().bnpk_bloom_query(nv.ptr(v.reshape(-1)), v.numel(), nv.ptr(self._offsets), self._offsets.numel(),
-                                               nv.ptr(self._mask), self._mask.numel(), nv.ptr(out), nv.stream_ptr()))
-        return out.to(torch.bool).reshape(v.shape)
+        return ops.bloom_query(v.reshape(-1), self._offsets, self._mask).to(torch.bool).reshape(v.shape)

@@ -173,9 +173,7 @@ class KmerCounter:
 
     def _status(self):
         """The status block (first ST_WORDS words of the state; the last word is n_used), re-initialised."""
-        status = self._state[:nv.ST_WORDS]
-        nv.check(nv.lib().bnpk_status_init(nv.ptr(status), nv.stream_ptr()))
-        return status
+        return ops.reset_status(self._state[:nv.ST_WORDS])
 
     def _read_state(self):
         words = self._state.tolist()

@@ -188,7 +188,7 @@ class _Pattern:
         out = torch.empty(total, dtype=torch.uint8, device=rows.base.device)
         status = ops.nv.new_status(rows.base.device)
         for g, s, idx in groups:
-            g_off = p_off if idx is None else p_off[idx].contiguous()
+            g_off = p_off if idx is None else p_off[torch.cat([idx, idx[-1:] + 1])]     # and the end of the last piece
             ops.rows_match(g.base, g.starts, g.lens, *self._launch_args(rows), same=s, lut=rows.lut, offsets=g_off,
                            status=status, out=out)
         rows.raise_bad_base(status, self._rescan if piece_row is not None else None)

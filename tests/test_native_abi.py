@@ -88,3 +88,38 @@ def test_dominant_kernels_are_sm90a_code_without_spills():
         seen[name] = (int(m.group(1)), int(m.group(2)))
         assert int(m.group(1)) <= regs_max and int(m.group(2)) == 0, (name, m.group(0))
     assert len(seen) == 2
+
+
+def _python_sources(path):
+    for dirpath, _, files in os.walk(path):
+        for f in sorted(files):
+            if f.endswith(".py"):
+                yield os.path.join(dirpath, f)
+
+
+def test_only_the_bindings_call_the_library():
+    """Every call of libbnpk.so from the package goes through ops.py, which checks its tensors, or _native.py: no other
+    module names a bnpk_* symbol.  In ops.py, only the one tensor rule (_pointer) makes pointers and only _on_device
+    switches the device."""
+    import ast
+    pkg = os.path.join(ROOT, "bionumpy_b200")
+    found = []
+    for path in _python_sources(pkg):
+        if os.path.basename(path) in ("ops.py", "_native.py") and os.path.dirname(path) == pkg:
+            continue
+        for node in ast.walk(ast.parse(open(path).read())):
+            name = getattr(node, "attr", None) or getattr(node, "id", None) or ""
+            if isinstance(node, ast.Constant) and isinstance(node.value, str):
+                name = node.value
+            if re.fullmatch(r"bnpk_\w+", name):
+                found.append(f"{os.path.relpath(path, ROOT)}:{node.lineno} {name}")
+    assert not found, found
+    tree = ast.parse(open(os.path.join(pkg, "ops.py")).read())
+    methods = [m for c in tree.body if isinstance(c, ast.ClassDef) for m in c.body]
+    for fn in [f for f in tree.body + methods if isinstance(f, ast.FunctionDef)]:
+        for node in ast.walk(fn):
+            if isinstance(node, ast.Call):
+                callee = ast.unparse(node.func)
+                assert callee != "ptr" or fn.name == "_pointer", f"ptr() in {fn.name}"
+                assert callee != "torch.cuda.device" or fn.name == "_on_device", f"a device switch in {fn.name}"
+                assert not callee.endswith(".data_ptr"), f"data_ptr() in {fn.name}"

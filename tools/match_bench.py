@@ -68,7 +68,7 @@ def case(name, seq, matcher, mode, iters):
     out = torch.empty(total, dtype=torch.uint8, device=rows.base.device)
     status = nv.new_status(rows.base.device)
     launch = pat._launch_args(rows)
-    prepared = [(g, s, p_off if idx is None else p_off[idx].contiguous()) for g, s, idx in groups]
+    prepared = [(g, s, p_off if idx is None else p_off[torch.cat([idx, idx[-1:] + 1])]) for g, s, idx in groups]
 
     def run_matches():
         for g, s, off in prepared:

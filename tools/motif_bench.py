@@ -66,7 +66,7 @@ def case(name, base, starts, lens, enc_mode, pwm, iters):
     best = torch.empty(p_lens.numel(), dtype=torch.float64, device=base.device)
     status = nv.new_status(base.device)
     lib = nv.lib()
-    args = ops._rows_args(base, p_starts, p_lens)
+    args, _ = ops._rows_args(base, p_starts, p_lens)
     st = nv.stream_ptr()
 
     def run_scores():
