@@ -24,9 +24,10 @@ from .sequence import KmerIndex, KmerLookup, BloomFilter
 from .sequence import count_kmers_exact, KmerCounter, KmerCounts
 from .io.buffers import CudaFastQBuffer, CudaTwoLineFastaBuffer, FastQBuffer, TwoLineFastaBuffer
 from .io.multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
-from .datatypes import SequenceEntry, SequenceEntryWithQuality, Interval, StrandedInterval, Bed6, BedGraph, replace
+from .datatypes import (SequenceEntry, SequenceEntryWithQuality, Interval, StrandedInterval, Bed6, BedGraph, BamEntry,
+                        replace)
 from . import datatypes
-from . import arithmetics, genomic_data
+from . import arithmetics, genomic_data, alignments
 from .genomic_data import Genome, GenomicIntervals, GenomicArray
 from .io.files import count_entries
 from .io.write import NpBufferedWriter

@@ -30,6 +30,10 @@ RUNS_MAX, RUNS_MIN, RUNS_SUM, RUNS_ANY = 0, 1, 2, 3
  OP_GE) = range(14)
 RUNS_TO_NONZERO, RUNS_TO_ALL = 0, 1
 MAX_OUT_COLUMNS = 8
+BAM_BAD_BLOCK_SIZE, BAM_BAD_REF_ID, BAM_BAD_NAME, BAM_BAD_SIZES, BAM_BAD_CIGAR_OP, BAM_TRUNCATED = 1, 2, 3, 4, 5, 6
+(BAM_F_REF_ID, BAM_F_POS, BAM_F_MAPQ, BAM_F_FLAG, BAM_F_NAME_START, BAM_F_NAME_LEN, BAM_F_CIGAR_START, BAM_F_N_CIGAR,
+ BAM_F_SEQ_START, BAM_F_L_SEQ, BAM_F_QUAL_START, BAM_F_REF_LEN) = range(12)
+BAM_FIELDS = 12
 INT64_MAX = (1 << 63) - 1
 SMEM_MAX_BINS = 32768
 
@@ -94,6 +98,10 @@ SIGNATURES = {
     "bnpk_runs_to_intervals": (_i, [_vp, _vp, _sz, _vp, _sz, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "bnpk_delimited_offsets": (_i, [_vp, _i, _sz, _vp, _vp, _vp, _sz, _vp]),
     "bnpk_delimited_format": (_i, [_vp, _i, _sz, _vp, _i64, _i64, _vp, _vp]),
+    "bnpk_bam_split": (_i, [_vp, _sz, _i, _sz, _vp, _sz, _vp, _vp, _sz, _vp]),
+    "bnpk_bam_fields": (_i, [_vp, _sz, _vp, _sz, _vp, _vp, _vp]),
+    "bnpk_bam_sequence": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp]),
+    "bnpk_bam_cigar": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
 }
 
 

@@ -692,6 +692,65 @@ Tensor delimited_format(const std::vector<Tensor> &columns, const std::vector<in
     return out;
 }
 
+// BAM records: (starts int64[n / 36 + 1], status); the first status[N_RECORDS] starts are the complete records
+std::tuple<Tensor, Tensor> bam_split(const Tensor &chunk, int64_t n_ref, int64_t segment_bytes) {
+    need(chunk, torch::kUInt8, "chunk");
+    TORCH_CHECK(segment_bytes >= 64, "bnpk: segment_bytes must be at least 64");
+    c10::cuda::CUDAGuard guard(chunk.device());
+    const int64_t n = chunk.numel();
+    Tensor starts = torch::empty({n / 36 + 1}, chunk.options().dtype(torch::kInt64));
+    Tensor status = new_status(chunk);
+    Tensor ws = torch::empty({7 * std::max<int64_t>((n + segment_bytes - 1) / segment_bytes, 1)}, starts.options());
+    check(bnpk_bam_split(u8(chunk), (size_t)n, (int)n_ref, (size_t)segment_bytes, starts.data_ptr<int64_t>(),
+                         (size_t)starts.numel(), status.data_ptr<int64_t>(), ws.data_ptr<int64_t>(), (size_t)ws.numel(),
+                         cur_stream(chunk)),
+          "bam_split");
+    return {starts, status};
+}
+
+// the fields of the records bam_split found: int64[BNPK_BAM_FIELDS, starts.numel()]
+Tensor bam_fields(const Tensor &chunk, const Tensor &starts, Tensor status) {
+    need(chunk, torch::kUInt8, "chunk");
+    need(starts, torch::kInt64, "starts", chunk);
+    need(status, torch::kInt64, "status", chunk);
+    TORCH_CHECK(status.numel() >= BNPK_ST_WORDS, "bnpk: status must have BNPK_ST_WORDS words");
+    c10::cuda::CUDAGuard guard(chunk.device());
+    Tensor fields = torch::empty({BNPK_BAM_FIELDS, starts.numel()}, starts.options());
+    check(bnpk_bam_fields(u8(chunk), (size_t)chunk.numel(), starts.data_ptr<int64_t>(), (size_t)starts.numel(),
+                          fields.data_ptr<int64_t>(), status.data_ptr<int64_t>(), cur_stream(chunk)),
+          "bam_fields");
+    return fields;
+}
+
+Tensor bam_sequence(const Tensor &chunk, const Tensor &seq_start, const Tensor &offsets, int64_t total) {
+    need(chunk, torch::kUInt8, "chunk");
+    need(seq_start, torch::kInt64, "seq_start", chunk);
+    const int64_t *off = need_offsets(offsets, (size_t)seq_start.numel(), chunk);
+    c10::cuda::CUDAGuard guard(chunk.device());
+    Tensor out = torch::empty({total}, chunk.options());
+    if (total == 0) return out;
+    check(bnpk_bam_sequence(u8(chunk), (size_t)chunk.numel(), seq_start.data_ptr<int64_t>(), off,
+                            (size_t)seq_start.numel(), out.data_ptr<uint8_t>(), cur_stream(chunk)),
+          "bam_sequence");
+    return out;
+}
+
+std::tuple<Tensor, Tensor> bam_cigar(const Tensor &chunk, const Tensor &cigar_start, const Tensor &offsets,
+                                     int64_t total) {
+    need(chunk, torch::kUInt8, "chunk");
+    need(cigar_start, torch::kInt64, "cigar_start", chunk);
+    const int64_t *off = need_offsets(offsets, (size_t)cigar_start.numel(), chunk);
+    c10::cuda::CUDAGuard guard(chunk.device());
+    Tensor op = torch::empty({total}, chunk.options());
+    Tensor length = torch::empty({total}, cigar_start.options());
+    if (total == 0) return {op, length};
+    check(bnpk_bam_cigar(u8(chunk), (size_t)chunk.numel(), cigar_start.data_ptr<int64_t>(), off,
+                         (size_t)cigar_start.numel(), op.data_ptr<uint8_t>(), length.data_ptr<int64_t>(),
+                         cur_stream(chunk)),
+          "bam_cigar");
+    return {op, length};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bnpk, m) {
@@ -738,6 +797,10 @@ TORCH_LIBRARY(bnpk, m) {
           "-> (Tensor, Tensor, Tensor, Tensor, Tensor)");
     m.def("delimited_offsets(Tensor[] columns, int[] kinds) -> (Tensor, Tensor)");
     m.def("delimited_format(Tensor[] columns, int[] kinds, Tensor offsets, int out_begin, int out_end) -> Tensor");
+    m.def("bam_split(Tensor chunk, int n_ref, int segment_bytes=4096) -> (Tensor, Tensor)");
+    m.def("bam_fields(Tensor chunk, Tensor starts, Tensor(a!) status) -> Tensor");
+    m.def("bam_sequence(Tensor chunk, Tensor seq_start, Tensor offsets, int total) -> Tensor");
+    m.def("bam_cigar(Tensor chunk, Tensor cigar_start, Tensor offsets, int total) -> (Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
@@ -769,4 +832,8 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("runs_to_intervals", &runs_to_intervals);
     m.impl("delimited_offsets", &delimited_offsets);
     m.impl("delimited_format", &delimited_format);
+    m.impl("bam_split", &bam_split);
+    m.impl("bam_fields", &bam_fields);
+    m.impl("bam_sequence", &bam_sequence);
+    m.impl("bam_cigar", &bam_cigar);
 }

@@ -110,6 +110,13 @@ class SequenceEntryWithQuality(_Entries):
     _fields = ("name", "sequence", "quality")
 
 
+class BamEntry(_Entries):
+    """datatypes/__init__.py:173-183: an alignment.  chromosome and name are text, flag, position (0-based) and mapq
+    int64 CUDA tensors, cigar_op CigarOpEncoding codes and cigar_length int64 per row, sequence BamEncoding codes and
+    quality the stored phred values (uint8, 0xFF where the read has none)."""
+    _fields = ("chromosome", "name", "flag", "position", "mapq", "cigar_op", "cigar_length", "sequence", "quality")
+
+
 def _interval_field(field, value):
     """Interval, Bed6 and BedGraph fields: text columns (chromosome, name) as text, integer columns (start, stop, score)
     as int64 CUDA tensors, a bedGraph value as a CUDA tensor of its own dtype and strand as StrandEncoding codes."""

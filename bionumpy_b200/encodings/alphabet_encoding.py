@@ -101,3 +101,5 @@ ACUGEncoding = AlphabetEncoding("ACUG")
 RNAENcoding = ACUGEncoding
 AminoAcidEncoding = AlphabetEncoding('ACDEFGHIKLMNPQRSTVWY*')
 StrandEncoding = AlphabetEncoding("+-.")      # alphabet_encoding.py:120: '+' 0, '-' 1, '.' 2
+BamEncoding = AlphabetEncoding("=ACMGRSVTWYHKDBN")   # the 4-bit base codes of BAM (SAM spec 4.2.3)
+CigarOpEncoding = AlphabetEncoding("MIDNSHP=X")      # the cigar op codes of BAM (SAM spec 4.2.2)

@@ -9,3 +9,5 @@ from .multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
 from .indexed_fasta import IndexedFasta, read_index, create_index, open_indexed
 from .delimited import DelimitedBuffer, BedBuffer, Bed6Buffer, BdgBuffer
 from .motifs import read_motif
+from .bam import BamBuffer, BamIntervalBuffer
+from . import bam

@@ -50,6 +50,7 @@ class CudaOneLineBuffer:
     _check_plus = False
     dataclass = SequenceEntry
     _field_lines = (0, 1)          # field number -> line of the entry
+    _final_newline = True          # the reader ends the last chunk with '\n' (parser.py:183-186)
 
     def __init__(self, data, n_records, cr):
         self._data = data              # device bytes, complete entries only
@@ -79,18 +80,32 @@ class CudaOneLineBuffer:
         """OneLineBuffer.from_raw_buffer + _validate (io/one_line_buffer.py:44-71,155-173;
         io/fastq_buffer.py:38-45)."""
         assert header_data is None
-        chunk = _to_device_bytes(chunk)
+        buff = cls.read_device_chunk(_to_device_bytes(chunk), True, 0)
+        if buff is None:
+            raise IncompleteEntryException("No complete entry in buffer. Try increasing chunk_size.")
+        return buff
+
+    @classmethod
+    def read_device_chunk(cls, chunk, last, n_lines_before):
+        """The complete entries at the head of the device bytes ``chunk`` as a buffer, or None when it holds none; a
+        bad entry raises FormatException with its line number counted from ``n_lines_before``."""
         lpe = cls.n_lines_per_entry
         _, _, status = ops.line_split(chunk, lpe, 1, 0, ord(cls.HEADER), cls._check_plus, -1, max_rows=0)
         st = ops.read_status(status)
         if st.n_lines < lpe:
-            raise IncompleteEntryException("No complete entry in buffer. Try increasing chunk_size.")
+            return None
         if st.bad_header_entry is not None:
             raise FormatException(f"Expected header line to start with {cls.HEADER}",
-                                  line_number=st.bad_header_entry * lpe)
+                                  line_number=st.bad_header_entry * lpe + n_lines_before)
         if st.bad_plus_entry is not None:
-            raise FormatException("Expected '+' at third line of entry", line_number=2 + st.bad_plus_entry * lpe)
+            raise FormatException("Expected '+' at third line of entry",
+                                  line_number=2 + st.bad_plus_entry * lpe + n_lines_before)
         return cls(chunk[: st.n_complete_bytes], st.n_records, st.cr)
+
+    @classmethod
+    def concatenate(cls, buffers):
+        """One buffer of the entries of consecutive chunks."""
+        return cls(torch.cat([b._data for b in buffers]), sum(b._n_records for b in buffers), buffers[0]._cr)
 
     @property
     def size(self) -> int:

@@ -31,8 +31,11 @@ def _buffer_type_for(suffix):
     if suffix == ".bdg":
         from .delimited import BdgBuffer
         return BdgBuffer
+    if suffix == ".bam":
+        from .bam import BamBuffer
+        return BamBuffer
     raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
-                       f"(supported: .fq .fastq .fa .fasta .bed .bdg and their .gz forms); pass buffer_type=")
+                       f"(supported: .fq .fastq .fa .fasta .bed .bdg and their .gz forms, and .bam); pass buffer_type=")
 
 
 def _suffix(path):
@@ -46,13 +49,16 @@ def _suffix(path):
 def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
     """files.py:85-182.  Reading ("r", "rb") gives an NpDataclassReader; writing ("w", "wb", "write") or appending
     ("a", "ab", "append") gives an NpBufferedWriter, which writes ``.gz`` files as BGZF.  ``.bdg`` (bedGraph) is
-    written only.  BED is written with the buffer type named: ``bnp.open("x.bed", "w", buffer_type=BedBuffer)`` (or
+    written only, ``.bam`` read only (as BGZF, whatever the suffix says).  BED is written with the buffer type named: ``bnp.open("x.bed", "w", buffer_type=BedBuffer)`` (or
     Bed6Buffer; either writes a record's own fields).  Opening ``.bed`` for writing by its suffix alone raises
     NotImplementedError, as it did before BED could be written, so code that relies on that keeps working."""
     if mode not in (None, "r", "rb") and mode not in WRITE_MODES:
         raise NotImplementedError(f"mode {mode!r}: use r/rb to read, w/wb/write or a/ab/append to write")
     path = str(filename)
     suffix, is_gzip = _suffix(path)
+    if mode in WRITE_MODES and buffer_type is None and suffix == ".bam":      # BAM is read only
+        raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
+                           f"(supported: .fq .fastq .fa .fasta .bed .bdg and their .gz forms); pass buffer_type=")
     if mode in WRITE_MODES and buffer_type is None and suffix == ".bed":
         raise NotImplementedError("writing .bed by its suffix alone is not supported: name the format with "
                                   "buffer_type=bnp.io.BedBuffer (or Bed6Buffer)")

@@ -207,7 +207,8 @@ class _GzipSource(_Source):
 
 
 class PinnedFileReader(CudaFileReader):
-    """The chunk reader over a _Source (plain file or inflated gzip) for the one-line buffer types."""
+    """The chunk reader over a _Source (plain file or inflated gzip) for the one-line buffer types and BAM.  The buffer
+    type finds the complete entries of each chunk (``read_device_chunk``) and joins chunks (``concatenate``)."""
 
     def __init__(self, file_obj, buffer_type, source):
         super().__init__(file_obj, buffer_type)
@@ -215,6 +216,13 @@ class PinnedFileReader(CudaFileReader):
         self._pending = None
         self._tail = None                              # device bytes that belong to the next chunk
         self._tail_last = NEWLINE                      # the tail's last byte, known on the host
+        self._exhausted = False                        # the header read the whole stream
+        if hasattr(buffer_type, "header"):             # BAM: the header lies inside the inflated stream
+            from .bam import read_stream_header
+            self._header_data, rest, self._exhausted = read_stream_header(source)
+            self._buffer_type = buffer_type.modify_class_with_header_data(self._header_data)
+            if rest:
+                self._tail = torch.frombuffer(bytearray(rest), dtype=torch.uint8).to(config.default_device())
 
     def close(self):
         self._source.close()
@@ -231,28 +239,29 @@ class PinnedFileReader(CudaFileReader):
             return None
         if len(chunks) == 1:
             return chunks[0]
-        data = torch.cat([c._data for c in chunks])
-        return self._buffer_type(data, sum(c._n_records for c in chunks), chunks[0]._cr)
+        return self._buffer_type.concatenate(chunks)
 
     def read_chunk(self, min_chunk_size: int = 5000000, max_chunk_size: int = None):
         if self._is_finished:
             return None
         bt = self._buffer_type
-        lpe = bt.n_lines_per_entry
         dev = config.default_device()
         while True:
-            handle = self._pending if self._pending is not None else self._source.start(min_chunk_size)
-            self._pending = None
-            pinned, nread, last = self._source.finish(handle)
-            if not last:
-                self._pending = self._source.start(min_chunk_size)      # the next chunk fills while the GPU works
+            if self._exhausted:
+                pinned, nread, last = None, 0, True
+            else:
+                handle = self._pending if self._pending is not None else self._source.start(min_chunk_size)
+                self._pending = None
+                pinned, nread, last = self._source.finish(handle)
+                if not last:
+                    self._pending = self._source.start(min_chunk_size)  # the next chunk fills while the GPU works
             tail_len = 0 if self._tail is None else self._tail.numel()
             total = tail_len + nread
             if total == 0:
                 self._is_finished = True
                 return None
             last_byte = int(pinned[nread - 1]) if nread else self._tail_last
-            add_nl = last and last_byte != NEWLINE                       # parser.py:183-186
+            add_nl = last and last_byte != NEWLINE and bt._final_newline   # parser.py:183-186
             d = torch.empty(total + (1 if add_nl else 0), dtype=torch.uint8, device=dev)
             if tail_len:
                 d[:tail_len] = self._tail
@@ -263,22 +272,14 @@ class PinnedFileReader(CudaFileReader):
                 last_byte = NEWLINE
             if max_chunk_size is not None and d.numel() > max_chunk_size:
                 raise Exception("No complete entry found")
-            _, _, status = ops.line_split(d, lpe, 1, 0, ord(bt.HEADER), bt._check_plus, -1, max_rows=0)
-            st = ops.read_status(status)                                 # the one synchronisation of this chunk
-            if st.n_lines < lpe:
+            buff = bt.read_device_chunk(d, last, self.n_lines_read)      # the one synchronisation of this chunk
+            if buff is None:
                 if last:
                     self._is_finished = True
                     return None
                 self._tail, self._tail_last = d, last_byte               # no complete entry yet: read more
                 continue
-            if st.bad_header_entry is not None:
-                raise FormatException(f"Expected header line to start with {bt.HEADER}",
-                                      line_number=st.bad_header_entry * lpe + self.n_lines_read)
-            if st.bad_plus_entry is not None:
-                raise FormatException("Expected '+' at third line of entry",
-                                      line_number=2 + st.bad_plus_entry * lpe + self.n_lines_read)
-            size = st.n_complete_bytes
-            buff = bt(d[:size], st.n_records, st.cr)
+            size = buff.size
             self._tail = None if last or size == d.numel() else d[size:].clone()
             self._tail_last = last_byte
             self._is_finished = last
@@ -288,8 +289,16 @@ class PinnedFileReader(CudaFileReader):
 
 
 def open_reader(path, file_obj, buffer_type, is_gzip):
-    """The ingest reader for `path` if the buffer type is one of the one-line CUDA buffers, else None."""
+    """The ingest reader for `path` if the buffer type is one of the one-line CUDA buffers or BAM, else None.  BAM is
+    always read as BGZF (or gzip)."""
+    from .bam import BamBuffer
     from .buffers import CudaOneLineBuffer
+    if isinstance(buffer_type, type) and issubclass(buffer_type, BamBuffer):
+        if file_obj.read(2) != b"\x1f\x8b":
+            file_obj.close()
+            raise FormatException(f"{path} is not a BAM file: BAM is BGZF-compressed, and this file is not gzip")
+        file_obj.seek(0)
+        return PinnedFileReader(file_obj, buffer_type, _GzipSource(path))
     if not (isinstance(buffer_type, type) and issubclass(buffer_type, CudaOneLineBuffer)):
         return None
     if is_gzip:

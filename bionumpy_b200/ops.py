@@ -842,3 +842,64 @@ def delimited_format(columns, offsets, out_begin=0, out_end=None, out=None):
     check(lib().bnpk_delimited_format(ctypes.cast(arr, ctypes.c_void_p), len(columns), n, offsets_p, out_begin,
                                       out_end, _pointer(out), stream_ptr()))
     return out
+
+
+BAM_SEGMENT_BYTES = 4096        # the bytes one warp of the BAM split speculates on (DESIGN §3 K15)
+BAM_MIN_RECORD = 36             # block_size word + the 32 fixed bytes
+
+
+@_on_device
+def bam_split(chunk, n_ref, segment_bytes=BAM_SEGMENT_BYTES, status=None):
+    """bnpk_bam_split: (starts int64[n // 36 + 1], status).  The first status[ST_N_RECORDS] starts are the chunk's
+    complete records; status[ST_N_COMPLETE_BYTES] is their size, status[ST_BAD_BASE] the first fault as
+    (record << 8 | nv.BAM_BAD_*) and status[ST_N_VALUES] the number of segments walked again."""
+    chunk_p = _pointer(chunk, "chunk", torch.uint8)
+    _status(status)
+    if segment_bytes < 64:
+        raise ValueError("segment_bytes must be at least 64")
+    n, dev = chunk.numel(), chunk.device
+    starts = torch.empty(n // BAM_MIN_RECORD + 1, dtype=torch.int64, device=dev)
+    status = nv.new_status(dev) if status is None else status
+    ws = torch.empty(7 * max(-(-n // segment_bytes), 1), dtype=torch.int64, device=dev)
+    check(lib().bnpk_bam_split(chunk_p, n, n_ref, segment_bytes, _pointer(starts), starts.numel(), _pointer(status),
+                               _pointer(ws), ws.numel(), stream_ptr()))
+    return starts, status
+
+
+@_on_device
+def bam_fields(chunk, starts, status):
+    """bnpk_bam_fields: int64[BAM_FIELDS, R] (R = starts.numel()); column r < status[ST_N_RECORDS] holds record r's
+    fields (nv.BAM_F_*).  A cigar op code above 8 is reported in status[ST_BAD_BASE]."""
+    chunk_p, starts_p = _pointer(chunk, "chunk", torch.uint8), _pointer(starts, "starts", torch.int64)
+    status_p = _status(status, optional=False)
+    fields = torch.empty(nv.BAM_FIELDS, starts.numel(), dtype=torch.int64, device=chunk.device)
+    check(lib().bnpk_bam_fields(chunk_p, chunk.numel(), starts_p, starts.numel(), _pointer(fields), status_p,
+                                stream_ptr()))
+    return fields
+
+
+@_on_device
+def bam_sequence(chunk, seq_start, offsets, total):
+    """bnpk_bam_sequence: uint8[total], the 4-bit base codes of the rows at offsets[r] .. offsets[r + 1]."""
+    chunk_p, start_p = _pointer(chunk, "chunk", torch.uint8), _pointer(seq_start, "seq_start", torch.int64)
+    offsets_p = _pointer(offsets, "offsets", torch.int64, n=seq_start.numel() + 1)
+    out = torch.empty(total, dtype=torch.uint8, device=chunk.device)
+    if total == 0:
+        return out
+    check(lib().bnpk_bam_sequence(chunk_p, chunk.numel(), start_p, offsets_p, seq_start.numel(), _pointer(out),
+                                  stream_ptr()))
+    return out
+
+
+@_on_device
+def bam_cigar(chunk, cigar_start, offsets, total):
+    """bnpk_bam_cigar: (op uint8[total], length int64[total]) of the rows' cigar words at offsets[r] .. offsets[r + 1]."""
+    chunk_p, start_p = _pointer(chunk, "chunk", torch.uint8), _pointer(cigar_start, "cigar_start", torch.int64)
+    offsets_p = _pointer(offsets, "offsets", torch.int64, n=cigar_start.numel() + 1)
+    op = torch.empty(total, dtype=torch.uint8, device=chunk.device)
+    length = torch.empty(total, dtype=torch.int64, device=chunk.device)
+    if total == 0:
+        return op, length
+    check(lib().bnpk_bam_cigar(chunk_p, chunk.numel(), start_p, offsets_p, cigar_start.numel(), _pointer(op),
+                               _pointer(length), stream_ptr()))
+    return op, length

@@ -554,6 +554,59 @@ int bnpk_delimited_format(const bnpk_out_column *columns, int n_columns, size_t 
                           int64_t out_begin, int64_t out_end, uint8_t *out, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K15  BAM records (BamBuffer._find_starts / BamBufferExtractor, io/bam.py:18-331; split_cigar /
+ * count_reference_length, alignments/cigar.py:8-24).  `chunk` holds inflated BAM bytes that start at a record.
+ *
+ *   bnpk_bam_split: the byte offset of every complete record of the chunk, in order, into starts int64[R]
+ *     (max_starts >= n / 36: a complete record is at least 36 bytes).  A speculative segmented walk: the chunk is cut
+ *     into segments of segment_bytes; a warp per segment finds the first offset whose record header (and the next
+ *     few records of its chain) passes the header check and walks from there to the segment's end; one warp then
+ *     confirms the segments in order from offset 0, walking again every segment whose speculative start is not the
+ *     confirmed exit of the segment before.  The result is exact whatever the speculation found.  The header check:
+ *     block_size >= 32, -1 <= refID, next_refID < n_ref, l_read_name >= 1 and the name ends in NUL, and
+ *     32 + l_read_name + 4 n_cigar_op + (l_seq + 1) / 2 + l_seq <= block_size with l_seq >= 0.
+ *     status (pre-initialised): [BNPK_ST_N_RECORDS] = R, [BNPK_ST_N_COMPLETE_BYTES] = the bytes of those records (the
+ *     rest begins the next chunk's first record), [BNPK_ST_BAD_BASE] = (R << 8 | BNPK_BAM_BAD_*) when the walk
+ *     stopped at a record that fails the check, [BNPK_ST_N_VALUES] = the segments walked again.  workspace int64[7 *
+ *     ceil(n / segment_bytes)]; three kernels, no synchronisation.
+ *   bnpk_bam_fields: one thread per record r < min(max_records, status[BNPK_ST_N_RECORDS]) writes
+ *     fields[f * max_records + r] for the BNPK_BAM_F_* below, and atomicMin-s (r << 8 | BNPK_BAM_BAD_CIGAR_OP) into
+ *     status[BNPK_ST_BAD_BASE] for a cigar op code above 8.  The records are those bnpk_bam_split found.
+ *   bnpk_bam_sequence: the l_seq 4-bit codes of every row, high nibble first, one byte each, at out[offsets[r] ..
+ *     offsets[r + 1]) (offsets = bnpk_row_offsets of l_seq); 16 output bytes per thread.
+ *   bnpk_bam_cigar: the n_cigar_op cigar words of every row as op = word & 15 (uint8) and length = word >> 4 (int64)
+ *     at offsets[r] .. offsets[r + 1]; 4 ops per thread.
+ * ------------------------------------------------------------------------------------- */
+#define BNPK_BAM_BAD_BLOCK_SIZE 1  /* block_size < 32                                             */
+#define BNPK_BAM_BAD_REF_ID     2  /* refID or next_refID outside -1 .. n_ref - 1                 */
+#define BNPK_BAM_BAD_NAME       3  /* l_read_name 0, or the name does not end in NUL              */
+#define BNPK_BAM_BAD_SIZES      4  /* l_seq < 0, or the fields do not fit block_size              */
+#define BNPK_BAM_BAD_CIGAR_OP   5  /* a cigar op code above 8 (MIDNSHP=X)                         */
+#define BNPK_BAM_TRUNCATED      6  /* the file ends inside a record (reported by the reader)      */
+#define BNPK_BAM_F_REF_ID     0
+#define BNPK_BAM_F_POS        1
+#define BNPK_BAM_F_MAPQ       2
+#define BNPK_BAM_F_FLAG       3
+#define BNPK_BAM_F_NAME_START 4    /* the name without its NUL: l_read_name - 1 bytes             */
+#define BNPK_BAM_F_NAME_LEN   5
+#define BNPK_BAM_F_CIGAR_START 6
+#define BNPK_BAM_F_N_CIGAR    7
+#define BNPK_BAM_F_SEQ_START  8
+#define BNPK_BAM_F_L_SEQ      9
+#define BNPK_BAM_F_QUAL_START 10   /* l_seq bytes                                                 */
+#define BNPK_BAM_F_REF_LEN    11   /* the summed lengths of the M, D, N, = and X ops              */
+#define BNPK_BAM_FIELDS       12
+
+int bnpk_bam_split(const uint8_t *chunk, size_t n, int n_ref, size_t segment_bytes, int64_t *starts, size_t max_starts,
+                   int64_t *status, int64_t *workspace, size_t workspace_words, void *stream);
+int bnpk_bam_fields(const uint8_t *chunk, size_t n, const int64_t *starts, size_t max_records, int64_t *fields,
+                    int64_t *status, void *stream);
+int bnpk_bam_sequence(const uint8_t *chunk, size_t n, const int64_t *seq_start, const int64_t *offsets, size_t n_rows,
+                      uint8_t *out, void *stream);
+int bnpk_bam_cigar(const uint8_t *chunk, size_t n, const int64_t *cigar_start, const int64_t *offsets, size_t n_rows,
+                   uint8_t *op, int64_t *length, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Host-buffer entry point (end-to-end): the call a reader loop makes with a chunk that is
  * still in host memory.  Copies `chunk_host` (pinned or pageable) to the device in slices on
  * a private copy stream, overlapping each slice's H2D with the fused count of the previous
