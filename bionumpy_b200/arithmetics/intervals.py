@@ -47,8 +47,8 @@ def coverage_runs(start, stop, size, mode):
     keys, _, _, status = ops.interval_events(start, stop, size=size)
     keys = torch.sort(keys).values
     starts, values, n_runs = ops.pileup_runs(keys, size, mode)
-    n, bad = torch.cat([n_runs, status[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]).cpu().tolist()
-    return starts[:n + 1], values[:n], None if bad == nv.INT64_MAX else bad
+    n, st = ops.read_back(n_runs, status)
+    return starts[:n + 1], values[:n], st.fault
 
 
 def _raise_bad(bad, start, stop, size):
@@ -104,8 +104,8 @@ def merge_intervals(intervals, distance: int = 0):
     elif chrom is not None:
         raise TypeError(f"merge_intervals: chromosome names must be text, not {type(chrom).__name__}")
     first, stops, n_out, status = ops.interval_merge(start, stop, same, distance)
-    k, bad = torch.cat([n_out, status[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]).cpu().tolist()
-    if bad != nv.INT64_MAX:
+    k, st = ops.read_back(n_out, status)
+    if st.fault is not None:
         raise AssertionError("merge_intervals requires intervals sorted on start position")
     return replace(intervals[first[:k]], stop=stops[:k])
 

@@ -172,7 +172,7 @@ __global__ void __launch_bounds__(32) bam_resolve_kernel(const __grid_constant__
         a.status[BNPK_ST_N_RECORDS] = total;
         a.status[BNPK_ST_N_COMPLETE_BYTES] = cur;
         a.status[BNPK_ST_N_VALUES] = redo;
-        if (state > 0) a.status[BNPK_ST_BAD_BASE] = total << 8 | state;
+        if (state > 0) a.status[BNPK_ST_BAD_BASE] = fault_record(total, state);
     }
 }
 
@@ -204,7 +204,7 @@ __global__ void __launch_bounds__(256) bam_fields_kernel(const uint8_t *c, const
             // M (0), D (2), N (3), = (7) and X (8) consume the reference
             if ((0x18du >> op) & 1) ref_len += w >> 4;
         }
-        if (bad_op) atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)(r << 8 | BNPK_BAM_BAD_CIGAR_OP));
+        if (bad_op) report_fault(status, fault_record(r, BNPK_BAM_BAD_CIGAR_OP));
         f[BNPK_BAM_F_REF_ID * max_records + r] = (int32_t)ld_u32(c + p + 4);
         f[BNPK_BAM_F_POS * max_records + r] = (int32_t)ld_u32(c + p + 8);
         f[BNPK_BAM_F_MAPQ * max_records + r] = __ldg(c + p + 13);

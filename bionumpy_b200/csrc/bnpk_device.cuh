@@ -74,6 +74,19 @@ __device__ __forceinline__ void load16(const uint8_t *p, uint32_t (&o)[4]) {
     for (int j = 0; j < 4; ++j) o[j] = __funnelshift_r(t[j], t[j + 1], sh);
 }
 
+// Faults: the first fault of a launch is the smallest word reported into status[BNPK_ST_BAD_BASE], packed in one of
+// the layouts bnpk.h names (ops.ScanStatus decodes them); a plain index needs no packer.  Reporting INT64_MAX ("no
+// fault") leaves the word as it is; a caller that usually has no fault tests for it first and skips the atomic.
+__device__ __forceinline__ void report_fault(int64_t *status, int64_t v) {
+    atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)v);
+}
+__device__ __forceinline__ int64_t fault_row_pos(int64_t row, int64_t pos) { return row << 32 | pos; }
+// column < 32: a line with more columns reports 31
+__device__ __forceinline__ int64_t fault_column(int64_t line, int column, int kind) {
+    return line << 8 | (int64_t)column << 3 | kind;
+}
+__device__ __forceinline__ int64_t fault_record(int64_t record, int kind) { return record << 8 | kind; }
+
 __device__ __forceinline__ uint64_t warp_sum_u64(uint64_t v) {
 #pragma unroll
     for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -328,8 +341,8 @@ __device__ __forceinline__ uint32_t encode_unit(const uint4 q, uint32_t seq16, c
 }
 
 // The same alphabets one byte at a time, for the rare rescan of a row some encode_unit flagged: the first byte of
-// bytes[p0, p1) outside the alphabet, as (entry << 32 | offset from the row's first byte b0) for the BAD_BASE status
-// word (a minimum); INT64_MAX if there is none.
+// bytes[p0, p1) outside the alphabet, as fault_row_pos(entry, offset from the row's first byte b0); INT64_MAX if there
+// is none.
 template <int ENC>
 __device__ __forceinline__ long long first_bad_base(const uint8_t *bytes, int p0, int p1, int b0, int64_t entry, const uint8_t *s_lut) {
     for (int p = p0; p < p1; ++p) {
@@ -338,7 +351,7 @@ __device__ __forceinline__ long long first_bad_base(const uint8_t *bytes, int p0
         if (ENC == BNPK_ENC_CODES) okb = c < 4;
         else if (ENC == BNPK_ENC_LUT) okb = s_lut[c] < 4;
         else { const uint32_t uu = c | 0x20u; okb = (uu == 'a' || uu == 'c' || uu == 'g' || uu == 't'); }
-        if (!okb) return (long long)((entry << 32) | (int64_t)(p - b0));
+        if (!okb) return (long long)fault_row_pos(entry, p - b0);
     }
     return INT64_MAX;
 }

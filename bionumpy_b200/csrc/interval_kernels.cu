@@ -34,14 +34,6 @@ struct ColArgs {
     int64_t *status;
 };
 
-__device__ __forceinline__ void report(int64_t *status, int64_t v) {
-    atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)v);
-}
-
-__device__ __forceinline__ int64_t col_fault(int64_t line, int col, int kind) {
-    return (line << 8) | ((int64_t)min(col, 31) << 3) | kind;
-}
-
 __global__ void __launch_bounds__(kColThreads) delimited_columns_kernel(const __grid_constant__ ColArgs a) {
     __shared__ uint4 s_stage[kColStage / 16];
     __shared__ int s_kind[BNPK_MAX_COLUMNS];
@@ -120,12 +112,12 @@ __global__ void __launch_bounds__(kColThreads) delimited_columns_kernel(const __
                 s_lens[col][line] = flen;
             } else if (kind == BNPK_COL_INT || kind == BNPK_COL_INT_OR_DOT) {
                 const bool dot = kind == BNPK_COL_INT_OR_DOT && flen == 1 && p[f0] == '.';
-                if (!dot && (bad || nd == 0 || nd > 18)) fault = min(fault, col_fault(line, col, BNPK_BAD_INT));
+                if (!dot && (bad || nd == 0 || nd > 18)) fault = min(fault, fault_column(line, min(col, 31), BNPK_BAD_INT));
                 reinterpret_cast<int64_t *>(s_out[col])[line] = dot ? 0 : neg ? -val : val;
             } else if (kind == BNPK_COL_STRAND) {
                 const uint8_t b = flen == 1 ? p[f0] : 0;
                 const int code = b == '+' ? 0 : b == '-' ? 1 : b == '.' ? 2 : -1;
-                if (code < 0) fault = min(fault, col_fault(line, col, BNPK_BAD_STRAND));
+                if (code < 0) fault = min(fault, fault_column(line, min(col, 31), BNPK_BAD_STRAND));
                 reinterpret_cast<uint8_t *>(s_out[col])[line] = (uint8_t)max(code, 0);
             }
             ++col;
@@ -135,9 +127,9 @@ __global__ void __launch_bounds__(kColThreads) delimited_columns_kernel(const __
             neg = bad = false;
         }
         // a line with another tab count is reported as that, before whatever its fields held
-        if (col - 1 != first_tabs) fault = col_fault(line, col, BNPK_BAD_TABS);
-        else if (col < a.n_columns) fault = col_fault(line, col, BNPK_BAD_COLUMNS);
-        if (fault != INT64_MAX) report(a.status, fault);
+        if (col - 1 != first_tabs) fault = fault_column(line, min(col, 31), BNPK_BAD_TABS);
+        else if (col < a.n_columns) fault = fault_column(line, min(col, 31), BNPK_BAD_COLUMNS);
+        if (fault != INT64_MAX) report_fault(a.status, fault);
     }
 }
 
@@ -173,7 +165,7 @@ __global__ void __launch_bounds__(256) name_lookup_kernel(const uint8_t *base, s
             }
         }
         out_ids[r] = id;
-        if (id < 0) report(status, (int64_t)r);
+        if (id < 0) report_fault(status, (int64_t)r);
     }
 }
 
@@ -224,7 +216,7 @@ __global__ void __launch_bounds__(256) interval_check_kernel(const __grid_consta
         bool ok = contig_of(a, r, c) && s >= 0 && e >= s && e <= c.len && e - s <= INT32_MAX;
         if (ok && e > s) ok = c.offset >= 0 && (uint64_t)file_pos(c, e - 1) < a.file_bytes;
         a.row_lens[r] = ok ? (int32_t)(e - s) : 0;
-        if (!ok) report(a.status, r);
+        if (!ok) report_fault(a.status, r);
     }
 }
 

@@ -125,7 +125,7 @@ __global__ void __launch_bounds__(512) bincount_kernel(const int64_t *values, si
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
         const int64_t v = values[i];
         if (v < 0) {
-            atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)i);
+            report_fault(status, (int64_t)i);
             continue;
         }
         const uint64_t b = mask ? ((uint64_t)v & mask) : ((uint64_t)v % n_bins);
@@ -151,7 +151,7 @@ __global__ void __launch_bounds__(256) bincount_rows_kernel(const int64_t *value
         const int64_t b = offsets[r], e = offsets[r + 1];
         for (int64_t i = b + lane; i < e; i += 32) {
             const int64_t v = values[i];
-            if (v < 0) { atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)i); continue; }
+            if (v < 0) { report_fault(status, i); continue; }
             atomicAdd(out + r * n_bins + ((uint64_t)v % n_bins), 1ull);
         }
     }

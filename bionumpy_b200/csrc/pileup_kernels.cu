@@ -34,10 +34,6 @@ constexpr uint64_t kBias = 1ull << 59;          // merge: stop + kBias in [0, 2^
 constexpr uint64_t kReset = 1ull << 61;         // merge: "a segment starts here" in the scanned word
 constexpr int64_t kMaxPos = (int64_t)1 << 59;   // positions are in [0, 2^59)
 
-__device__ __forceinline__ void report(int64_t *status, int64_t v) {
-    atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)v);
-}
-
 // the value of a 62-bit look-back word as a signed number
 __device__ __forceinline__ int64_t signed62(uint64_t v) { return (int64_t)(v << 2) >> 2; }
 
@@ -94,7 +90,7 @@ __global__ void __launch_bounds__(256) interval_events_kernel(const __grid_const
         }
         if (a.g_start) a.g_start[r] = live ? off + s : 0;
         if (a.g_stop) a.g_stop[r] = live ? off + e : 0;
-        if (!ok) report(a.status, r);
+        if (!ok) report_fault(a.status, r);
     }
 }
 
@@ -365,7 +361,7 @@ __global__ void __launch_bounds__(kScanThreads) interval_merge_kernel(const __gr
             if (i >= a.n) break;
             const int64_t before = (int64_t)(run & ~kReset) - (int64_t)kBias;
             if (seg[j] || st[j] > before + d) first |= 1u << j;
-            if (!seg[j] && st[j] < (j ? st[j - 1] : prev_start)) report(a.status, i);
+            if (!seg[j] && st[j] < (j ? st[j - 1] : prev_start)) report_fault(a.status, i);
             run = SegMax::combine(run, (seg[j] ? kReset : 0) | (uint64_t)(sp[j] + (int64_t)kBias));
             incl[j] = (int64_t)(run & ~kReset) - (int64_t)kBias;
         }

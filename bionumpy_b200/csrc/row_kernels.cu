@@ -190,7 +190,7 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_bad, c
             if (bad >= 0) {
                 reported = true;
                 if (lane == 0)
-                    atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE], (long long)((r << 32) | (seg_start + bad - off)));
+                    report_fault(a.status, fault_row_pos(r, seg_start + bad - off));
             }
         }
         if constexpr (RM == RM_ENCODE) {
@@ -209,7 +209,7 @@ __device__ void warp_row(const RowArgs &a, uint32_t *w_codes, uint32_t *w_bad, c
                 if (first_bad != INT_MAX && !reported) {
                     reported = true;
                     if (lane == 0)
-                        atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE], (long long)((r << 32) | (seg_start + first_bad)));
+                        report_fault(a.status, fault_row_pos(r, seg_start + first_bad));
                 }
             } else {
                 for (int p = lane; p < seg_len; p += 32) {
@@ -489,7 +489,7 @@ __global__ void __launch_bounds__(256) rows_generic_hash_kernel(const uint8_t *b
         const int64_t start = starts[r], L = lens[r], o = offsets[r];
         for (int64_t i = lane; i < L; i += 32) {                    // validity of every symbol of the row
             const uint8_t c = s_lut[base[start + i]];
-            if (c >= alphabet_size) atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)(((int64_t)r << 32) | i));
+            if (c >= alphabet_size) report_fault(status, fault_row_pos(r, i));
         }
         for (int64_t i = lane; i + k <= L; i += 32) {
             unsigned long long h = 0;
@@ -529,7 +529,7 @@ __global__ void __launch_bounds__(256) rows_pwm_generic_kernel(const uint8_t *ba
 #pragma unroll
             for (int o = 16; o; o >>= 1) first_bad = min(first_bad, __shfl_xor_sync(0xffffffffu, first_bad, o));
             if (lane == 0 && first_bad != INT64_MAX)
-                atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)(((int64_t)r << 32) | first_bad));
+                report_fault(status, fault_row_pos(r, first_bad));
             const int64_t npos = tail ? L : L - m + 1;
             double *o_row = SCORES ? out + offsets[r] : nullptr;
             for (int64_t i = lane; i < npos; i += 32) {
@@ -600,7 +600,7 @@ __global__ void __launch_bounds__(256) rows_match_generic_kernel(const uint8_t *
 #pragma unroll
                 for (int o = 16; o; o >>= 1) first_bad = min(first_bad, __shfl_xor_sync(0xffffffffu, first_bad, o));
                 if (lane == 0 && first_bad != INT64_MAX)
-                    atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)(((int64_t)r << 32) | first_bad));
+                    report_fault(status, fault_row_pos(r, first_bad));
             }
             const int64_t npos = m.same ? L : L - m.span + 1;
             uint8_t *o_row = OUT ? reinterpret_cast<uint8_t *>(out) + offsets[r] : nullptr;

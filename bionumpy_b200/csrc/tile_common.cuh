@@ -35,8 +35,8 @@ struct TileArgs {
 template <int ENC>
 __device__ __forceinline__ void report_bad_base(const TileArgs &a, const uint8_t *bytes, int p0, int p1, int b0, int64_t entry,
                                                 const uint8_t *s_lut) {
-    const long long v = first_bad_base<ENC>(bytes, p0, p1, b0, entry, s_lut);
-    if (v != INT64_MAX) atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE], v);
+    const int64_t v = first_bad_base<ENC>(bytes, p0, p1, b0, entry, s_lut);
+    if (v != INT64_MAX) report_fault(a.status, v);
 }
 
 // A row the kernel cannot finish (no newline inside the staged bytes, or too long for its row walk): (first byte, entry)

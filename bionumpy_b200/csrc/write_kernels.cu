@@ -144,11 +144,6 @@ __device__ __forceinline__ Src whole_unit(const FmtArgs &a, const Entry &E, int6
     return {-1, 0, 0};
 }
 
-// bad bytes are the error path: each one goes straight to the status word
-__device__ __forceinline__ void report_bad(int64_t *status, int64_t v) {
-    atomicMin((long long *)&status[BNPK_ST_BAD_BASE], (long long)v);
-}
-
 template <bool CHECK>
 __global__ void __launch_bounds__(kFmtThreads) format_kernel(const __grid_constant__ FmtArgs a) {
     __shared__ uint8_t s_lut[3][256];
@@ -200,7 +195,7 @@ __global__ void __launch_bounds__(kFmtThreads) format_kernel(const __grid_consta
 #pragma unroll
                             for (int b = 0; b < 4; ++b) {
                                 const uint8_t c = s_lut[f][(w[i] >> (8 * b)) & 255];
-                                if (CHECK && c == 0) report_bad(a.status, (E.e << 32) | (whole.idx + 4 * i + b));
+                                if (CHECK && c == 0) report_fault(a.status, fault_row_pos(E.e, whole.idx + 4 * i + b));
                                 r |= (uint32_t)c << (8 * b);
                             }
                             w[i] = r;
@@ -220,7 +215,7 @@ __global__ void __launch_bounds__(kFmtThreads) format_kernel(const __grid_consta
                             const int64_t src = E.start(s.field) + s.idx;
                             const uint8_t raw = (src >= 0 && (uint64_t)src < a.base_bytes[s.field]) ? a.base[s.field][src] : 0;
                             c = s_lut[s.field][raw];
-                            if (CHECK && s.field == 1 && a.lut[1] && c == 0) report_bad(a.status, (E.e << 32) | s.idx);
+                            if (CHECK && s.field == 1 && a.lut[1] && c == 0) report_fault(a.status, fault_row_pos(E.e, s.idx));
                         }
                         w[i >> 2] |= (uint32_t)c << (8 * (i & 3));
                     }
@@ -317,7 +312,7 @@ __global__ void __launch_bounds__(kScanThreads) delimited_offsets_kernel(const _
             const DelimColumn &c = a.col[k];
             size += field_width(c, e);
             if (c.kind == BNPK_COL_STRAND && c.data[e] > 2)
-                atomicMin((long long *)&a.status[BNPK_ST_BAD_BASE], (long long)(e << 8 | k << 3 | BNPK_BAD_STRAND));
+                report_fault(a.status, fault_column(e, k, BNPK_BAD_STRAND));
         }
         return (uint64_t)size;
     });

@@ -91,8 +91,7 @@ def concatenate(a, b, extra=()):
             fields[f] = torch.cat([x, y])
         else:
             raise TypeError(f"cannot concatenate the {f} fields ({type(x).__name__}, {type(y).__name__})")
-    values = torch.cat([w.to(torch.int64).reshape(1) for w in words + list(extra)]).cpu().tolist() if words or extra \
-        else []
+    values = ops.read_back(*words, *extra)
     for i, (f, parts) in enumerate(texts.items()):
         flat = [ops.interval_copy(rows.base, rows.starts, rows.starts + rows.lens.to(torch.int64), offsets, total)
                 for (rows, offsets), total in zip(parts, values[2 * i:2 * i + 2])]

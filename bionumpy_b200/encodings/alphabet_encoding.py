@@ -41,9 +41,8 @@ class AlphabetEncoding(OneToOneEncoding):
             self._dev_luts[key] = torch.from_numpy(self._lookup.copy()).to(device)
         return self._dev_luts[key]
 
-    def _raise_encoding_error(self, row, pos, lens, sample_bytes=None):
+    def _raise_encoding_error(self, offset):
         """alphabet_encoding.py:37-46: offset = first invalid index of the flattened array."""
-        offset = int(lens[:row].to(torch.int64).sum().item()) + pos if row else pos
         raise EncodingError(f"Error when encoding to {self.__class__.__name__}({''.join(self._raw_alphabet)}). "
                             f"Invalid character at flat offset {offset}", offset)
 

@@ -173,12 +173,11 @@ class GenomicIntervals:
         ids, st_names = ops.name_lookup(rows.base, rows.starts, rows.lens, text, name_offsets)
         _, g_start, g_stop, st_rows = ops.interval_events(start, stop, ids, offset, size, keys=False, glob=True)
         keep = offset[ids.clamp(min=0).to(torch.int64)] >= 0
-        unknown, bad, n_keep = torch.cat([st_names[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1],
-                                          st_rows[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1],
-                                          keep.sum().reshape(1)]).cpu().tolist()
-        if unknown != nv.INT64_MAX:
-            raise KeyError(record.chromosome[unknown].to_string())
-        if bad != nv.INT64_MAX:
+        st_names, st_rows, n_keep = ops.read_back(st_names, st_rows, keep.sum())
+        if st_names.fault is not None:
+            raise KeyError(record.chromosome[st_names.fault].to_string())
+        bad = st_rows.fault
+        if bad is not None:
             name = record.chromosome[bad].to_string()
             raise ValueError(f"interval {bad} ({name}:{int(start[bad])}-{int(stop[bad])}) is not inside the contig "
                              f"({genome._all[name]} bases)")

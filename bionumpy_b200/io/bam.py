@@ -138,12 +138,12 @@ class BamBuffer:
         starts, status = ops.bam_split(d, len(cls.header.names))
         fields = ops.bam_fields(d, starts, status)
         st = ops.read_status(status)                                 # the one synchronisation of this chunk
-        n, size, fault = st.n_records, st.n_complete_bytes, st.words[nv.ST_BAD_BASE]
-        if fault == nv.INT64_MAX and last and size < d.numel():
-            fault = n << 8 | nv.BAM_TRUNCATED
-        if fault != nv.INT64_MAX:
-            record = n_before + (fault >> 8)
-            raise FormatException(f"BAM record {record}: {FAULTS.get(fault & 255, 'invalid record')}",
+        n, size, fault = st.n_records, st.n_complete_bytes, st.record_fault()
+        if fault is None and last and size < d.numel():
+            fault = n, nv.BAM_TRUNCATED
+        if fault is not None:
+            record = n_before + fault[0]
+            raise FormatException(f"BAM record {record}: {FAULTS.get(fault[1], 'invalid record')}",
                                   line_number=record)
         if n == 0:
             return None

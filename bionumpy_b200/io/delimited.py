@@ -69,10 +69,9 @@ class DelimitedBuffer:
         starts, lens, _ = ops.line_split(chunk, 1, 0, 0, ord(cls.COMMENT), False, 0, max_rows=n_lines)
         cols, status = ops.delimited_columns(chunk, starts, lens, cls._kinds)
         # the one synchronisation of the columns: the first fault and the chunk's size
-        fault, last_end = (int(x) for x in torch.cat([status[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1],
-                                                      starts[-1:] + lens[-1:]]).cpu().tolist())
-        if fault != nv.INT64_MAX:
-            line, col, kind = fault >> 8, (fault >> 3) & 31, fault & 7
+        st, last_end = ops.read_back(status, starts[-1:] + lens[-1:])
+        if st.fault is not None:
+            line, col, kind = st.column_fault()
             raise FormatException(f"{_FAULTS.get(kind, 'Invalid line')} (column {col})", line_number=line)
         data = chunk[:last_end + 1]
         fields = []
@@ -178,10 +177,9 @@ class DelimitedText:
                             f"{', '.join(t.__name__ for t in _WRITTEN)} are written")
         self.columns = [_column(entries, f) for f in entries._fields]
         self.offsets, status = ops.delimited_offsets(self.columns)
-        self.size, fault = (int(x) for x in torch.cat([self.offsets[-1:],
-                                                       status[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]).cpu().tolist())
-        if fault != nv.INT64_MAX:
-            line, col = fault >> 8, (fault >> 3) & 31
+        self.size, st = ops.read_back(self.offsets[-1:], status)
+        if st.fault is not None:
+            line, col, _ = st.column_fault()
             raise ValueError(f"line {line}: the {entries._fields[col]} column holds a strand code that is not "
                              "'+', '-' or '.'")
 

@@ -136,7 +136,7 @@ class IndexedFasta:
             rows = RowView(intervals.chromosome)
             start, stop = intervals.start.to(torch.int64).contiguous(), intervals.stop.to(torch.int64).contiguous()
             ids, st_names = ops.name_lookup(rows.base, rows.starts, rows.lens, text, name_offsets)
-            bad_names = [st_names[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1]]
+            extra = [st_names]
             name_of = lambda r: intervals.chromosome[r].to_string()
         else:
             if hasattr(intervals, "chromosome"):
@@ -145,10 +145,10 @@ class IndexedFasta:
             name_of = lambda r: rows[r][0]
             cols = torch.tensor([[contig_ids[n] for n, _, _ in rows], [a for _, a, _ in rows], [b for _, _, b in rows]],
                                 dtype=torch.int64).to(self._file.device)
-            ids, start, stop, bad_names = cols[0].to(torch.int32), cols[1], cols[2], []
-        out, row_lens, bad_row, bad_name = ops.interval_gather(self._file, start, stop, ids, contigs, extra=bad_names)
-        if bad_name and bad_name[0] != nv.INT64_MAX:
-            raise KeyError(name_of(bad_name[0]))
+            ids, start, stop, extra = cols[0].to(torch.int32), cols[1], cols[2], []
+        out, row_lens, bad_row, st_names = ops.interval_gather(self._file, start, stop, ids, contigs, extra=extra)
+        if st_names and st_names[0].fault is not None:
+            raise KeyError(name_of(st_names[0].fault))
         if bad_row is not None:
             name = name_of(bad_row)
             where = f"interval {bad_row} ({name}:{int(start[bad_row])}-{int(stop[bad_row])})"

@@ -120,15 +120,10 @@ class Formatted:
     def __init__(self, fields, fmt, line_width):
         self.fields, self.fmt, self.line_width = fields, fmt, line_width
         self.offsets, status = ops.format_offsets(fmt, line_width, fields)
-        words = torch.cat([self.offsets[-1:], status]).cpu().tolist()     # the one synchronisation
-        self.size = int(words[0])
-        st = ops.ScanStatus(words[1:])
-        bad = st.bad_base(fields[1][2].numel())
-        if bad is not None:
-            seq = fields[1]
+        self.size, st = ops.read_back(self.offsets[-1:], status)
+        offset = st.bad_base_offset(fields[1][2])
+        if offset is not None:
             from ..encodings import EncodingError
-            row, pos = bad
-            offset = int(seq[2][:row].to(torch.int64).sum().item()) + pos
             raise EncodingError(f"Invalid sequence code at flat offset {offset}: it is not a letter of the alphabet",
                                 offset)
 

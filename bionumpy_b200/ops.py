@@ -92,19 +92,55 @@ class ScanStatus:
         v = self.words[nv.ST_BAD_PLUS_ENTRY]
         return None if v == nv.INT64_MAX or v >= self.n_records else v
 
+    # The first fault a kernel reported in status[ST_BAD_BASE], in one of the layouts of bnpk.h (bnpk_device.cuh packs
+    # them): a plain index, (row << 32 | position), (line << 8 | column << 3 | kind) or (record << 8 | kind).
+    @property
+    def fault(self):
+        """The raw fault word, or None."""
+        v = self.words[nv.ST_BAD_BASE]
+        return None if v == nv.INT64_MAX else v
+
     def bad_base(self, n_rows=None):
         """(row, position) of the first byte outside the alphabet, or None."""
-        v = self.words[nv.ST_BAD_BASE]
-        if v == nv.INT64_MAX:
+        v = self.fault
+        if v is None or n_rows is not None and v >> 32 >= n_rows:
             return None
-        row, pos = v >> 32, v & 0xFFFFFFFF
-        if n_rows is not None and row >= n_rows:
+        return v >> 32, v & 0xFFFFFFFF
+
+    def bad_base_offset(self, lens):
+        """The flat offset of the first byte outside the alphabet in rows of lengths ``lens`` (a tensor), or None:
+        the offset the reference's EncodingError names.  The lengths before the row are read only for a row > 0."""
+        bad = self.bad_base(lens.numel())
+        if bad is None:
             return None
-        return row, pos
+        row, pos = bad
+        return int(lens[:row].to(torch.int64).sum().item()) + pos if row else pos
+
+    def column_fault(self):
+        """(line, column, nv.BAD_*) of the first bad field of a delimited text, or None."""
+        v = self.fault
+        return None if v is None else (v >> 8, (v >> 3) & 31, v & 7)
+
+    def record_fault(self):
+        """(record, nv.BAM_BAD_*) of the first bad record, or None."""
+        v = self.fault
+        return None if v is None else (v >> 8, v & 0xFF)
 
 
 def read_status(status_t) -> ScanStatus:
     return ScanStatus(status_t.cpu().tolist())   # synchronises the stream
+
+
+def read_back(*tensors):
+    """Status blocks and one-word device tensors copied to the host by one .cpu(), the one synchronisation: a
+    ScanStatus for each status block (its first ST_WORDS words) and an int for each one-word tensor, in order."""
+    parts = [t.reshape(-1)[:1 if t.numel() == 1 else nv.ST_WORDS].to(torch.int64) for t in tensors]
+    words = torch.cat(parts).cpu().tolist() if parts else []
+    out = []
+    for p in parts:
+        out.append(words[0] if p.numel() == 1 else ScanStatus(words[:nv.ST_WORDS]))
+        words = words[p.numel():]
+    return out
 
 
 @_on_device
@@ -551,7 +587,7 @@ def format_records(fmt, line_width, fields, offsets, out_begin=0, out_end=None, 
 def delimited_columns(chunk, starts, lens, kinds, status=None):
     """The tab-separated columns of the lines (starts, lens) of ``chunk``, one nv.COL_* kind per column.  Returns
     (columns, status): per column None (COL_SKIP), (starts int64, lens int32) of text, int64 values or uint8 strand
-    codes; the first fault is (line << 8 | column << 3 | nv.BAD_*) in status[ST_BAD_BASE]."""
+    codes; the first fault is in status[ST_BAD_BASE] (ScanStatus.column_fault)."""
     head, _ = _rows_args(chunk, starts, lens, status=status)
     n, dev = lens.numel(), chunk.device
     if not 1 <= len(kinds) <= nv.MAX_COLUMNS:
@@ -637,14 +673,14 @@ def interval_copy(file, start, stop, offsets, total, ids=None, contigs=None, str
 
 def interval_gather(file, start, stop, ids=None, contigs=None, strand=None, complement_lut=None, extra=()):
     """Both passes of bnpk_interval_gather around the one synchronisation a gather needs: the check pass, the row
-    offsets, then a single .cpu() of the output size, the first bad row and the ``extra`` one-word device tensors (a
-    caller's own status words).  Returns (out, row_lens, bad_row, extra words).  With a bad row the copy pass is not
+    offsets, then a single read_back of the output size, the first bad row and the ``extra`` status blocks and
+    one-word device tensors of the caller.  Returns (out, row_lens, bad_row, what read_back gives for ``extra``).  With a bad row the copy pass is not
     launched and ``out`` is None: the caller words the error.  A row of more than INT32_MAX bases is a bad row."""
     row_lens, status = interval_check(file, start, stop, ids, contigs)
     offsets = row_offsets(row_lens)
-    total, bad, *words = torch.cat([offsets[-1:], status[nv.ST_BAD_BASE:nv.ST_BAD_BASE + 1], *extra]).cpu().tolist()
-    if bad != nv.INT64_MAX:
-        return None, row_lens, bad, words
+    total, st, *words = read_back(offsets[-1:], status, *extra)
+    if st.fault is not None:
+        return None, row_lens, st.fault, words
     return interval_copy(file, start, stop, offsets, total, ids, contigs, strand, complement_lut), row_lens, None, words
 
 
@@ -821,7 +857,7 @@ def _out_columns(columns):
 @_on_device
 def delimited_offsets(columns, status=None):
     """bnpk_delimited_offsets: (int64[E + 1] line offsets, status); a strand code above 2 is reported in
-    status[ST_BAD_BASE] as (line << 8 | column << 3 | nv.BAD_STRAND)."""
+    status[ST_BAD_BASE] (ScanStatus.column_fault)."""
     arr, n, dev = _out_columns(columns)
     _status(status)
     offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
@@ -851,8 +887,8 @@ BAM_MIN_RECORD = 36             # block_size word + the 32 fixed bytes
 @_on_device
 def bam_split(chunk, n_ref, segment_bytes=BAM_SEGMENT_BYTES, status=None):
     """bnpk_bam_split: (starts int64[n // 36 + 1], status).  The first status[ST_N_RECORDS] starts are the chunk's
-    complete records; status[ST_N_COMPLETE_BYTES] is their size, status[ST_BAD_BASE] the first fault as
-    (record << 8 | nv.BAM_BAD_*) and status[ST_N_VALUES] the number of segments walked again."""
+    complete records; status[ST_N_COMPLETE_BYTES] is their size, status[ST_BAD_BASE] the first fault
+    (ScanStatus.record_fault) and status[ST_N_VALUES] the number of segments walked again."""
     chunk_p = _pointer(chunk, "chunk", torch.uint8)
     _status(status)
     if segment_bytes < 64:

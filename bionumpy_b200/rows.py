@@ -97,6 +97,6 @@ class RowView:
             status = ops.read_status(status)
         if rescan is not None and status.bad_base() is not None:
             status = ops.read_status(rescan(self))
-        bad = status.bad_base(self.lens.numel())
-        if bad is not None:
-            self.alphabet_encoding._raise_encoding_error(bad[0], bad[1], self.lens)
+        offset = status.bad_base_offset(self.lens)
+        if offset is not None:
+            self.alphabet_encoding._raise_encoding_error(offset)

@@ -181,7 +181,7 @@ class KmerCounter:
         if words[nv.ST_TABLE_FULL]:
             self._error = RuntimeError("k-mer table overflowed (the load limit was not kept): counts are incomplete")
             raise self._error
-        return words
+        return ops.ScanStatus(words)
 
     def _grow(self, slots):
         dev = self._keys.device
@@ -238,8 +238,7 @@ class KmerCounter:
                 self._grow(slots)
             ops.rows_kmer_table_insert(rows.base, pieces.starts[row:end], pieces.lens[row:end], rows.enc_mode, k,
                                        self._keys, self._counts, n_used_t, self._cxor, rows.lut, status=self._status())
-            words = self._read_state()
-            if words[nv.ST_BAD_BASE] != nv.INT64_MAX:
+            if self._read_state().fault is not None:
                 try:
                     rows.raise_bad_base(self._state[:nv.ST_WORDS], rescan_kmers)
                 except EncodingError as e:

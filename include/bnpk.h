@@ -63,9 +63,13 @@ enum {
                                      io/one_line_buffer.py:155-173                         */
     BNPK_ST_BAD_PLUS_ENTRY = 4,   /* min entry whose 3rd line does not start with '+'
                                      -> line_number = 2 + entry*4, io/fastq_buffer.py:38-45 */
-    BNPK_ST_BAD_BASE = 5,      /* min (row << 32 | position-in-row) of a byte outside the
-                                  alphabet (INT64_MAX = none) -> EncodingError(offset),
-                                  encodings/alphabet_encoding.py:34-46                     */
+    BNPK_ST_BAD_BASE = 5,      /* the smallest fault reported (INT64_MAX = none), in one of four
+                                  layouts, each packed by one helper of csrc/bnpk_device.cuh:
+                                  fault_row_pos  (row << 32 | position-in-row): a byte outside the
+                                    alphabet -> EncodingError(offset), alphabet_encoding.py:34-46
+                                  fault_column   (line << 8 | column << 3 | BNPK_BAD_*), column <= 31
+                                  fault_record   (record << 8 | BNPK_BAM_BAD_*)
+                                  or a plain row / value index                             */
     BNPK_ST_N_BASES = 6,       /* sum of row lengths processed                             */
     BNPK_ST_N_VALUES = 7,      /* k-mers / minimizers produced or counted                  */
     BNPK_ST_N_LONG_ROWS = 8,   /* rows that did not fit a tile halo and took the long path */
@@ -318,7 +322,7 @@ int bnpk_multiline_entries(const uint8_t *chunk, const int64_t *line_starts, con
  *     BNPK_COL_INT_OR_DOT  as BNPK_COL_INT, and "." reads as 0 (Optional[int], io/strops.py:69-83)
  *     BNPK_COL_STRAND      out = uint8[n_lines] StrandEncoding code: '+' 0, '-' 1, '.' 2
  *   When the first line ends in '\r', a '\r' that ends a line is not part of its last column.  The first fault is
- *   atomicMin-ed into status[BNPK_ST_BAD_BASE] as (line << 8 | column << 3 | BNPK_BAD_*) (status pre-initialised).
+ *   atomicMin-ed into status[BNPK_ST_BAD_BASE] as fault_column(line, column, BNPK_BAD_*) (status pre-initialised).
  *   BNPK_E_BADARG for a NULL pointer with n_lines > 0, n_columns outside 1..BNPK_MAX_COLUMNS, an unknown kind or a
  *   missing output.
  * bnpk_name_lookup: out_ids[r] = the index k of the name table with names[name_offsets[k] .. name_offsets[k + 1]) equal
@@ -514,8 +518,9 @@ typedef struct bnpk_field {
 
 /* out_offsets int64[E+1]: the exclusive prefix sum of the entry sizes, out_offsets[E] = the text's size (int64: a
  * wrapped chromosome with a long name can exceed int32).  When the sequence field has a LUT, also reads every sequence
- * byte once: the first byte b with lut256[b] == 0 is reported as (entry << 32 | position) in status[BNPK_ST_BAD_BASE]
- * (status pre-initialised; EncodingError(offset), encodings/alphabet_encoding.py:34-46).  Raw text is not read.
+ * byte once: the first byte b with lut256[b] == 0 is reported as fault_row_pos(entry, position) in
+ * status[BNPK_ST_BAD_BASE] (status pre-initialised; EncodingError(offset), encodings/alphabet_encoding.py:34-46).  Raw
+ * text is not read.
  * workspace as for bnpk_row_offsets with n := E. */
 int bnpk_format_offsets(int format, int line_width, size_t n_entries, const bnpk_field *fields, int64_t *out_offsets,
                         int64_t *status, void *workspace, size_t workspace_bytes, void *stream);
@@ -533,8 +538,8 @@ int bnpk_format_records(int format, int line_width, size_t n_entries, const bnpk
  *     BNPK_COL_STRAND  codes[e] (uint8, StrandEncoding) as '+' (0), '-' (1), '.' (2); another code is written as '.'
  *                      and reported by bnpk_delimited_offsets
  *   bnpk_delimited_offsets: out_offsets int64[E + 1], the exclusive prefix sum of the line sizes (out_offsets[E] = the
- *   text's size); the first bad strand code is atomicMin-ed into status[BNPK_ST_BAD_BASE] as (line << 8 | column << 3
- *   | BNPK_BAD_STRAND) (status pre-initialised).  workspace as for bnpk_row_offsets with n := E.
+ *   text's size); the first bad strand code is atomicMin-ed into status[BNPK_ST_BAD_BASE] as fault_column(line,
+ *   column, BNPK_BAD_STRAND) (status pre-initialised).  workspace as for bnpk_row_offsets with n := E.
  *   bnpk_delimited_format: bytes [out_begin, out_end) of that text written to out[0 .. out_end - out_begin), as
  *   bnpk_format_records.  BNPK_E_BADARG before any device work for a bad column count or kind, a missing pointer,
  *   out_begin < 0 or out_end < out_begin. */
@@ -566,12 +571,13 @@ int bnpk_delimited_format(const bnpk_out_column *columns, int n_columns, size_t 
  *     block_size >= 32, -1 <= refID, next_refID < n_ref, l_read_name >= 1 and the name ends in NUL, and
  *     32 + l_read_name + 4 n_cigar_op + (l_seq + 1) / 2 + l_seq <= block_size with l_seq >= 0.
  *     status (pre-initialised): [BNPK_ST_N_RECORDS] = R, [BNPK_ST_N_COMPLETE_BYTES] = the bytes of those records (the
- *     rest begins the next chunk's first record), [BNPK_ST_BAD_BASE] = (R << 8 | BNPK_BAM_BAD_*) when the walk
+ *     rest begins the next chunk's first record), [BNPK_ST_BAD_BASE] = fault_record(R, BNPK_BAM_BAD_*) when the walk
  *     stopped at a record that fails the check, [BNPK_ST_N_VALUES] = the segments walked again.  workspace int64[7 *
  *     ceil(n / segment_bytes)]; three kernels, no synchronisation.
  *   bnpk_bam_fields: one thread per record r < min(max_records, status[BNPK_ST_N_RECORDS]) writes
- *     fields[f * max_records + r] for the BNPK_BAM_F_* below, and atomicMin-s (r << 8 | BNPK_BAM_BAD_CIGAR_OP) into
- *     status[BNPK_ST_BAD_BASE] for a cigar op code above 8.  The records are those bnpk_bam_split found.
+ *     fields[f * max_records + r] for the BNPK_BAM_F_* below, and atomicMin-s fault_record(r,
+ *     BNPK_BAM_BAD_CIGAR_OP) into status[BNPK_ST_BAD_BASE] for a cigar op code above 8.  The records are those
+ *     bnpk_bam_split found.
  *   bnpk_bam_sequence: the l_seq 4-bit codes of every row, high nibble first, one byte each, at out[offsets[r] ..
  *     offsets[r + 1]) (offsets = bnpk_row_offsets of l_seq); 16 output bytes per thread.
  *   bnpk_bam_cigar: the n_cigar_op cigar words of every row as op = word & 15 (uint8) and length = word >> 4 (int64)
