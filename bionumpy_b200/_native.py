@@ -23,7 +23,9 @@ ST_WORDS = 16
 FMT_FASTQ, FMT_FASTA, FMT_FASTA_WRAPPED = 0, 1, 2
 MAX_COLUMNS = 16
 COL_SKIP, COL_TEXT, COL_INT, COL_INT_OR_DOT, COL_STRAND = 0, 1, 2, 3, 4
-BAD_TABS, BAD_COLUMNS, BAD_INT, BAD_STRAND = 1, 2, 3, 4
+BAD_TABS, BAD_COLUMNS, BAD_INT, BAD_STRAND, BAD_ATTRIBUTE = 1, 2, 3, 4, 5
+MAX_KEYS, MAX_KEY_LEN = 8, 32
+ATTR_GTF, ATTR_GFF = 0, 1
 PILEUP_COUNT, PILEUP_ANY = 0, 1
 RUNS_MAX, RUNS_MIN, RUNS_SUM, RUNS_ANY = 0, 1, 2, 3
 (OP_ADD, OP_SUB, OP_MUL, OP_AND, OP_OR, OP_XOR, OP_MIN, OP_MAX, OP_EQ, OP_NE, OP_LT, OP_LE, OP_GT,
@@ -87,6 +89,7 @@ SIGNATURES = {
     "bnpk_name_lookup": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
     "bnpk_interval_gather": (_i, [_vp, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                   _vp]),
+    "bnpk_attribute_values": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "bnpk_interval_events": (_i, [_vp, _vp, _vp, _vp, _vp, _sz, _i64, _sz, _vp, _vp, _vp, _vp, _vp]),
     "bnpk_pileup_runs": (_i, [_vp, _sz, _i64, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "bnpk_runs_reduce": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _sz, _vp]),

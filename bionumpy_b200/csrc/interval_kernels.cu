@@ -10,6 +10,8 @@
 // interval_copy_kernel: eight lanes per row; every 16-byte output unit (aligned on the output address) whose source
 //   lies on one line of the file is one unaligned 16-byte gather and one vector store, reversed and complemented in
 //   registers for a '-' row; the units at the row's ends and those that straddle a line end go byte by byte.
+// attribute_values_kernel: one warp per row of a GTF/GFF attribute column, 32-byte windows balloted into masks of
+//   ';', '"', ' ' and '=' and walked one attribute boundary at a time (GTFEntry._get_attributes, datatypes/gtf.py).
 #include "bnpk_host.h"
 
 namespace bnpk {
@@ -267,6 +269,166 @@ __global__ void __launch_bounds__(kCopyThreads) interval_copy_kernel(const __gri
     }
 }
 
+// attribute_values_kernel: one warp per row of a GTF/GFF attribute column.  The warp reads the row in 32-byte windows,
+// one byte per lane, and ballots the window's ';', '"', ' ' and '=' into four masks.  Every lane then runs the same
+// scalar walk over those masks: each step takes the first bit of the mask its state waits for, so the walk costs one
+// step per attribute boundary, not per byte, and the bytes are read once, coalesced.  At a key's end the lanes compare
+// the key with the requested keys of its length (one byte per lane).  Lane k keeps key k's value.
+constexpr int kAttrThreads = 256;
+enum AttrState { kPre, kKey, kGap, kQuote, kTail, kVal };
+
+// the bits of a window starting at w that lie at or after position cur
+__device__ __forceinline__ unsigned from_mask(int32_t cur, int32_t w) {
+    return cur <= w ? ~0u : cur - w >= 32 ? 0u : ~0u << (cur - w);
+}
+
+struct AttrArgs {
+    const uint8_t *base;
+    uint64_t base_bytes;
+    const int64_t *starts;
+    const int32_t *lens;
+    int64_t n_rows;
+    const uint8_t *select;
+    int n_keys;
+    int gff;
+    int key_len[BNPK_MAX_KEYS];
+    uint8_t keys[BNPK_MAX_KEYS][BNPK_MAX_KEY_LEN];
+    int64_t *out_starts;
+    int32_t *out_lens;
+    int64_t *status;
+};
+
+__global__ void __launch_bounds__(kAttrThreads) attribute_values_kernel(const __grid_constant__ AttrArgs a) {
+    __shared__ uint8_t s_keys[BNPK_MAX_KEYS][BNPK_MAX_KEY_LEN];
+    for (int i = threadIdx.x; i < BNPK_MAX_KEYS * BNPK_MAX_KEY_LEN; i += kAttrThreads)
+        s_keys[i / BNPK_MAX_KEY_LEN][i % BNPK_MAX_KEY_LEN] = a.keys[i / BNPK_MAX_KEY_LEN][i % BNPK_MAX_KEY_LEN];
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const unsigned all = (1u << a.n_keys) - 1;
+    const int64_t n_warps = (int64_t)gridDim.x * (kAttrThreads / 32);
+    for (int64_t r = ((int64_t)blockIdx.x * kAttrThreads + threadIdx.x) / 32; r < a.n_rows; r += n_warps) {
+        const int64_t s = a.starts[r];
+        int64_t my_start = s;
+        int32_t my_len = 0;
+        if (a.select && !a.select[r]) {
+            if (lane < a.n_keys) {
+                a.out_starts[lane * a.n_rows + r] = my_start;
+                a.out_lens[lane * a.n_rows + r] = my_len;
+            }
+            continue;
+        }
+        int32_t L = max(a.lens[r], 0);
+        if (s < 0 || (uint64_t)s + (uint64_t)L > a.base_bytes) L = 0;
+        const uint8_t *row = a.base + (s < 0 ? 0 : s);
+        int state = kPre;
+        int32_t cur = 0, ks = 0, vs = 0, last_ns = -1;
+        unsigned found = 0, match = 0;
+        // record the value [v0, v0 + n) of the keys in `match` that have none yet
+        auto record = [&](int32_t v0, int32_t n) {
+            const unsigned fresh = match & ~found;
+            found |= fresh;
+            if (fresh >> lane & 1) {
+                my_start = s + v0;
+                my_len = n;
+            }
+        };
+        for (int32_t w = 0; w < L && found != all; w += 32) {
+            const int32_t i = w + lane;
+            const uint8_t c = i < L ? row[i] : (uint8_t)0;
+            const unsigned valid = L - w >= 32 ? ~0u : (1u << (L - w)) - 1;
+            const unsigned semi = __ballot_sync(~0u, c == ';');
+            const unsigned quote = __ballot_sync(~0u, c == '"');
+            const unsigned nonsp = ~__ballot_sync(~0u, c == ' ') & valid;
+            const unsigned key_end = a.gff ? (__ballot_sync(~0u, c == '=') | semi) : (~nonsp & valid) | semi;
+            for (;;) {
+                const unsigned from = from_mask(cur, w);
+                const unsigned wait = state == kPre || state == kGap ? nonsp
+                                      : state == kKey              ? key_end
+                                      : state == kQuote            ? quote
+                                                                   : semi;
+                const unsigned ev = wait & from;
+                if (!ev) break;
+                const int bit = __ffs(ev) - 1;
+                const int32_t p = w + bit;
+                const bool at_semi = semi >> bit & 1;
+                cur = p + 1;
+                if (state == kPre) {
+                    if (!at_semi) {
+                        ks = p;
+                        cur = p;
+                        state = kKey;
+                    }
+                } else if (state == kKey) {
+                    match = 0;
+                    if (at_semi) {
+                        state = kPre;       // an attribute without a value
+                        continue;
+                    }
+                    const int32_t n = p - ks;
+                    unsigned cand = 0;
+#pragma unroll
+                    for (int k = 0; k < BNPK_MAX_KEYS; ++k)
+                        if (a.key_len[k] == n && !(found >> k & 1)) cand |= 1u << k;
+                    cand &= all;
+                    if (cand) {
+                        const uint8_t b = lane < n ? row[ks + lane] : (uint8_t)0;
+                        while (cand) {
+                            const int k = __ffs(cand) - 1;
+                            cand &= cand - 1;
+                            if (__ballot_sync(~0u, lane >= n || b == s_keys[k][lane]) == ~0u) match |= 1u << k;
+                        }
+                    }
+                    if (a.gff) {
+                        vs = p + 1;
+                        state = kVal;
+                    } else {
+                        state = kGap;
+                    }
+                } else if (state == kGap) {
+                    if (at_semi) {
+                        record(p, 0);
+                        state = kPre;
+                    } else if (quote >> bit & 1) {
+                        vs = p + 1;
+                        state = kQuote;
+                    } else {
+                        vs = last_ns = p;
+                        state = kVal;
+                    }
+                } else if (state == kQuote) {
+                    record(vs, p - vs);
+                    state = kTail;
+                } else if (state == kTail) {
+                    state = kPre;
+                } else {
+                    if (a.gff) {
+                        record(vs, p - vs);
+                    } else {
+                        const unsigned before = nonsp & from & ((1u << bit) - 1);
+                        const int32_t last = before ? w + 31 - __clz(before) : last_ns;
+                        record(vs, last + 1 - vs);
+                    }
+                    state = kPre;
+                }
+            }
+            if (state == kVal && !a.gff) {
+                const unsigned ns = nonsp & from_mask(cur, w);
+                if (ns) last_ns = w + 31 - __clz(ns);
+            }
+        }
+        if (found != all) {
+            if (state == kGap) record(L, 0);
+            else if (state == kQuote) record(vs, L - vs);
+            else if (state == kVal) record(vs, (a.gff ? L : last_ns + 1) - vs);
+        }
+        if (lane < a.n_keys) {
+            a.out_starts[lane * a.n_rows + r] = my_start;
+            a.out_lens[lane * a.n_rows + r] = my_len;
+            if (!(found >> lane & 1)) report_fault(a.status, fault_column(r, lane, BNPK_BAD_ATTRIBUTE));
+        }
+    }
+}
+
 }  // namespace
 }  // namespace bnpk
 
@@ -334,6 +496,40 @@ int bnpk_interval_gather(const uint8_t *file, size_t file_bytes, size_t n_rows, 
     const size_t rows_per_cta = kCopyThreads / kLanesPerRow;
     return launch("interval_copy_kernel", interval_copy_kernel, grid_cap((n_rows + rows_per_cta - 1) / rows_per_cta, 8),
                   kCopyThreads, 0, (cudaStream_t)stream, false, a);
+}
+
+int bnpk_attribute_values(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                          size_t n_rows, const uint8_t *select, const uint8_t *keys, const int64_t *key_offsets,
+                          int n_keys, int mode, int64_t *out_starts, int32_t *out_lens, int64_t *status, void *stream) {
+    if (n_keys < 1 || n_keys > BNPK_MAX_KEYS || !keys || !key_offsets)
+        return set_err(BNPK_E_BADARG, "1 to BNPK_MAX_KEYS keys, as a host table (keys, key_offsets)");
+    if (mode != BNPK_ATTR_GTF && mode != BNPK_ATTR_GFF) return set_err(BNPK_E_BADARG, "unknown attribute mode");
+    AttrArgs a;
+    memset(&a, 0, sizeof(a));
+    for (int k = 0; k < n_keys; ++k) {
+        const int64_t n = key_offsets[k + 1] - key_offsets[k];
+        if (n < 1 || n > BNPK_MAX_KEY_LEN) return set_err(BNPK_E_BADARG, "a key holds 1 to BNPK_MAX_KEY_LEN bytes");
+        a.key_len[k] = (int)n;
+        memcpy(a.keys[k], keys + key_offsets[k], (size_t)n);
+    }
+    if (n_rows == 0) return 0;
+    if (!base || !starts || !lens || !out_starts || !out_lens || !status)
+        return set_err(BNPK_E_BADARG, "base, starts, lens, out_starts, out_lens and status are required");
+    a.base = base;
+    a.base_bytes = (uint64_t)base_bytes;
+    a.starts = starts;
+    a.lens = lens;
+    a.n_rows = (int64_t)n_rows;
+    a.select = select;
+    a.n_keys = n_keys;
+    a.gff = mode == BNPK_ATTR_GFF;
+    a.out_starts = out_starts;
+    a.out_lens = out_lens;
+    a.status = status;
+    const size_t rows_per_cta = kAttrThreads / 32;
+    return launch("attribute_values_kernel", attribute_values_kernel,
+                  grid_cap((n_rows + rows_per_cta - 1) / rows_per_cta, 8), kAttrThreads, 0, (cudaStream_t)stream, false,
+                  a);
 }
 
 }  // extern "C"

@@ -349,6 +349,36 @@ std::tuple<Tensor, Tensor> name_lookup(const Tensor &base, const Tensor &starts,
     return {ids, status};
 }
 
+// GTF/GFF attribute values: (value starts int64[K, R], value lens int32[K, R], status) of the keys (strings) in the
+// attribute column rows; rows where `select` (uint8[R]) is 0 are not read
+std::tuple<Tensor, Tensor, Tensor> attribute_values(const Tensor &base, const Tensor &starts, const Tensor &lens,
+                                                    std::vector<std::string> keys, int64_t mode,
+                                                    const c10::optional<Tensor> &select) {
+    const Rows r = need_rows(base, starts, lens, c10::nullopt);
+    const uint8_t *sel = nullptr;
+    if (select) {
+        need(*select, torch::kUInt8, "select", base);
+        TORCH_CHECK((size_t)select->numel() == r.n_rows, "bnpk: select needs one flag per row");
+        sel = select->data_ptr<uint8_t>();
+    }
+    std::string text;
+    std::vector<int64_t> offsets{0};
+    for (const std::string &k : keys) {
+        text += k;
+        offsets.push_back((int64_t)text.size());
+    }
+    c10::cuda::CUDAGuard guard(base.device());
+    const int64_t n_keys = (int64_t)keys.size(), n = (int64_t)r.n_rows;
+    Tensor out_starts = torch::empty({n_keys, n}, base.options().dtype(torch::kInt64));
+    Tensor out_lens = torch::empty({n_keys, n}, base.options().dtype(torch::kInt32));
+    Tensor status = new_status(base);
+    check(r.call(bnpk_attribute_values, sel, reinterpret_cast<const uint8_t *>(text.data()), offsets.data(),
+                 (int)n_keys, (int)mode, out_starts.data_ptr<int64_t>(), out_lens.data_ptr<int32_t>(),
+                 status.data_ptr<int64_t>(), cur_stream(base)),
+          "attribute_values");
+    return {out_starts, out_lens, status};
+}
+
 // interval gather over a file image: ids (int32) index contigs = [offset int64, lenc int32, lenb int32, length int64];
 // no ids = one flat contig.  check: (row_lens int32, status); copy: uint8[total] at offsets (int64[R+1])
 struct Intervals {
@@ -788,6 +818,8 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("runs_reduce(Tensor run_starts, Tensor values, Tensor q_start, Tensor q_stop, int mode) -> Tensor");
     m.def("runs_extract(Tensor run_starts, Tensor values, Tensor q_start, Tensor offsets, int total) -> Tensor");
     m.def("interval_merge(Tensor start, Tensor stop, Tensor? same_prev, int distance) -> (Tensor, Tensor, Tensor, Tensor)");
+    m.def("attribute_values(Tensor base, Tensor starts, Tensor lens, str[] keys, int mode, Tensor? select) -> "
+          "(Tensor, Tensor, Tensor)");
     m.def("rows_equal_prev(Tensor base, Tensor starts, Tensor lens) -> Tensor");
     m.def("runs_combine(Tensor a_starts, Tensor a_values, Tensor b_starts, Tensor b_values, int op) "
           "-> (Tensor, Tensor, Tensor)");
@@ -826,6 +858,7 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("runs_reduce", &runs_reduce);
     m.impl("runs_extract", &runs_extract);
     m.impl("interval_merge", &interval_merge);
+    m.impl("attribute_values", &attribute_values);
     m.impl("rows_equal_prev", &rows_equal_prev);
     m.impl("runs_combine", &runs_combine);
     m.impl("interval_intersect", &interval_intersect);

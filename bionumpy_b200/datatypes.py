@@ -180,3 +180,83 @@ class BedGraph(_IntervalEntries):
     """datatypes/__init__.py:27-31: chromosome, start, stop and value.  The value is an integer (or bool) tensor here:
     the tracks it comes from hold integers, and a float value cannot be written."""
     _fields = ("chromosome", "start", "stop", "value")
+
+
+# GTF/GFF feature types that the selection methods pick, sorted as bytes for bnpk_name_lookup
+_FEATURE_TYPES = ("exon", "gene", "transcript")
+_feature_tables = {}
+
+
+def _feature_table(device):
+    """The feature types as a device name table (text, offsets int64[4]), built once per device."""
+    if device not in _feature_tables:
+        raw = [f.encode() for f in _FEATURE_TYPES]
+        text = torch.frombuffer(bytearray(b"".join(raw)), dtype=torch.uint8).to(device)
+        offsets = torch.tensor(np.cumsum([0] + [len(b) for b in raw]), dtype=torch.int64).to(device)
+        _feature_tables[device] = (text, offsets)
+    return _feature_tables[device]
+
+
+class GTFEntry(_Entries):
+    """datatypes/gtf.py GTFEntry: the nine GTF columns as text views of the chunk, start and stop int64 as written
+    (the start is not shifted from GTF's 1-based coordinates, as in the reference) and strand StrandEncoding codes.
+    ``score`` and ``phase`` stay text.  The attribute column keeps the reference's spelling, ``atributes``."""
+    _fields = ("chromosome", "source", "feature_type", "start", "stop", "score", "strand", "phase", "atributes")
+    _attribute_mode = 0         # nv.ATTR_GTF: key "value"
+
+    def get_genes(self):
+        """The rows whose feature_type is ``gene``, with their gene_id (GFFGeneEntry)."""
+        return self._select("gene", GFFGeneEntry)
+
+    def get_transcripts(self):
+        """The rows whose feature_type is ``transcript``, with gene_id and transcript_id (GFFTranscriptEntry)."""
+        return self._select("transcript", GFFTranscriptEntry)
+
+    def get_exons(self):
+        """The rows whose feature_type is ``exon``, with gene_id, transcript_id and exon_id (GFFExonEntry)."""
+        return self._select("exon", GFFExonEntry)
+
+    def _select(self, feature, cls):
+        """The rows of one feature type and the attribute values ``cls`` adds, as text views of the attribute column
+        (no copy).  The feature type is looked up on the device (other types get -1, which is no error), the attribute
+        kernel reads the selected rows once for every key, and the selected count and the first missing attribute
+        are read in one synchronisation.  A selected row without an attribute raises FormatException naming it, with
+        line_number = the row's index in this record set."""
+        from . import _native as nv
+        from . import ops
+        from .io.buffers import FieldView
+        from .io.exceptions import FormatException
+        from .rows import RowView
+        keys = cls._fields[len(GTFEntry._fields):]
+        types = RowView(self.feature_type)
+        text, offsets = _feature_table(types.base.device)
+        ids, _ = ops.name_lookup(types.base, types.starts, types.lens, text, offsets)
+        select = (ids == _FEATURE_TYPES.index(feature)).to(torch.uint8)
+        attributes = RowView(self.atributes)
+        starts, lens, status = ops.attribute_values(attributes.base, attributes.starts, attributes.lens, keys,
+                                                    nv.ATTR_GFF if self._attribute_mode else nv.ATTR_GTF, select)
+        st, n = ops.read_back(status, select.sum())
+        if st.fault is not None:
+            row, key, _ = st.column_fault()
+            raise FormatException(f"the {feature} has no {keys[key]} attribute", line_number=row)
+        idx = torch.nonzero_static(select, size=n).reshape(-1)
+        values = [getattr(self, f)[idx] for f in GTFEntry._fields]
+        values += [FieldView(attributes.base, lens[k][idx], starts[k][idx]) for k in range(len(keys))]
+        return cls(*values)
+
+
+class GFFEntry(GTFEntry):
+    """datatypes/gtf.py GFFEntry: the GTF columns, with GFF3 attributes (key=value)."""
+    _attribute_mode = 1         # nv.ATTR_GFF
+
+
+class GFFGeneEntry(GFFEntry):
+    _fields = GTFEntry._fields + ("gene_id",)
+
+
+class GFFTranscriptEntry(GFFGeneEntry):
+    _fields = GFFGeneEntry._fields + ("transcript_id",)
+
+
+class GFFExonEntry(GFFTranscriptEntry):
+    _fields = GFFTranscriptEntry._fields + ("exon_id",)

@@ -144,6 +144,12 @@ class Genome:
             buffer_type = Bed6Buffer
         return self.get_intervals(bnp_open(filename, buffer_type=buffer_type).read(), stranded)
 
+    def read_annotation(self, filename) -> "GenomicAnnotation":
+        """genome.py:390-422: a GTF or GFF file read on the device, with its genes, transcripts and exons placed on
+        this genome when first asked for (rows on contigs the genome leaves out are dropped)."""
+        from ..io.files import bnp_open
+        return GenomicAnnotation(bnp_open(filename).read(), self)
+
 
 def _read_sizes(filename):
     out = {}
@@ -222,7 +228,7 @@ class GenomicIntervals:
             idx = torch.as_tensor(np.asarray(idx))
         if isinstance(idx, torch.Tensor):
             idx = idx.to(self._ids.device)
-        return GenomicIntervals(self._record[idx], self._ids[idx], self._g_start[idx], self._g_stop[idx], self._genome)
+        return type(self)(self._record[idx], self._ids[idx], self._g_start[idx], self._g_stop[idx], self._genome)
 
     def __repr__(self):
         names = list(self._genome._sizes)
@@ -266,6 +272,64 @@ class GenomicIntervals:
         record = self._record[sel]
         local = stops[:k] - g_start[first] + _int64(record.start, ids.device)
         return GenomicIntervals(replace(record, stop=local), ids[first], g_start[first], stops[:k], self._genome)
+
+
+class Genes(GenomicIntervals):
+    """annotation.py Genes: gene intervals with their strand and gene_id."""
+
+    @property
+    def strand(self):
+        return self._record.strand
+
+    @property
+    def gene_id(self):
+        return self._record.gene_id
+
+
+class Transcripts(Genes):
+    @property
+    def transcript_id(self):
+        return self._record.transcript_id
+
+
+class Exons(Transcripts):
+    @property
+    def exon_id(self):
+        return self._record.exon_id
+
+
+class GenomicAnnotation:
+    """annotation.py GenomicAnnotation: the genes, transcripts and exons of GTF/GFF entries on a genome, each selected
+    and placed on the genome the first time it is asked for."""
+
+    def __init__(self, data, genome):
+        self._data, self._genome = data, genome
+        self._genes = self._transcripts = self._exons = None
+
+    @classmethod
+    def from_gtf_entries(cls, gtf_entries, genome) -> "GenomicAnnotation":
+        return cls(gtf_entries, genome)
+
+    @property
+    def genes(self) -> Genes:
+        if self._genes is None:
+            self._genes = Genes.from_intervals(self._data.get_genes(), self._genome)
+        return self._genes
+
+    @property
+    def transcripts(self) -> Transcripts:
+        if self._transcripts is None:
+            self._transcripts = Transcripts.from_intervals(self._data.get_transcripts(), self._genome)
+        return self._transcripts
+
+    @property
+    def exons(self) -> Exons:
+        if self._exons is None:
+            self._exons = Exons.from_intervals(self._data.get_exons(), self._genome)
+        return self._exons
+
+    def __repr__(self):
+        return f"GenomicAnnotation(genome={self._genome!r}, data={self._data!r})"
 
 
 class GenomicArray:
@@ -355,4 +419,5 @@ class GenomicArray:
 
 _add_operators(GenomicArray)
 
-__all__ = ["Genome", "GenomicIntervals", "GenomicArray", "ignore_underscores", "keep_all"]
+__all__ = ["Genome", "GenomicIntervals", "GenomicArray", "GenomicAnnotation", "Genes", "Transcripts", "Exons",
+           "ignore_underscores", "keep_all"]

@@ -11,7 +11,7 @@ import torch
 
 from .. import _native as nv
 from .. import ops
-from ..datatypes import Bed6, BedGraph, Interval, StrandedInterval
+from ..datatypes import Bed6, BedGraph, GFFEntry, GTFEntry, Interval, StrandedInterval
 from ..encoded_array import EncodedArray, EncodedRaggedArray, BaseEncoding
 from ..encodings import StrandEncoding
 from .buffers import FieldView, _to_device_bytes
@@ -141,6 +141,71 @@ class BdgBuffer(DelimitedBuffer):
     @classmethod
     def from_raw_buffer(cls, chunk, header_data=None):
         raise NotImplementedError("reading bedGraph is not supported: its values are floats")
+
+
+_GTF_KINDS = (nv.COL_TEXT, nv.COL_TEXT, nv.COL_TEXT, nv.COL_INT, nv.COL_INT, nv.COL_TEXT, nv.COL_STRAND, nv.COL_TEXT,
+              nv.COL_TEXT)
+
+
+class GTFBuffer(DelimitedBuffer):
+    """delimited_buffers.py GTFBuffer: the nine GTF columns (GTFEntry).  Read only."""
+    dataclass = GTFEntry
+    _kinds = _GTF_KINDS
+
+    @classmethod
+    def formatted(cls, entries):
+        raise NotImplementedError(f"writing {cls.__name__[:3]} is not supported")
+
+    from_data = formatted
+
+
+class GFFBuffer(GTFBuffer):
+    """delimited_buffers.py GFFBuffer (DelimitedBufferWithInernalComments): the GTF columns with GFF3 attributes, and
+    comment lines inside the chunk (``##sequence-region`` lines, ``###`` separators) dropped after the line split.
+    Two synchronisations: the comment count, then the columns.  A FormatException counts the chunk's lines, comments
+    included."""
+    dataclass = GFFEntry
+
+    @classmethod
+    def from_raw_buffer(cls, chunk, header_data=None):
+        chunk = _to_device_bytes(chunk)
+        n_lines = ops.count_byte(chunk, 10) if chunk.numel() else 0
+        if n_lines == 0:
+            raise IncompleteEntryException("No complete line in the buffer. Try increasing chunk_size.")
+        starts, lens, _ = ops.line_split(chunk, 1, 0, 0, ord(cls.COMMENT), False, 0, max_rows=n_lines)
+        keep = ((chunk[starts] != ord(cls.COMMENT)) | (lens == 0)).to(torch.uint8)
+        n_keep, last_end = ops.read_back(keep.sum(), starts[-1:] + lens[-1:])
+        data = chunk[:last_end + 1]
+        lines = torch.nonzero_static(keep, size=n_keep).reshape(-1)
+        if n_keep == 0:
+            empty = torch.zeros(0, dtype=torch.int64, device=chunk.device)
+            buf = cls(data, 0, [FieldView(data, lens[:0], starts[:0]) if k == nv.COL_TEXT else
+                                EncodedArray(empty.to(torch.uint8), StrandEncoding) if k == nv.COL_STRAND else empty
+                                for k in cls._kinds])
+            buf._n_chunk_lines = n_lines
+            return buf
+        cols, status = ops.delimited_columns(chunk, starts[lines], lens[lines], cls._kinds)
+        st, = ops.read_back(status)
+        if st.fault is not None:
+            line, col, kind = st.column_fault()
+            raise FormatException(f"{_FAULTS.get(kind, 'Invalid line')} (column {col})",
+                                  line_number=int(lines[line].item()))
+        fields = []
+        for kind, col in zip(cls._kinds, cols):
+            if kind == nv.COL_TEXT:
+                fields.append(FieldView(data, col[1], col[0]))
+            elif kind == nv.COL_STRAND:
+                fields.append(EncodedArray(col, StrandEncoding))
+            else:
+                fields.append(col)
+        buf = cls(data, n_keep, fields)
+        buf._n_chunk_lines = n_lines
+        return buf
+
+    @property
+    def n_lines(self) -> int:
+        """The chunk's lines, comments included (the reader counts a FormatException's line number with them)."""
+        return getattr(self, "_n_chunk_lines", self._n_lines)
 
 
 _WRITTEN = (Interval, StrandedInterval, Bed6, BedGraph)

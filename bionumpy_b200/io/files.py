@@ -34,8 +34,15 @@ def _buffer_type_for(suffix):
     if suffix == ".bam":
         from .bam import BamBuffer
         return BamBuffer
+    if suffix == ".gtf":
+        from .delimited import GTFBuffer
+        return GTFBuffer
+    if suffix in (".gff", ".gff3"):
+        from .delimited import GFFBuffer
+        return GFFBuffer
     raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
-                       f"(supported: .fq .fastq .fa .fasta .bed .bdg and their .gz forms, and .bam); pass buffer_type=")
+                       f"(supported: .fq .fastq .fa .fasta .bed .bdg .gtf .gff .gff3 and their .gz forms, and .bam); "
+                       f"pass buffer_type=")
 
 
 def _suffix(path):
@@ -59,6 +66,8 @@ def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
     if mode in WRITE_MODES and buffer_type is None and suffix == ".bam":      # BAM is read only
         raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
                            f"(supported: .fq .fastq .fa .fasta .bed .bdg and their .gz forms); pass buffer_type=")
+    if mode in WRITE_MODES and buffer_type is None and suffix in (".gtf", ".gff", ".gff3"):
+        raise NotImplementedError(f"writing {suffix} is not supported: GTF and GFF are read only")
     if mode in WRITE_MODES and buffer_type is None and suffix == ".bed":
         raise NotImplementedError("writing .bed by its suffix alone is not supported: name the format with "
                                   "buffer_type=bnp.io.BedBuffer (or Bed6Buffer)")

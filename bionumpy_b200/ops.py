@@ -625,6 +625,30 @@ def name_lookup(base, starts, lens, names, name_offsets, status=None):
     return ids, status
 
 
+@_on_device
+def attribute_values(base, starts, lens, keys, mode=nv.ATTR_GTF, select=None, status=None):
+    """bnpk_attribute_values: the values of the attributes ``keys`` (1 to MAX_KEYS strings) in the GTF
+    (nv.ATTR_GTF) or GFF (nv.ATTR_GFF) attribute column rows (base, starts, lens), read once for every key.  Returns
+    (value starts int64[K, R], value lens int32[K, R], status); rows where ``select`` (uint8[R]) is 0 are not read, and
+    the first selected row without a key is in status[ST_BAD_BASE] (ScanStatus.column_fault: row, key index,
+    nv.BAD_ATTRIBUTE)."""
+    head, _ = _rows_args(base, starts, lens, status=status)
+    n = starts.numel()
+    select_p = _pointer(select, "select", torch.uint8, n=n, optional=True)
+    raw = [k.encode() if isinstance(k, str) else bytes(k) for k in keys]
+    if not 1 <= len(raw) <= nv.MAX_KEYS or not all(1 <= len(k) <= nv.MAX_KEY_LEN for k in raw):
+        raise ValueError(f"1 to {nv.MAX_KEYS} keys of 1 to {nv.MAX_KEY_LEN} bytes, not {keys!r}")
+    text = ctypes.create_string_buffer(b"".join(raw), max(sum(map(len, raw)), 1))
+    offsets = (ctypes.c_int64 * (len(raw) + 1))(*[sum(map(len, raw[:i])) for i in range(len(raw) + 1)])
+    out_starts = torch.empty((len(raw), n), dtype=torch.int64, device=base.device)
+    out_lens = torch.empty((len(raw), n), dtype=torch.int32, device=base.device)
+    status = nv.new_status(base.device) if status is None else status
+    check(lib().bnpk_attribute_values(*head, select_p, ctypes.cast(text, ctypes.c_void_p),
+                                      ctypes.cast(offsets, ctypes.c_void_p), len(raw), mode, _pointer(out_starts),
+                                      _pointer(out_lens), _pointer(status), stream_ptr()))
+    return out_starts, out_lens, status
+
+
 def _intervals(start, stop):
     """(start, stop, R) of R intervals: int64 starts and one int64 stop per start."""
     start_p = _pointer(start, "start", torch.int64)

@@ -7,3 +7,4 @@ from .indexing import KmerIndex, KmerLookup
 from .bloom_filter import BloomFilter
 from .position_weight_matrix import get_motif_scores, PWM
 from .string_matcher import match_string, StringMatcher, FixedLenRegexMatcher, RegexMatcher
+from .genes import get_transcript_sequences

@@ -368,6 +368,32 @@ int bnpk_interval_gather(const uint8_t *file, size_t file_bytes, size_t n_rows, 
                          const uint8_t *complement_lut256, int32_t *row_lens, const int64_t *out_offsets, uint8_t *out,
                          int64_t *status, void *stream);
 
+/* bnpk_attribute_values: the values of up to BNPK_MAX_KEYS attributes in the GTF/GFF attribute column of every row
+ *   (GTFEntry._get_attributes / GFFEntry._get_attributes, datatypes/gtf.py), the row's text base[starts[r] .. + lens[r]).
+ *   `keys` is a HOST table: key k is keys[key_offsets[k] .. key_offsets[k + 1]), 1 to BNPK_MAX_KEY_LEN bytes.
+ *   Attributes are separated by ';'; spaces before a key are skipped.  The key must equal a requested key byte for byte
+ *   (gene_id matches neither havana_gene_id nor gene_idx); the first attribute with the key wins.
+ *     BNPK_ATTR_GTF  `key value`: the key ends at the first ' ', the value starts at the next byte that is not ' '.  A
+ *                    value that starts with '"' is the bytes up to the next '"' (a ';' inside the quotes does not end
+ *                    the attribute; no closing quote: up to the end of the row); any other value runs to the next ';'
+ *                    or the end of the row, trailing spaces trimmed.
+ *     BNPK_ATTR_GFF  `key=value`: the key ends at the first '=', the value runs to the next ';' or the end of the row,
+ *                    as written (no percent-decoding; "a,b" stays one value).
+ *   An attribute without a value (GTF: no ' ' before its ';'; GFF: no '=') matches no key.  Output: key k of row r at
+ *   out_starts[k * n_rows + r] (a base offset) and out_lens[k * n_rows + r]; a row with no value for a key, or not
+ *   selected (select != NULL and select[r] == 0), gets (starts[r], 0).  A selected row without key k is atomicMin-ed
+ *   into status[BNPK_ST_BAD_BASE] as fault_column(r, k, BNPK_BAD_ATTRIBUTE); rows not selected are not read.
+ *   BNPK_E_BADARG for n_keys outside 1..BNPK_MAX_KEYS, an empty or too long key, an unknown mode or a NULL pointer with
+ *   n_rows > 0. */
+#define BNPK_MAX_KEYS        8
+#define BNPK_MAX_KEY_LEN     32
+#define BNPK_ATTR_GTF        0
+#define BNPK_ATTR_GFF        1
+#define BNPK_BAD_ATTRIBUTE   5   /* a selected row without the requested attribute          */
+int bnpk_attribute_values(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                          size_t n_rows, const uint8_t *select, const uint8_t *keys, const int64_t *key_offsets,
+                          int n_keys, int mode, int64_t *out_starts, int32_t *out_lens, int64_t *status, void *stream);
+
 /* ---------------------------------------------------------------------------------------
  * Pileups, run-length tracks and interval merges (get_pileup, get_boolean_mask, merge_intervals
  * arithmetics/intervals.py:137-304; GenomicRunLengthArray and GenomicArray, genomic_data/genomic_track.py).
