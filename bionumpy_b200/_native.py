@@ -36,6 +36,11 @@ BAM_BAD_BLOCK_SIZE, BAM_BAD_REF_ID, BAM_BAD_NAME, BAM_BAD_SIZES, BAM_BAD_CIGAR_O
 (BAM_F_REF_ID, BAM_F_POS, BAM_F_MAPQ, BAM_F_FLAG, BAM_F_NAME_START, BAM_F_NAME_LEN, BAM_F_CIGAR_START, BAM_F_N_CIGAR,
  BAM_F_SEQ_START, BAM_F_L_SEQ, BAM_F_QUAL_START, BAM_F_REF_LEN) = range(12)
 BAM_FIELDS = 12
+BAD_CIGAR = 6
+(SAM_F_NAME_START, SAM_F_NAME_LEN, SAM_F_RNAME_START, SAM_F_RNAME_LEN, SAM_F_CIGAR_START, SAM_F_CIGAR_LEN,
+ SAM_F_RNEXT_START, SAM_F_RNEXT_LEN, SAM_F_SEQ_START, SAM_F_SEQ_LEN, SAM_F_QUAL_START, SAM_F_QUAL_LEN, SAM_F_EXTRA_START,
+ SAM_F_EXTRA_LEN, SAM_F_FLAG, SAM_F_POS, SAM_F_MAPQ, SAM_F_PNEXT, SAM_F_TLEN) = range(19)
+SAM_FIELDS = 19
 INT64_MAX = (1 << 63) - 1
 SMEM_MAX_BINS = 32768
 
@@ -105,6 +110,9 @@ SIGNATURES = {
     "bnpk_bam_fields": (_i, [_vp, _sz, _vp, _sz, _vp, _vp, _vp]),
     "bnpk_bam_sequence": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp]),
     "bnpk_bam_cigar": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "bnpk_sam_columns": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "bnpk_cigar_count": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "bnpk_cigar_unpack": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
 }
 
 

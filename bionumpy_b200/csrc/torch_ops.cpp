@@ -781,6 +781,45 @@ std::tuple<Tensor, Tensor> bam_cigar(const Tensor &chunk, const Tensor &cigar_st
     return {op, length};
 }
 
+// SAM lines: (fields int64[BNPK_SAM_FIELDS, R], status) of the lines (starts, lens) of bnpk_line_split
+std::tuple<Tensor, Tensor> sam_columns(const Tensor &chunk, const Tensor &starts, const Tensor &lens) {
+    const Rows r = need_rows(chunk, starts, lens, c10::nullopt);
+    c10::cuda::CUDAGuard guard(chunk.device());
+    Tensor fields = torch::empty({BNPK_SAM_FIELDS, (int64_t)r.n_rows}, starts.options());
+    Tensor status = new_status(chunk);
+    check(r.call(bnpk_sam_columns, fields.data_ptr<int64_t>(), status.data_ptr<int64_t>(), cur_stream(chunk)),
+          "sam_columns");
+    return {fields, status};
+}
+
+// rows of CIGAR text: (op counts int32[R], reference lengths int64[R], status)
+std::tuple<Tensor, Tensor, Tensor> cigar_count(const Tensor &base, const Tensor &starts, const Tensor &lens) {
+    const Rows r = need_rows(base, starts, lens, c10::nullopt);
+    c10::cuda::CUDAGuard guard(base.device());
+    Tensor counts = torch::empty({(int64_t)r.n_rows}, lens.options());
+    Tensor ref_len = torch::empty({(int64_t)r.n_rows}, starts.options());
+    Tensor status = new_status(base);
+    check(r.call(bnpk_cigar_count, counts.data_ptr<int32_t>(), ref_len.data_ptr<int64_t>(), status.data_ptr<int64_t>(),
+                 cur_stream(base)),
+          "cigar_count");
+    return {counts, ref_len, status};
+}
+
+// the ops of rows of CIGAR text at offsets[r] .. offsets[r + 1]: (op uint8[total], length int64[total])
+std::tuple<Tensor, Tensor> cigar_unpack(const Tensor &base, const Tensor &starts, const Tensor &lens,
+                                        const Tensor &offsets, int64_t total) {
+    const Rows r = need_rows(base, starts, lens, c10::nullopt);
+    const int64_t *off = need_offsets(offsets, r.n_rows, base);
+    TORCH_CHECK(total >= 0, "bnpk: total must be >= 0");
+    c10::cuda::CUDAGuard guard(base.device());
+    Tensor op = torch::empty({total}, base.options());
+    Tensor length = torch::empty({total}, starts.options());
+    if (total == 0) return {op, length};
+    check(r.call(bnpk_cigar_unpack, off, op.data_ptr<uint8_t>(), length.data_ptr<int64_t>(), cur_stream(base)),
+          "cigar_unpack");
+    return {op, length};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bnpk, m) {
@@ -833,6 +872,9 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("bam_fields(Tensor chunk, Tensor starts, Tensor(a!) status) -> Tensor");
     m.def("bam_sequence(Tensor chunk, Tensor seq_start, Tensor offsets, int total) -> Tensor");
     m.def("bam_cigar(Tensor chunk, Tensor cigar_start, Tensor offsets, int total) -> (Tensor, Tensor)");
+    m.def("sam_columns(Tensor chunk, Tensor starts, Tensor lens) -> (Tensor, Tensor)");
+    m.def("cigar_count(Tensor base, Tensor starts, Tensor lens) -> (Tensor, Tensor, Tensor)");
+    m.def("cigar_unpack(Tensor base, Tensor starts, Tensor lens, Tensor offsets, int total) -> (Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
@@ -869,4 +911,7 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("bam_fields", &bam_fields);
     m.impl("bam_sequence", &bam_sequence);
     m.impl("bam_cigar", &bam_cigar);
+    m.impl("sam_columns", &sam_columns);
+    m.impl("cigar_count", &cigar_count);
+    m.impl("cigar_unpack", &cigar_unpack);
 }

@@ -116,6 +116,14 @@ class BamEntry(_Entries):
     _fields = ("chromosome", "name", "flag", "position", "mapq", "cigar_op", "cigar_length", "sequence", "quality")
 
 
+class SAMEntry(_Entries):
+    """datatypes/__init__.py:158-171: an alignment as SAM text.  name, chromosome, cigar, next_chromosome, sequence,
+    quality and extra (the optional tags, tabs included) are text views of the chunk; flag, position and next_position
+    (1-based, as written), mapq and length (TLEN) int64 CUDA tensors."""
+    _fields = ("name", "flag", "chromosome", "position", "mapq", "cigar", "next_chromosome", "next_position", "length",
+               "sequence", "quality", "extra")
+
+
 def _interval_field(field, value):
     """Interval, Bed6 and BedGraph fields: text columns (chromosome, name) as text, integer columns (start, stop, score)
     as int64 CUDA tensors, a bedGraph value as a CUDA tensor of its own dtype and strand as StrandEncoding codes."""

@@ -131,14 +131,18 @@ class Genome:
         return GenomicIntervals.from_intervals(intervals, self)
 
     def read_intervals(self, filename, stranded=False, stream=False, buffer_type=None) -> "GenomicIntervals":
-        """genome.py:211-261: a BED file, or the alignments of a BAM file (BamIntervalBuffer), read on the device and
-        placed on this genome (stream=False only)."""
+        """genome.py:211-261: a BED file, or the alignments of a BAM or SAM file (BamIntervalBuffer, SAMIntervalBuffer),
+        read on the device and placed on this genome (stream=False only)."""
         if stream:
             raise NotImplementedError("streamed genomes are not supported")
         from ..io.files import bnp_open, _suffix
-        if buffer_type is None and _suffix(str(filename))[0] == ".bam":
+        suffix = _suffix(str(filename))[0]
+        if buffer_type is None and suffix == ".bam":
             from ..io.bam import BamIntervalBuffer       # genome.py:258-259: alignments as intervals
             buffer_type = BamIntervalBuffer
+        if buffer_type is None and suffix == ".sam":
+            from ..io.sam import SAMIntervalBuffer
+            buffer_type = SAMIntervalBuffer
         if buffer_type is None and stranded:
             from ..io.delimited import Bed6Buffer
             buffer_type = Bed6Buffer

@@ -10,4 +10,5 @@ from .indexed_fasta import IndexedFasta, read_index, create_index, open_indexed
 from .delimited import DelimitedBuffer, BedBuffer, Bed6Buffer, BdgBuffer, GTFBuffer, GFFBuffer
 from .motifs import read_motif
 from .bam import BamBuffer, BamIntervalBuffer
-from . import bam
+from .sam import SAMBuffer, SAMIntervalBuffer
+from . import bam, sam

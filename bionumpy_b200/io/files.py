@@ -40,9 +40,12 @@ def _buffer_type_for(suffix):
     if suffix in (".gff", ".gff3"):
         from .delimited import GFFBuffer
         return GFFBuffer
+    if suffix == ".sam":
+        from .sam import SAMBuffer
+        return SAMBuffer
     raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
-                       f"(supported: .fq .fastq .fa .fasta .bed .bdg .gtf .gff .gff3 and their .gz forms, and .bam); "
-                       f"pass buffer_type=")
+                       f"(supported: .fq .fastq .fa .fasta .bed .bdg .gtf .gff .gff3 .sam and their .gz forms, and "
+                       f".bam); pass buffer_type=")
 
 
 def _suffix(path):
@@ -56,7 +59,8 @@ def _suffix(path):
 def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
     """files.py:85-182.  Reading ("r", "rb") gives an NpDataclassReader; writing ("w", "wb", "write") or appending
     ("a", "ab", "append") gives an NpBufferedWriter, which writes ``.gz`` files as BGZF.  ``.bdg`` (bedGraph) is
-    written only, ``.bam`` read only (as BGZF, whatever the suffix says).  BED is written with the buffer type named: ``bnp.open("x.bed", "w", buffer_type=BedBuffer)`` (or
+    written only, ``.sam`` read only (opening it for writing raises the RuntimeError it raised before SAM could be
+    read), ``.bam`` read only (as BGZF, whatever the suffix says).  BED is written with the buffer type named: ``bnp.open("x.bed", "w", buffer_type=BedBuffer)`` (or
     Bed6Buffer; either writes a record's own fields).  Opening ``.bed`` for writing by its suffix alone raises
     NotImplementedError, as it did before BED could be written, so code that relies on that keeps working."""
     if mode not in (None, "r", "rb") and mode not in WRITE_MODES:
@@ -66,6 +70,10 @@ def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
     if mode in WRITE_MODES and buffer_type is None and suffix == ".bam":      # BAM is read only
         raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
                            f"(supported: .fq .fastq .fa .fasta .bed .bdg and their .gz forms); pass buffer_type=")
+    if mode in WRITE_MODES and buffer_type is None and suffix == ".sam":      # SAM is read only
+        raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
+                           f"(supported: .fq .fastq .fa .fasta .bed .bdg .gtf .gff .gff3 and their .gz forms, and "
+                           f".bam); pass buffer_type=")
     if mode in WRITE_MODES and buffer_type is None and suffix in (".gtf", ".gff", ".gff3"):
         raise NotImplementedError(f"writing {suffix} is not supported: GTF and GFF are read only")
     if mode in WRITE_MODES and buffer_type is None and suffix == ".bed":

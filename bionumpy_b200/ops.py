@@ -963,3 +963,41 @@ def bam_cigar(chunk, cigar_start, offsets, total):
     check(lib().bnpk_bam_cigar(chunk_p, chunk.numel(), start_p, offsets_p, cigar_start.numel(), _pointer(op),
                                _pointer(length), stream_ptr()))
     return op, length
+
+
+@_on_device
+def sam_columns(chunk, starts, lens, status=None):
+    """bnpk_sam_columns: the 11 mandatory columns and the extra text of the lines (starts, lens) of ``chunk``.  Returns
+    (fields int64[SAM_FIELDS, R], status); text columns are chunk offsets and lengths, integers values (nv.SAM_F_*),
+    and the first fault is in status[ST_BAD_BASE] (ScanStatus.column_fault)."""
+    head, _ = _rows_args(chunk, starts, lens, status=status)
+    fields = torch.empty(nv.SAM_FIELDS, starts.numel(), dtype=torch.int64, device=chunk.device)
+    status = nv.new_status(chunk.device) if status is None else status
+    check(lib().bnpk_sam_columns(*head, _pointer(fields), _pointer(status), stream_ptr()))
+    return fields, status
+
+
+@_on_device
+def cigar_count(base, starts, lens, status=None):
+    """bnpk_cigar_count: (op counts int32[R], reference lengths int64[R], status) of the rows of CIGAR text; the first
+    invalid row is in status[ST_BAD_BASE] (ScanStatus.column_fault: row, 5, nv.BAD_CIGAR)."""
+    head, _ = _rows_args(base, starts, lens, status=status)
+    counts = torch.empty(starts.numel(), dtype=torch.int32, device=base.device)
+    ref_len = torch.empty(starts.numel(), dtype=torch.int64, device=base.device)
+    status = nv.new_status(base.device) if status is None else status
+    check(lib().bnpk_cigar_count(*head, _pointer(counts), _pointer(ref_len), _pointer(status), stream_ptr()))
+    return counts, ref_len, status
+
+
+@_on_device
+def cigar_unpack(base, starts, lens, offsets, total):
+    """bnpk_cigar_unpack: (op uint8[total] CigarOpEncoding codes, length int64[total]) of the rows of CIGAR text at
+    offsets[r] .. offsets[r + 1] (int64[R + 1], row_offsets of cigar_count's counts)."""
+    head, _ = _rows_args(base, starts, lens)
+    offsets_p = _pointer(offsets, "offsets", torch.int64, n=starts.numel() + 1)
+    op = torch.empty(total, dtype=torch.uint8, device=base.device)
+    length = torch.empty(total, dtype=torch.int64, device=base.device)
+    if total == 0:
+        return op, length
+    check(lib().bnpk_cigar_unpack(*head, offsets_p, _pointer(op), _pointer(length), stream_ptr()))
+    return op, length

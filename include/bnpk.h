@@ -639,6 +639,55 @@ int bnpk_bam_cigar(const uint8_t *chunk, size_t n, const int64_t *cigar_start, c
                    uint8_t *op, int64_t *length, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K16  SAM alignments (SAMBuffer, io/buffers/sam.py; SAMEntry, datatypes/__init__.py:158-171).
+ *
+ *   bnpk_sam_columns: the 11 mandatory tab-separated columns and the rest of every line (line_starts, line_lens) of
+ *     bnpk_line_split(lines_per_entry = 1).  One warp per line walks it in steps of 512 bytes (one aligned 16-byte
+ *     load per lane, bytes outside the line masked) and stops at the window that holds the 11th tab; a line of any
+ *     length is read.  fields[f * n_lines + r] for the BNPK_SAM_F_* below: QNAME, RNAME, CIGAR, RNEXT, SEQ, QUAL and
+ *     extra (everything after the 11th column's tab, tabs included; empty for a line of exactly 11 columns) as chunk
+ *     offset and length, FLAG, POS, MAPQ, PNEXT and TLEN as values (an optional '-' or '+' and 1 to 18 digits).  When
+ *     the first line ends in '\r', a '\r' that ends a line is not part of its last column.  The first fault is
+ *     atomicMin-ed into status[BNPK_ST_BAD_BASE] (pre-initialised): fault_column(line, columns, BNPK_BAD_COLUMNS) for a
+ *     line of fewer than 11 columns (every field of it is then empty), else fault_column(line, column, BNPK_BAD_INT).
+ *   bnpk_cigar_count: for every row of CIGAR text base[starts[r] .. + lens[r]), counts[r] = its op count (int32) and
+ *     ref_len[r] = the summed lengths of its M, D, N, = and X ops.  Valid text is "*" (no ops) or one or more ops of 1
+ *     to 9 digits and one of MIDNSHP=X; any other row gets 0 and 0 and is atomicMin-ed into status[BNPK_ST_BAD_BASE]
+ *     as fault_column(r, 5, BNPK_BAD_CIGAR).  One thread per row.
+ *   bnpk_cigar_unpack: the ops of every row as op = the CigarOpEncoding code (the index in "MIDNSHP=X", uint8) and
+ *     length (int64) at offsets[r] .. offsets[r + 1] (offsets = bnpk_row_offsets of counts); at most offsets[r + 1] -
+ *     offsets[r] ops of a row are written, whatever its text.  One thread per row.
+ * ------------------------------------------------------------------------------------- */
+#define BNPK_BAD_CIGAR          6  /* CIGAR text that is not "*" or ops of 1-9 digits and MIDNSHP=X */
+#define BNPK_SAM_F_NAME_START   0
+#define BNPK_SAM_F_NAME_LEN     1
+#define BNPK_SAM_F_RNAME_START  2
+#define BNPK_SAM_F_RNAME_LEN    3
+#define BNPK_SAM_F_CIGAR_START  4
+#define BNPK_SAM_F_CIGAR_LEN    5
+#define BNPK_SAM_F_RNEXT_START  6
+#define BNPK_SAM_F_RNEXT_LEN    7
+#define BNPK_SAM_F_SEQ_START    8
+#define BNPK_SAM_F_SEQ_LEN      9
+#define BNPK_SAM_F_QUAL_START   10
+#define BNPK_SAM_F_QUAL_LEN     11
+#define BNPK_SAM_F_EXTRA_START  12
+#define BNPK_SAM_F_EXTRA_LEN    13
+#define BNPK_SAM_F_FLAG         14
+#define BNPK_SAM_F_POS          15   /* 1-based, as written                                         */
+#define BNPK_SAM_F_MAPQ         16
+#define BNPK_SAM_F_PNEXT        17
+#define BNPK_SAM_F_TLEN         18
+#define BNPK_SAM_FIELDS         19
+
+int bnpk_sam_columns(const uint8_t *chunk, size_t n, const int64_t *line_starts, const int32_t *line_lens,
+                     size_t n_lines, int64_t *fields, int64_t *status, void *stream);
+int bnpk_cigar_count(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
+                     int32_t *counts, int64_t *ref_len, int64_t *status, void *stream);
+int bnpk_cigar_unpack(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens,
+                      size_t n_rows, const int64_t *offsets, uint8_t *op, int64_t *length, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Host-buffer entry point (end-to-end): the call a reader loop makes with a chunk that is
  * still in host memory.  Copies `chunk_host` (pinned or pageable) to the device in slices on
  * a private copy stream, overlapping each slice's H2D with the fused count of the previous
