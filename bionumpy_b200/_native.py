@@ -37,6 +37,9 @@ BAM_BAD_BLOCK_SIZE, BAM_BAD_REF_ID, BAM_BAD_NAME, BAM_BAD_SIZES, BAM_BAD_CIGAR_O
  BAM_F_SEQ_START, BAM_F_L_SEQ, BAM_F_QUAL_START, BAM_F_REF_LEN) = range(12)
 BAM_FIELDS = 12
 BAD_CIGAR = 6
+BAD_FLOAT = 7
+OP_DIV = 14
+POW5_MIN, POW5_MAX = -342, 308
 (SAM_F_NAME_START, SAM_F_NAME_LEN, SAM_F_RNAME_START, SAM_F_RNAME_LEN, SAM_F_CIGAR_START, SAM_F_CIGAR_LEN,
  SAM_F_RNEXT_START, SAM_F_RNEXT_LEN, SAM_F_SEQ_START, SAM_F_SEQ_LEN, SAM_F_QUAL_START, SAM_F_QUAL_LEN, SAM_F_EXTRA_START,
  SAM_F_EXTRA_LEN, SAM_F_FLAG, SAM_F_POS, SAM_F_MAPQ, SAM_F_PNEXT, SAM_F_TLEN) = range(19)
@@ -113,6 +116,9 @@ SIGNATURES = {
     "bnpk_sam_columns": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
     "bnpk_cigar_count": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
     "bnpk_cigar_unpack": (_i, [_vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "bnpk_parse_float": (_i, [_vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _vp]),
+    "bnpk_track_f64_reduce": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "bnpk_track_f64_combine": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
 

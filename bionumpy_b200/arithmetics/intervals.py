@@ -8,7 +8,10 @@
                                   (bnpk_rows_equal_prev); one synchronisation.
   GenomicRunLengthArray         : runs on the device; indexing by intervals gives a lazy ragged result whose per-row
                                   max / min / sum / mean / any run fused over the runs (bnpk_runs_reduce) and whose
-                                  values, when asked for, are gathered by bnpk_runs_extract."""
+                                  values, when asked for, are gathered by bnpk_runs_extract.
+  FloatRunLengthArray           : the same with float64 values: fused reductions by bnpk_track_f64_reduce (sums with
+                                  the same bits on every call), operators by bnpk_track_f64_combine, and the gathers and
+                                  bedGraph rows of the integer kernels through an int64 view of the values' bits."""
 import numpy as np
 import torch
 
@@ -197,16 +200,26 @@ class GenomicRunLengthArray:
         a = self.to_array().cpu().numpy()
         return a.astype(dtype) if dtype is not None else a
 
+    def _reduce_rows(self, q_start, q_stop, mode):
+        """The reduction ``mode`` (nv.RUNS_*) of the track over every query [q_start, q_stop): max and min in the
+        track's dtype, the sum as the kernel gives it, any as bool.  The one place the reductions reach a kernel."""
+        if mode == nv.RUNS_MAX and self.dtype == torch.bool:
+            mode = nv.RUNS_ANY                  # the largest of bool values
+        out = ops.runs_reduce(self._events, self._values64(), q_start, q_stop, mode)
+        if mode == nv.RUNS_ANY:
+            return out != 0
+        return self._cast(out) if mode != nv.RUNS_SUM else out
+
     def _reduce(self, mode):
         dev = self._events.device
         q0 = torch.zeros(1, dtype=torch.int64, device=dev)
-        return ops.runs_reduce(self._events, self._values64(), q0, self._events[-1:].contiguous(), mode)[0]
+        return self._reduce_rows(q0, self._events[-1:].contiguous(), mode)[0]
 
     def max(self, axis=None, **kwargs):
-        return self._cast(self._reduce(nv.RUNS_ANY if self.dtype == torch.bool else nv.RUNS_MAX))
+        return self._reduce(nv.RUNS_MAX)
 
     def min(self, axis=None, **kwargs):
-        return self._cast(self._reduce(nv.RUNS_MIN))
+        return self._reduce(nv.RUNS_MIN)
 
     def sum(self, axis=None, **kwargs):
         return self._reduce(nv.RUNS_SUM)
@@ -215,7 +228,7 @@ class GenomicRunLengthArray:
         return self._reduce(nv.RUNS_SUM).to(torch.float64) / self._events[-1].to(torch.float64)
 
     def any(self, axis=None, **kwargs):
-        return self._reduce(nv.RUNS_ANY) != 0
+        return self._reduce(nv.RUNS_ANY)
 
     def __getitem__(self, idx):
         if isinstance(idx, (int, np.integer)):
@@ -254,7 +267,7 @@ class GenomicRunLengthArray:
         i0, i1 = bounds.cpu().tolist()
         i1 = max(i1, i0 + 1)
         events = (self._events[i0:i1 + 1] - a).clamp_(0, b - a)
-        return GenomicRunLengthArray(events, self._values[i0:i1], b - a)
+        return type(self)(events, self._values[i0:i1], b - a)
 
     def to_bedgraph(self, sequence_name):
         """The runs as BedGraph rows on contig ``sequence_name`` (arithmetics/intervals.py:119-121): every run as it
@@ -316,6 +329,50 @@ def _add_operators(cls):
 
 _add_operators(GenomicRunLengthArray)
 
+
+class FloatRunLengthArray(GenomicRunLengthArray):
+    """A track of float64 runs.  float16 and float32 values (and integer ones) are converted to float64; neighbouring
+    runs are one run only when their values are bitwise equal, so -0.0 next to +0.0 stays two runs and NaN runs are
+    never merged with a different NaN.  max / min / sum / mean / any follow NumPy: a NaN in a range makes max, min, sum
+    and mean NaN, any counts it as true, and an empty range gives -inf, +inf, 0.0, NaN and False.  Sums are rounded
+    per run and added in a fixed order: the same bits on every call."""
+
+    def __init__(self, events, values, size=None):
+        if values.is_complex():
+            raise TypeError(f"run-length values must be real, not {values.dtype}")
+        self._events = events
+        self._values = values.to(torch.float64)
+        self._size = None if size is None else int(size)
+
+    def _values64(self):
+        return self._values.contiguous().view(torch.int64)
+
+    def _cast(self, t):
+        return t.view(torch.float64)
+
+    def astype(self, dtype):
+        raise TypeError("float tracks are not converted to another type")
+
+    def _reduce_rows(self, q_start, q_stop, mode):
+        out = ops.track_f64_reduce(self._events, self._values.contiguous(), q_start, q_stop, mode)
+        return out != 0 if mode == nv.RUNS_ANY else out
+
+
+def _is_float_track(x):
+    return isinstance(getattr(x, "_global", x), FloatRunLengthArray)
+
+
+def _truediv(self, other):
+    return np.true_divide(self, other) if _is_float_track(self) or _is_float_track(other) else NotImplemented
+
+
+def _rtruediv(self, other):
+    return np.true_divide(other, self) if _is_float_track(self) or _is_float_track(other) else NotImplemented
+
+
+GenomicRunLengthArray.__truediv__ = _truediv
+GenomicRunLengthArray.__rtruediv__ = _rtruediv
+
 # ufunc -> the kernel's operator; the logical ones first map each value to (value != 0)
 TRACK_UFUNCS = {np.add: nv.OP_ADD, np.subtract: nv.OP_SUB, np.multiply: nv.OP_MUL, np.bitwise_and: nv.OP_AND,
                 np.bitwise_or: nv.OP_OR, np.bitwise_xor: nv.OP_XOR, np.minimum: nv.OP_MIN, np.maximum: nv.OP_MAX,
@@ -346,6 +403,8 @@ def track_ufunc(ufunc, method, inputs, kwargs):
     sizes raise ValueError; what NumPy refuses (bool - bool, -bool) raises its TypeError."""
     if method != "__call__" or kwargs:
         return None
+    if any(isinstance(x, FloatRunLengthArray) for x in inputs):
+        return float_track_ufunc(ufunc, inputs)
     if len(inputs) == 1:
         (x,) = inputs
         if not isinstance(x, GenomicRunLengthArray):
@@ -409,6 +468,60 @@ def track_ufunc(ufunc, method, inputs, kwargs):
     return GenomicRunLengthArray(starts[:n + 1], values, size)
 
 
+FLOAT_UFUNCS = {np.add: nv.OP_ADD, np.subtract: nv.OP_SUB, np.multiply: nv.OP_MUL, np.true_divide: nv.OP_DIV,
+                np.minimum: nv.OP_MIN, np.maximum: nv.OP_MAX, np.equal: nv.OP_EQ, np.not_equal: nv.OP_NE,
+                np.less: nv.OP_LT, np.less_equal: nv.OP_LE, np.greater: nv.OP_GT, np.greater_equal: nv.OP_GE}
+_COMPARISONS = (np.equal, np.not_equal, np.less, np.less_equal, np.greater, np.greater_equal)
+
+
+def float_track_ufunc(ufunc, inputs):
+    """``ufunc(*inputs)`` where an operand is a FloatRunLengthArray, or None for a call the runs do not serve.  The
+    other operand is a float track, an integer or bool track (its values converted to float64 as NumPy converts them)
+    or an int or float scalar.  np.negative flips the sign bit, np.logical_not(x) is x == 0; FLOAT_UFUNCS run on the
+    runs (bnpk_track_f64_combine, one synchronisation): comparisons give bool tracks, the others float tracks.  Tracks
+    of different sizes raise ValueError."""
+    if len(inputs) == 1:
+        (x,) = inputs
+        if ufunc is np.negative:
+            flipped = x._values.contiguous().view(torch.int64) ^ torch.iinfo(torch.int64).min
+            return FloatRunLengthArray(x._events, flipped.view(torch.float64), x._size)
+        if ufunc is np.logical_not:
+            return float_track_ufunc(np.equal, (x, 0.0))
+        return None
+    if len(inputs) != 2 or ufunc not in FLOAT_UFUNCS:
+        return None
+    scalar = (bool, int, float, np.bool_, np.integer, np.floating)
+    if not all(isinstance(x, GenomicRunLengthArray) or isinstance(x, scalar) for x in inputs):
+        return None
+    if any(isinstance(x, (int, np.integer)) and abs(int(x)) >= 2 ** 1024 for x in inputs):
+        return None
+    tracks = [x for x in inputs if isinstance(x, GenomicRunLengthArray)]
+    size = len(tracks[0])
+    if any(len(t) != size for t in tracks):
+        raise ValueError(f"tracks of sizes {len(tracks[0])} and {len(tracks[1])} cannot be combined")
+    dev = tracks[0]._events.device
+    runs = []
+    for x in inputs:
+        if isinstance(x, GenomicRunLengthArray):
+            runs.append((x._events, x._values.to(torch.float64)))
+        else:
+            runs.append((torch.arange(2, dtype=torch.int64, device=dev) * size,      # made on the device: no copy
+                         torch.full((1,), float(x), dtype=torch.float64, device=dev)))
+    (a_starts, a_values), (b_starts, b_values) = runs
+    if size == 0:          # a size-0 track has one empty run; the kernel needs both sides alike
+        a_starts, a_values = a_starts[:1], a_values[:0]
+        b_starts, b_values = b_starts[:1], b_values[:0]
+    starts, values, n_runs = ops.track_f64_combine(a_starts.contiguous(), a_values.contiguous(),
+                                                   b_starts.contiguous(), b_values.contiguous(), FLOAT_UFUNCS[ufunc])
+    n = int(n_runs.item())
+    if size == 0:
+        starts, values, n = torch.zeros(2, dtype=torch.int64, device=dev), torch.zeros(1, dtype=torch.float64,
+                                                                                      device=dev), 1
+    if ufunc in _COMPARISONS:
+        return GenomicRunLengthArray(starts[:n + 1], values[:n] != 0, size)
+    return FloatRunLengthArray(starts[:n + 1], values[:n], size)
+
+
 class RunsRaggedArray(LazyRaggedArray):
     """``track[intervals]``: one row per interval, the track's values over [start, stop) clipped to [0, len(track)),
     the same rows for the fused reductions and the gathered values (a part of an interval outside the track has no
@@ -431,17 +544,17 @@ class RunsRaggedArray(LazyRaggedArray):
         return self._track._cast(out)
 
     def _reduce(self, mode):
-        return ops.runs_reduce(self._track._events, self._track._values64(), self._q_start, self._q_stop, mode)
+        return self._track._reduce_rows(self._q_start, self._q_stop, mode)
 
     def max(self, axis=None, **kwargs):
         if axis not in (-1, 1):
             return super().max(axis, **kwargs)
-        return self._track._cast(self._reduce(nv.RUNS_ANY if self.dtype == torch.bool else nv.RUNS_MAX))
+        return self._reduce(nv.RUNS_MAX)
 
     def min(self, axis=None, **kwargs):
         if axis not in (-1, 1):
             return super().min(axis, **kwargs)
-        return self._track._cast(self._reduce(nv.RUNS_MIN))
+        return self._reduce(nv.RUNS_MIN)
 
     def sum(self, axis=None, **kwargs):
         if axis not in (-1, 1):
@@ -456,7 +569,7 @@ class RunsRaggedArray(LazyRaggedArray):
     def any(self, axis=None, **kwargs):
         if axis not in (-1, 1):
             return super().any(axis, **kwargs)
-        return self._reduce(nv.RUNS_ANY) != 0
+        return self._reduce(nv.RUNS_ANY)
 
     @property
     def dtype(self):

@@ -820,6 +820,68 @@ std::tuple<Tensor, Tensor> cigar_unpack(const Tensor &base, const Tensor &starts
     return {op, length};
 }
 
+// rows of decimal text: (values float64[R], status), each equal to Python's float(text); pow5_table int64[2 * 651]
+std::tuple<Tensor, Tensor> parse_float(const Tensor &base, const Tensor &starts, const Tensor &lens, int64_t column,
+                                       const Tensor &pow5_table) {
+    const Rows r = need_rows(base, starts, lens, c10::nullopt);
+    need(pow5_table, torch::kInt64, "pow5_table", base);
+    TORCH_CHECK(pow5_table.numel() == 2 * 651, "bnpk: pow5_table must have 2 * 651 entries");
+    c10::cuda::CUDAGuard guard(base.device());
+    Tensor out = torch::empty({(int64_t)r.n_rows}, starts.options().dtype(torch::kFloat64));
+    Tensor status = new_status(base);
+    check(r.call(bnpk_parse_float, (int)column, (const uint64_t *)pow5_table.data_ptr<int64_t>(),
+                 out.data_ptr<double>(), status.data_ptr<int64_t>(), cur_stream(base)),
+          "parse_float");
+    return {out, status};
+}
+
+void need_f64_track(const Tensor &run_starts, const Tensor &values, const Tensor &on = Tensor()) {
+    need(run_starts, torch::kInt64, "run_starts", on);
+    need(values, torch::kFloat64, "values", run_starts);
+    TORCH_CHECK(run_starts.numel() == values.numel() + 1, "bnpk: a track is R values and R + 1 run starts");
+}
+
+Tensor track_f64_reduce(const Tensor &run_starts, const Tensor &values, const Tensor &q_start, const Tensor &q_stop,
+                        int64_t mode) {
+    need_f64_track(run_starts, values);
+    TORCH_CHECK(values.numel() >= 1, "bnpk: a track is R >= 1 values and R + 1 run starts");
+    need(q_start, torch::kInt64, "q_start", run_starts);
+    need(q_stop, torch::kInt64, "q_stop", run_starts);
+    TORCH_CHECK(q_start.numel() == q_stop.numel(), "bnpk: q_start and q_stop differ in length");
+    c10::cuda::CUDAGuard guard(run_starts.device());
+    const int64_t n = q_start.numel();
+    const int64_t n_chunks = (n + values.numel()) / 16 + 1024;
+    Tensor out = torch::empty({n}, values.options());
+    Tensor scratch = torch::empty({3 * n + 1}, run_starts.options());
+    Tensor partial = torch::empty({2 * n_chunks}, values.options());
+    Tensor ws = new_workspace(run_starts, (size_t)std::max<int64_t>(n, 1));
+    check(bnpk_track_f64_reduce(run_starts.data_ptr<int64_t>(), values.data_ptr<double>(), (size_t)values.numel(),
+                                q_start.data_ptr<int64_t>(), q_stop.data_ptr<int64_t>(), (size_t)n, (int)mode,
+                                out.data_ptr<double>(), scratch.data_ptr<int64_t>(), partial.data_ptr<double>(),
+                                (size_t)n_chunks, ws.data_ptr<uint8_t>(), (size_t)ws.numel(), cur_stream(run_starts)),
+          "track_f64_reduce");
+    return out;
+}
+
+std::tuple<Tensor, Tensor, Tensor> track_f64_combine(const Tensor &a_starts, const Tensor &a_values,
+                                                     const Tensor &b_starts, const Tensor &b_values, int64_t op) {
+    need_f64_track(a_starts, a_values);
+    need_f64_track(b_starts, b_values, a_starts);
+    c10::cuda::CUDAGuard guard(a_starts.device());
+    const int64_t n = a_values.numel() + b_values.numel();
+    Tensor starts = torch::empty({n + 1}, a_starts.options());
+    Tensor values = torch::empty({std::max<int64_t>(n, 1)}, a_values.options());
+    Tensor n_runs = torch::empty({1}, a_starts.options());
+    Tensor ws = new_workspace(a_starts, (size_t)std::max<int64_t>(n, 1));
+    check(bnpk_track_f64_combine(a_starts.data_ptr<int64_t>(), a_values.data_ptr<double>(), (size_t)a_values.numel(),
+                                 b_starts.data_ptr<int64_t>(), b_values.data_ptr<double>(), (size_t)b_values.numel(),
+                                 (int)op, starts.data_ptr<int64_t>(), values.data_ptr<double>(),
+                                 n_runs.data_ptr<int64_t>(), ws.data_ptr<uint8_t>(), (size_t)ws.numel(),
+                                 cur_stream(a_starts)),
+          "track_f64_combine");
+    return {starts, values, n_runs};
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bnpk, m) {
@@ -875,6 +937,10 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("sam_columns(Tensor chunk, Tensor starts, Tensor lens) -> (Tensor, Tensor)");
     m.def("cigar_count(Tensor base, Tensor starts, Tensor lens) -> (Tensor, Tensor, Tensor)");
     m.def("cigar_unpack(Tensor base, Tensor starts, Tensor lens, Tensor offsets, int total) -> (Tensor, Tensor)");
+    m.def("parse_float(Tensor base, Tensor starts, Tensor lens, int column, Tensor pow5_table) -> (Tensor, Tensor)");
+    m.def("track_f64_reduce(Tensor run_starts, Tensor values, Tensor q_start, Tensor q_stop, int mode) -> Tensor");
+    m.def("track_f64_combine(Tensor a_starts, Tensor a_values, Tensor b_starts, Tensor b_values, int op) "
+          "-> (Tensor, Tensor, Tensor)");
 }
 
 TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
@@ -914,4 +980,7 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("sam_columns", &sam_columns);
     m.impl("cigar_count", &cigar_count);
     m.impl("cigar_unpack", &cigar_unpack);
+    m.impl("parse_float", &parse_float);
+    m.impl("track_f64_reduce", &track_f64_reduce);
+    m.impl("track_f64_combine", &track_f64_combine);
 }

@@ -185,8 +185,9 @@ class Bed6(_IntervalEntries):
 
 
 class BedGraph(_IntervalEntries):
-    """datatypes/__init__.py:27-31: chromosome, start, stop and value.  The value is an integer (or bool) tensor here:
-    the tracks it comes from hold integers, and a float value cannot be written."""
+    """datatypes/__init__.py:27-31: chromosome, start, stop and value.  The value is a tensor of its own dtype: float64
+    when read from a bedGraph file (BedGraphBuffer) or taken from a float track, integer or bool from integer tracks.
+    Only integer and bool values can be written."""
     _fields = ("chromosome", "start", "stop", "value")
 
 

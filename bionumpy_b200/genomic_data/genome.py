@@ -12,8 +12,8 @@ import torch
 
 from .. import _native as nv
 from .. import ops
-from ..arithmetics.intervals import (GenomicRunLengthArray, RunsRaggedArray, _add_operators, _device, _int64,
-                                     coverage_runs, to_device, track_ufunc)
+from ..arithmetics.intervals import (FloatRunLengthArray, GenomicRunLengthArray, RunsRaggedArray, _add_operators,
+                                     _device, _int64, _rtruediv, _truediv, coverage_runs, to_device, track_ufunc)
 from ..datatypes import BedGraph, Interval, replace
 from ..encoded_array import BaseEncoding, EncodedArray, EncodedRaggedArray
 from ..rows import RowView
@@ -147,6 +147,84 @@ class Genome:
             from ..io.delimited import Bed6Buffer
             buffer_type = Bed6Buffer
         return self.get_intervals(bnp_open(filename, buffer_type=buffer_type).read(), stranded)
+
+    def get_track(self, bedgraph) -> "GenomicArray":
+        """genome.py:127-152: the GenomicArray of BedGraph rows, placed as GenomicIntervals.from_intervals places
+        intervals (an unknown name raises KeyError, a row with stop < start or past its contig ValueError naming it, and
+        rows on contigs the genome leaves out are dropped).  The rows may come in any order: they are sorted by global
+        start on the device.  Rows that overlap raise ValueError naming the first pair (the reference assumes sorted,
+        disjoint rows).  Empty rows add nothing; the positions no row covers are +0.0; neighbouring runs whose values
+        are bitwise equal are one run.  Float values give a float track, integer or bool values an integer or bool one.
+
+        The lookup, bounds, overlap check and run count are read back in one synchronisation; the library launches
+        two kernels (the name lookup and the bounds check), the runs are built by torch ops.
+
+        >>> bedgraph = BedGraph(['chr1', 'chr1', 'chr2'], [0, 10, 0], [5, 15, 5], [1, 2, 3])
+        >>> Genome.from_dict({'chr1': 20, 'chr2': 10}).get_track(bedgraph)
+        chr1: [1 1 1 1 1 0 0 0 0 0 2 2 2 2 2 0 0 0 0 0]
+        chr2: [3 3 3 3 3 0 0 0 0 0]"""
+        names, text, name_offsets, offset, size = self._name_table()
+        dev, G = text.device, self.size
+        value = bedgraph.value if isinstance(bedgraph.value, torch.Tensor) else torch.as_tensor(np.asarray(bedgraph.value))
+        value = value.to(dev)
+        is_float = value.is_floating_point()
+        bits = value.to(torch.float64).view(torch.int64) if is_float else value.to(torch.int64)
+        zero = torch.zeros(1, dtype=torch.int64, device=dev)
+        start, stop = _int64(bedgraph.start, dev), _int64(bedgraph.stop, dev)
+        if start.numel() == 0 or G == 0:
+            events = torch.cat([zero, torch.full((1,), G, dtype=torch.int64, device=dev)])
+            return self._track_of(events, zero, value.dtype)
+        rows = RowView(bedgraph.chromosome)
+        ids, st_names = ops.name_lookup(rows.base, rows.starts, rows.lens, text, name_offsets)
+        _, g_start, g_stop, st_rows = ops.interval_events(start, stop, ids, offset, size, keys=False, glob=True)
+        keep = (offset[ids.clamp(min=0).to(torch.int64)] >= 0) & (g_stop > g_start)
+        # the kept rows by global start, then every other row as an empty row at the end, then one more: row i
+        # contributes the gap [e[i - 1], s[i]) of +0.0 and its own run [s[i], e[i])
+        end = torch.full((1,), G, dtype=torch.int64, device=dev)
+        order = torch.sort(torch.where(keep, g_start, G), stable=True).indices
+        s = torch.cat([torch.where(keep, g_start, G)[order], end])
+        e = torch.cat([torch.where(keep, g_stop, G)[order], end])
+        v = torch.cat([bits[order], zero])
+        prev_e, prev_v = torch.cat([zero, e[:-1]]), torch.cat([zero, v[:-1]])
+        index = torch.arange(s.numel(), dtype=torch.int64, device=dev)
+        first_overlap = torch.where(prev_e > s, index, s.numel()).min().reshape(1)       # s.numel(): none
+        first, gap = index == 0, s > prev_e
+        # a run starts where the value's bits differ from those of the non-empty piece before it
+        emit_gap = gap & (first | (prev_v != 0))
+        emit_row = (e > s) & torch.where(gap, v != 0, first | (v != prev_v))
+        emit = torch.stack([emit_gap, emit_row], 1).reshape(-1)
+        st_names, st_rows, n_runs, bad = ops.read_back(st_names, st_rows, emit.sum(), first_overlap)
+        if st_names.fault is not None:
+            raise KeyError(bedgraph.chromosome[st_names.fault].to_string())
+        if st_rows.fault is not None:
+            row = st_rows.fault
+            name = bedgraph.chromosome[row].to_string()
+            raise ValueError(f"bedGraph row {row} ({name}:{int(start[row])}-{int(stop[row])}) is not inside the "
+                             f"contig ({self._all[name]} bases)")
+        if bad < s.numel():
+            a, b = order[bad - 1:bad + 1].cpu().tolist()
+            raise ValueError(f"bedGraph rows {a} and {b} overlap: {bedgraph.chromosome[a].to_string()}:"
+                             f"{int(start[a])}-{int(stop[a])} and {bedgraph.chromosome[b].to_string()}:"
+                             f"{int(start[b])}-{int(stop[b])}")
+        picked = torch.nonzero_static(emit, size=n_runs).reshape(-1)
+        run_starts = torch.stack([prev_e, s], 1).reshape(-1)[picked]
+        run_bits = torch.stack([torch.zeros_like(v), v], 1).reshape(-1)[picked]
+        return self._track_of(torch.cat([run_starts, end]), run_bits, value.dtype)
+
+    def _track_of(self, events, bits, dtype):
+        """A GenomicArray of runs whose values are int64 (their bits, for a float dtype)."""
+        if dtype.is_floating_point:
+            return GenomicArray._of(FloatRunLengthArray(events, bits.view(torch.float64), self.size), self)
+        values = bits != 0 if dtype == torch.bool else bits
+        return GenomicArray._of(GenomicRunLengthArray(events, values, self.size), self)
+
+    def read_track(self, filename, stream=False) -> "GenomicArray":
+        """genome.py:154-179: a bedGraph file (.bdg, .bdg.gz) read on the device and made a GenomicArray by get_track
+        (stream=False only)."""
+        if stream:
+            raise NotImplementedError("streamed genomes are not supported")
+        from ..io.files import bnp_open
+        return self.get_track(bnp_open(filename).read())
 
     def read_annotation(self, filename) -> "GenomicAnnotation":
         """genome.py:390-422: a GTF or GFF file read on the device, with its genes, transcripts and exons placed on
@@ -394,15 +472,15 @@ class GenomicArray:
         i0, i1 = torch.cat([i0, i1]).cpu().tolist()
         i1 = max(i1, i0 + 1)
         events = (self._global._events[i0:i1 + 1] - off).clamp_(0, size)
-        return GenomicRunLengthArray(events, self._global.values[i0:i1], size)
+        return type(self._global)(events, self._global.values[i0:i1], size)
 
     def to_dict(self):
         return {name: self._contig(name) for name in self._genome._sizes}
 
     def get_data(self):
         """genomic_track.py:199-218: a bool track as the Interval rows where it is True (GenomicIntervals.from_track),
-        any other track as a BedGraph of every run, cut at contig borders, with the track's values; one
-        synchronisation."""
+        any other track as a BedGraph of every run, cut at contig borders, with the track's values (float64 for a
+        float track); one synchronisation."""
         if self.dtype == torch.bool:
             return GenomicIntervals.from_track(self).get_data()
         genome = self._genome
@@ -422,6 +500,7 @@ class GenomicArray:
 
 
 _add_operators(GenomicArray)
+GenomicArray.__truediv__, GenomicArray.__rtruediv__ = _truediv, _rtruediv
 
 __all__ = ["Genome", "GenomicIntervals", "GenomicArray", "GenomicAnnotation", "Genes", "Transcripts", "Exons",
            "ignore_underscores", "keep_all"]

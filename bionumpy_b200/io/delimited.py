@@ -20,7 +20,9 @@ from .exceptions import FormatException, IncompleteEntryException
 _FAULTS = {nv.BAD_TABS: "Irregular number of delimiters per line",
            nv.BAD_COLUMNS: "Too few columns for the record type",
            nv.BAD_INT: "Invalid integer (an optional sign and 1 to 18 digits)",
-           nv.BAD_STRAND: "Invalid strand (one of '+', '-', '.')"}
+           nv.BAD_STRAND: "Invalid strand (one of '+', '-', '.')",
+           nv.BAD_FLOAT: "Invalid number ([+-]? (digits ['.' digits?] | '.' digits) ([eE] [+-]? digits)?, at most 19 "
+                         "significant digits; nan and inf are not read)"}
 
 
 class DelimitedBuffer:
@@ -134,13 +136,54 @@ class Bed6Buffer(DelimitedBuffer):
 
 
 class BdgBuffer(DelimitedBuffer):
-    """bedGraph: chromosome, start, stop and an integer value.  Written only: the reference reads bedGraph values as
-    floats, and this package has no float tracks."""
+    """bedGraph for writing: chromosome, start, stop and an integer value (a float value cannot be written yet).  It
+    does not read: BedGraphBuffer reads bedGraph, with float64 values."""
     dataclass = BedGraph
 
     @classmethod
     def from_raw_buffer(cls, chunk, header_data=None):
-        raise NotImplementedError("reading bedGraph is not supported: its values are floats")
+        raise NotImplementedError("BdgBuffer writes bedGraph; read it with BedGraphBuffer")
+
+
+class BedGraphBuffer(BdgBuffer):
+    """bedGraph read on the device (delimited_buffers.py BedGraphBuffer): chromosome, start, stop and a float64 value.
+    The columns are read as a BED chunk's are, then the value column's text is parsed by bnpk_parse_float into the same
+    status block, so a chunk takes the two synchronisations of a BED chunk.  Each value equals Python's float(text);
+    the grammar is [+-]? (digits ['.' digits?] | '.' digits) ([eE] [+-]? digits)? of at most 19 significant digits,
+    so nan, inf and longer significands raise FormatException naming the line.  Leading ``#``, ``track`` and
+    ``browser`` lines are the header."""
+    _kinds = (nv.COL_TEXT, nv.COL_INT, nv.COL_INT, nv.COL_TEXT)
+
+    @classmethod
+    def read_header(cls, file_object):
+        header = []
+        for line in file_object:
+            if not (line.startswith(b"#") or line.startswith(b"track") or line.startswith(b"browser")):
+                file_object.seek(-len(line), 1)
+                break
+            header.append(line.decode("utf-8"))
+        return "".join(header)
+
+    @classmethod
+    def from_raw_buffer(cls, chunk, header_data=None):
+        from .decimal import pow5_table
+        chunk = _to_device_bytes(chunk)
+        n_lines = ops.count_byte(chunk, 10) if chunk.numel() else 0
+        if n_lines == 0:
+            raise IncompleteEntryException("No complete line in the buffer. Try increasing chunk_size.")
+        starts, lens, _ = ops.line_split(chunk, 1, 0, 0, ord(cls.COMMENT), False, 0, max_rows=n_lines)
+        cols, status = ops.delimited_columns(chunk, starts, lens, cls._kinds)
+        # a line without a value column leaves its view unwritten: keep the parse inside the chunk (the column fault
+        # of such a line is smaller than any value fault of it)
+        v_start = cols[3][0].clamp(0, chunk.numel())
+        v_lens = torch.minimum(cols[3][1].clamp(min=0).to(torch.int64), chunk.numel() - v_start).to(torch.int32)
+        values, _ = ops.parse_float(chunk, v_start, v_lens, 3, pow5_table(chunk.device), status)
+        st, last_end = ops.read_back(status, starts[-1:] + lens[-1:])
+        if st.fault is not None:
+            line, col, kind = st.column_fault()
+            raise FormatException(f"{_FAULTS.get(kind, 'Invalid line')} (column {col})", line_number=line)
+        data = chunk[:last_end + 1]
+        return cls(data, n_lines, [FieldView(data, cols[0][1], cols[0][0]), cols[1], cols[2], values])
 
 
 _GTF_KINDS = (nv.COL_TEXT, nv.COL_TEXT, nv.COL_TEXT, nv.COL_INT, nv.COL_INT, nv.COL_TEXT, nv.COL_STRAND, nv.COL_TEXT,

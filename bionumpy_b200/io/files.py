@@ -56,10 +56,17 @@ def _suffix(path):
     return suffix, is_gzip
 
 
+def _read_buffer_type_for(suffix):
+    if suffix == ".bdg":
+        from .delimited import BedGraphBuffer
+        return BedGraphBuffer
+    return _buffer_type_for(suffix)
+
+
 def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
     """files.py:85-182.  Reading ("r", "rb") gives an NpDataclassReader; writing ("w", "wb", "write") or appending
     ("a", "ab", "append") gives an NpBufferedWriter, which writes ``.gz`` files as BGZF.  ``.bdg`` (bedGraph) is
-    written only, ``.sam`` read only (opening it for writing raises the RuntimeError it raised before SAM could be
+    read with float64 values (BedGraphBuffer) and written with integer values (BdgBuffer), ``.sam`` read only (opening it for writing raises the RuntimeError it raised before SAM could be
     read), ``.bam`` read only (as BGZF, whatever the suffix says).  BED is written with the buffer type named: ``bnp.open("x.bed", "w", buffer_type=BedBuffer)`` (or
     Bed6Buffer; either writes a record's own fields).  Opening ``.bed`` for writing by its suffix alone raises
     NotImplementedError, as it did before BED could be written, so code that relies on that keeps working."""
@@ -80,7 +87,7 @@ def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
         raise NotImplementedError("writing .bed by its suffix alone is not supported: name the format with "
                                   "buffer_type=bnp.io.BedBuffer (or Bed6Buffer)")
     if buffer_type is None:
-        buffer_type = _buffer_type_for(suffix)
+        buffer_type = _buffer_type_for(suffix) if mode in WRITE_MODES else _read_buffer_type_for(suffix)
     if mode in WRITE_MODES:
         from .write import NpBufferedWriter
         raw = open(path, WRITE_MODES[mode])

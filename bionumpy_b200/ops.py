@@ -1001,3 +1001,54 @@ def cigar_unpack(base, starts, lens, offsets, total):
         return op, length
     check(lib().bnpk_cigar_unpack(*head, offsets_p, _pointer(op), _pointer(length), stream_ptr()))
     return op, length
+
+
+@_on_device
+def parse_float(base, starts, lens, column, pow5_table, status=None):
+    """bnpk_parse_float: (values float64[R], status) of the rows of decimal text, each equal to Python's float(text);
+    the first row outside the grammar is in status[ST_BAD_BASE] (ScanStatus.column_fault: row, column, nv.BAD_FLOAT).
+    ``pow5_table`` is io.decimal.pow5_table's device int64[2 * 651] (the bits of the C-ABI's uint64 words)."""
+    head, _ = _rows_args(base, starts, lens, status=status)
+    table_p = _pointer(pow5_table, "pow5_table", torch.int64, n=2 * (nv.POW5_MAX - nv.POW5_MIN + 1))
+    out = torch.empty(starts.numel(), dtype=torch.float64, device=base.device)
+    status = nv.new_status(base.device) if status is None else status
+    check(lib().bnpk_parse_float(*head, int(column), table_p, _pointer(out), _pointer(status), stream_ptr()))
+    return out, status
+
+
+def _f64_runs_args(run_starts, values, min_runs=0):
+    """(run_starts, values, R) of a float64 track: R float64 values (at least ``min_runs``) and R + 1 int64 run starts."""
+    values_p = _pointer(values, "values", torch.float64, at_least=min_runs)
+    return _pointer(run_starts, "run_starts", torch.int64, n=values.numel() + 1), values_p, values.numel()
+
+
+@_on_device
+def track_f64_reduce(run_starts, values, q_start, q_stop, mode):
+    """bnpk_track_f64_reduce: float64[Q], one reduction (nv.RUNS_*) per query [q_start, q_stop) of a float64 track,
+    with the same bits on every call; no synchronisation."""
+    runs, (q0_p, q1_p, n) = _f64_runs_args(run_starts, values, 1), _intervals(q_start, q_stop)
+    dev = q_start.device
+    out = torch.empty(n, dtype=torch.float64, device=dev)
+    scratch = torch.empty(3 * n + 1, dtype=torch.int64, device=dev)
+    n_chunks = (n + values.numel()) // 16 + 1024          # the pair list is cut into at most this many chunks
+    partial = torch.empty(2 * n_chunks, dtype=torch.float64, device=dev)
+    ws = nv.workspace(max(n, 1), dev)
+    check(lib().bnpk_track_f64_reduce(*runs, q0_p, q1_p, n, mode, _pointer(out), _pointer(scratch), _pointer(partial),
+                                      n_chunks, _pointer(ws), ws.numel(), stream_ptr()))
+    return out
+
+
+@_on_device
+def track_f64_combine(a_starts, a_values, b_starts, b_values, op):
+    """bnpk_track_f64_combine: (run_starts int64[Ra + Rb + 1], run_values float64[Ra + Rb], n_runs int64[1]), the runs
+    of op(A, B) (nv.OP_ADD, SUB, MUL, DIV, MIN, MAX or a comparison) of two float64 tracks of one size, canonical under
+    bitwise equality, the first n_runs + 1 starts and n_runs values valid (nothing is read back)."""
+    a, b = _f64_runs_args(a_starts, a_values), _f64_runs_args(b_starts, b_values)
+    n, dev = a[2] + b[2], a_starts.device
+    starts = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    values = torch.empty(max(n, 1), dtype=torch.float64, device=dev)
+    n_runs = torch.empty(1, dtype=torch.int64, device=dev)
+    ws = nv.workspace(max(n, 1), dev)
+    check(lib().bnpk_track_f64_combine(*a, *b, op, _pointer(starts), _pointer(values), _pointer(n_runs), _pointer(ws),
+                                       ws.numel(), stream_ptr()))
+    return starts, values, n_runs

@@ -504,6 +504,37 @@ int bnpk_runs_to_intervals(const int64_t *run_starts, const int64_t *values, siz
                            size_t n_contigs, int mode, int32_t *out_contig, int64_t *out_start, int64_t *out_stop,
                            int64_t *out_value, int64_t *n_out, void *workspace, size_t workspace_bytes, void *stream);
 
+/* K17  float64 signal tracks (bedGraph values; GenomicArray of floats, genomic_data/genomic_track.py).
+ * bnpk_parse_float: out[r] = the double of the text base[starts[r] .. + lens[r]) (negative length = empty), equal to
+ *   Python's float(text) bit for bit (round half to even; -0.0, subnormals, underflow to +-0 and overflow to +-inf).
+ *   Grammar: [+-]? (digits ['.' digits?] | '.' digits) ([eE] [+-]? digits)?, at most 19 significant digits (leading
+ *   zeros and the trailing zeros of the significand not counted); exponents of any length.  A row outside it (empty,
+ *   a bare sign or '.', a dangling exponent, a second '.', nan, inf, hex, '_', spaces, a 20th significant digit) gives
+ *   0.0 and is atomicMin-ed into status[BNPK_ST_BAD_BASE] as fault_column(r, column, BNPK_BAD_FLOAT) (status
+ *   pre-initialised).  pow5_table is uint64[2 * 651]: for q = -342 .. 308 the high and low words of 5^q truncated to
+ *   128 bits with the top bit set (negative q: floor(2^b / 5^-q) + 1 for the b that gives 128 bits, b = z + 127 for
+ *   q >= -27 and 2z + 128 below, z the bit length of 5^-q, then truncated).
+ * bnpk_track_f64_reduce: bnpk_runs_reduce over float64 values (run_starts int64[R + 1], values double[R]): out[q]
+ *   (double) is BNPK_RUNS_MAX / MIN (a NaN in the range gives NaN; +0.0 is above -0.0), BNPK_RUNS_SUM the sum of value x
+ *   positions, BNPK_RUNS_ANY 1.0 if a value is not 0 (NaN counts) else 0.0.  An empty query gives -inf, +inf, 0.0 and
+ *   0.0.  The (query, run) pairs are cut into chunks of max(16, ceil(pairs / n_chunks_cap)) pairs and summed in a fixed
+ *   order, so every result has the same bits on every call whatever the grid.  scratch is int64[3 * n_q + 1], partial
+ *   double[2 * n_chunks_cap]; workspace as for bnpk_row_offsets with n := n_q.  No synchronisation.
+ * bnpk_track_f64_combine: bnpk_runs_combine over float64 values: BNPK_OP_ADD, SUB, MUL and DIV (IEEE: x / 0 is +-inf
+ *   or NaN), MIN and MAX (NumPy's minimum / maximum: NaN wins, else the second operand unless the first is strictly
+ *   smaller / larger) and EQ, NE, LT, LE, GT and GE (1.0 or 0.0).  A run starts where the value's bits change, so -0.0
+ *   next to +0.0 is two runs.  BNPK_E_BADARG for another operator. */
+#define BNPK_BAD_FLOAT 7   /* a value outside the decimal grammar, or of more than 19 significant digits */
+#define BNPK_OP_DIV    14
+int bnpk_parse_float(const uint8_t *base, size_t base_bytes, const int64_t *starts, const int32_t *lens, size_t n_rows,
+                     int column, const uint64_t *pow5_table, double *out, int64_t *status, void *stream);
+int bnpk_track_f64_reduce(const int64_t *run_starts, const double *values, size_t n_runs, const int64_t *q_start,
+                          const int64_t *q_stop, size_t n_q, int mode, double *out, int64_t *scratch, double *partial,
+                          size_t n_chunks_cap, void *workspace, size_t workspace_bytes, void *stream);
+int bnpk_track_f64_combine(const int64_t *a_starts, const double *a_values, size_t n_a, const int64_t *b_starts,
+                           const double *b_values, size_t n_b, int op, int64_t *out_starts, double *out_values,
+                           int64_t *n_out, void *workspace, size_t workspace_bytes, void *stream);
+
 /* Bloom filter over k-mer hashes (sequence/bloom_filter.py:15-42): hash function i is v ^ offsets[i]; the filter is
  * one byte per position (the reference's bool mask).  insert: mask[(v ^ offsets[i]) % mask_size] = 1 for every value and
  * function; query: out[j] = AND over the functions. */
