@@ -25,10 +25,11 @@ from .sequence import count_kmers_exact, KmerCounter, KmerCounts
 from .io.buffers import CudaFastQBuffer, CudaTwoLineFastaBuffer, FastQBuffer, TwoLineFastaBuffer
 from .io.multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
 from .datatypes import (SequenceEntry, SequenceEntryWithQuality, Interval, StrandedInterval, Bed6, BedGraph, BamEntry,
-                        SAMEntry, GTFEntry, GFFEntry, GFFGeneEntry, GFFTranscriptEntry, GFFExonEntry, replace)
+                        SAMEntry, GTFEntry, GFFEntry, GFFGeneEntry, GFFTranscriptEntry, GFFExonEntry, NarrowPeak,
+                        LocationEntry, StrandedLocationEntry, replace)
 from . import datatypes
 from . import arithmetics, genomic_data, alignments
-from .genomic_data import Genome, GenomicIntervals, GenomicArray
+from .genomic_data import Genome, GenomicIntervals, GenomicArray, GenomicLocation
 from .io.files import count_entries
 from .io.write import NpBufferedWriter
 

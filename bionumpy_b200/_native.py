@@ -40,6 +40,7 @@ BAD_CIGAR = 6
 BAD_FLOAT = 7
 OP_DIV = 14
 POW5_MIN, POW5_MAX = -342, 308
+COLUMN_BLOCK_ROWS = 256
 (SAM_F_NAME_START, SAM_F_NAME_LEN, SAM_F_RNAME_START, SAM_F_RNAME_LEN, SAM_F_CIGAR_START, SAM_F_CIGAR_LEN,
  SAM_F_RNEXT_START, SAM_F_RNEXT_LEN, SAM_F_SEQ_START, SAM_F_SEQ_LEN, SAM_F_QUAL_START, SAM_F_QUAL_LEN, SAM_F_EXTRA_START,
  SAM_F_EXTRA_LEN, SAM_F_FLAG, SAM_F_POS, SAM_F_MAPQ, SAM_F_PNEXT, SAM_F_TLEN) = range(19)
@@ -119,6 +120,8 @@ SIGNATURES = {
     "bnpk_parse_float": (_i, [_vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _vp]),
     "bnpk_track_f64_reduce": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "bnpk_track_f64_combine": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "bnpk_runs_column_sum": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i64, _vp, _vp, _vp]),
+    "bnpk_track_f64_column_sum": (_i, [_vp, _vp, _sz, _vp, _vp, _sz, _i64, _vp, _vp, _vp]),
 }
 
 

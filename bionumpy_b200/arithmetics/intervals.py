@@ -527,24 +527,59 @@ class RunsRaggedArray(LazyRaggedArray):
     the same rows for the fused reductions and the gathered values (a part of an interval outside the track has no
     values).  ``max``, ``min``, ``sum``, ``mean`` and ``any`` along the rows run fused over the runs (no
     synchronisation, the positions are never written); anything else gathers the values (one synchronisation, for
-    their number)."""
+    their number).  ``reverse`` (a bool or uint8 device tensor, one flag per row, or None) gives the values of the
+    flagged rows back to front, as the windows of '-' strand features are read (an index permutation after the gather,
+    which at its peak needs about three times the gather's memory); the reductions along the rows do not depend on
+    it.  ``sum(axis=0)`` and ``mean(axis=0)`` of rows of one length run fused over the runs too
+    (bnpk_runs_column_sum / bnpk_track_f64_column_sum): one synchronisation, for the width and the length check."""
 
-    def __init__(self, track, start, stop):
+    def __init__(self, track, start, stop, reverse=None):
         size = len(track)
         start = start.clamp(0, size)
         stop = torch.maximum(stop.clamp(max=size), start)
         super().__init__(stop - start, 0)
         self._track = track
         self._q_start, self._q_stop = start.contiguous(), stop.contiguous()
+        self._reverse = None if reverse is None else reverse.to(torch.uint8).contiguous()
 
     def _compute(self):
         offsets = ops.row_offsets(self._lens)
-        out = ops.runs_extract(self._track._events, self._track._values64(), self._q_start, offsets,
-                               int(offsets[-1].item()))
+        total = int(offsets[-1].item())
+        out = ops.runs_extract(self._track._events, self._track._values64(), self._q_start, offsets, total)
+        if self._reverse is not None and total:
+            # the value at flat index j of a reversed row [o, o + L) is the gathered one at 2o + L - 1 - j: one mirror
+            # point per row (-1 on forward rows) spread over the row's positions, the permutation built in place.  At
+            # its peak this holds two int64 and one bool per position beside the gathered values: about three times
+            # the memory of an unstranded gather.
+            lens = self._lens.to(torch.int64)
+            mirror = torch.where(self._reverse != 0, 2 * offsets[:-1] + lens - 1, -1)
+            src = torch.repeat_interleave(mirror, lens, output_size=total)
+            idx = torch.arange(total, dtype=torch.int64, device=lens.device)
+            flip = src >= 0
+            torch.where(flip, src.sub_(idx), idx, out=idx)
+            del src, flip
+            out = out[idx]
         return self._track._cast(out)
 
     def _reduce(self, mode):
         return self._track._reduce_rows(self._q_start, self._q_stop, mode)
+
+    def _column_sum(self):
+        """The sum of every column of rows of one length, and the row count: int64 for integer and bool tracks,
+        float64 for float tracks.  One synchronisation reads the width and the number of rows of another length."""
+        n = len(self)
+        lens = self._lens.to(torch.int64)
+        if n == 0:
+            raise NotImplementedError("mean(axis=0) needs rows of one length: there are no rows")
+        width, n_other = ops.read_back(lens[:1], (lens != lens[0]).sum())
+        if n_other:
+            raise NotImplementedError(f"mean(axis=0) needs rows of one length: {n_other} of the {n} rows differ in "
+                                      f"length from the first ({width})")
+        track = self._track
+        if isinstance(track, FloatRunLengthArray):
+            return ops.track_f64_column_sum(track._events, track._values.contiguous(), self._q_start, width,
+                                            self._reverse), n
+        return ops.runs_column_sum(track._events, track._values64(), self._q_start, width, self._reverse), n
 
     def max(self, axis=None, **kwargs):
         if axis not in (-1, 1):
@@ -557,11 +592,17 @@ class RunsRaggedArray(LazyRaggedArray):
         return self._reduce(nv.RUNS_MIN)
 
     def sum(self, axis=None, **kwargs):
+        if axis == 0:
+            return self._column_sum()[0]
         if axis not in (-1, 1):
             return super().sum(axis, **kwargs)
         return self._reduce(nv.RUNS_SUM)
 
     def mean(self, axis=None, **kwargs):
+        if axis == 0:
+            total, n = self._column_sum()
+            # a true division: torch divides by a Python scalar as a multiply by its reciprocal
+            return total.to(torch.float64) / torch.full_like(total, n, dtype=torch.float64)
         if axis not in (-1, 1):
             return super().mean(axis, **kwargs)
         return self._reduce(nv.RUNS_SUM).to(torch.float64) / self._lens.to(torch.float64)

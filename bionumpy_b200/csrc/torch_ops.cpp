@@ -882,6 +882,48 @@ std::tuple<Tensor, Tensor, Tensor> track_f64_combine(const Tensor &a_starts, con
     return {starts, values, n_runs};
 }
 
+// out[j] = the sum over rows q of the track's value at q_start[q] + j (q_start[q] + width - 1 - j where reverse[q]);
+// int64 values give the wrapping int64 sum, float64 values the float64 sum in the fixed order of include/bnpk.h
+Tensor column_sum(const Tensor &run_starts, const Tensor &values, const Tensor &q_start, int64_t width,
+                  const c10::optional<Tensor> &reverse, bool f64) {
+    need(run_starts, torch::kInt64, "run_starts");
+    need(values, f64 ? torch::kFloat64 : torch::kInt64, "values", run_starts);
+    TORCH_CHECK(values.numel() >= 1 && run_starts.numel() == values.numel() + 1,
+                "bnpk: a track is R >= 1 values and R + 1 run starts");
+    need(q_start, torch::kInt64, "q_start", run_starts);
+    const int64_t n = q_start.numel();
+    const uint8_t *rev = nullptr;
+    if (reverse) {
+        need(*reverse, torch::kUInt8, "reverse", run_starts);
+        TORCH_CHECK(reverse->numel() == n, "bnpk: reverse needs one flag per row");
+        rev = u8(*reverse);
+    }
+    TORCH_CHECK(width >= 0 && width < ((int64_t)1 << 31), "bnpk: width must be in [0, 2^31)");
+    c10::cuda::CUDAGuard guard(run_starts.device());
+    Tensor out = torch::empty({width}, values.options());
+    Tensor partial = torch::empty({(n + BNPK_COLUMN_BLOCK_ROWS - 1) / BNPK_COLUMN_BLOCK_ROWS * width}, values.options());
+    const int64_t *q = n ? q_start.data_ptr<int64_t>() : nullptr;
+    if (f64)
+        check(bnpk_track_f64_column_sum(run_starts.data_ptr<int64_t>(), values.data_ptr<double>(), (size_t)values.numel(),
+                                        q, rev, (size_t)n, width, width ? out.data_ptr<double>() : nullptr,
+                                        n && width ? partial.data_ptr<double>() : nullptr, cur_stream(run_starts)),
+              "track_f64_column_sum");
+    else
+        check(bnpk_runs_column_sum(run_starts.data_ptr<int64_t>(), values.data_ptr<int64_t>(), (size_t)values.numel(),
+                                   q, rev, (size_t)n, width, width ? out.data_ptr<int64_t>() : nullptr,
+                                   n && width ? partial.data_ptr<int64_t>() : nullptr, cur_stream(run_starts)),
+              "runs_column_sum");
+    return out;
+}
+Tensor runs_column_sum(const Tensor &run_starts, const Tensor &values, const Tensor &q_start, int64_t width,
+                       const c10::optional<Tensor> &reverse) {
+    return column_sum(run_starts, values, q_start, width, reverse, false);
+}
+Tensor track_f64_column_sum(const Tensor &run_starts, const Tensor &values, const Tensor &q_start, int64_t width,
+                            const c10::optional<Tensor> &reverse) {
+    return column_sum(run_starts, values, q_start, width, reverse, true);
+}
+
 }  // namespace
 
 TORCH_LIBRARY(bnpk, m) {
@@ -941,6 +983,10 @@ TORCH_LIBRARY(bnpk, m) {
     m.def("track_f64_reduce(Tensor run_starts, Tensor values, Tensor q_start, Tensor q_stop, int mode) -> Tensor");
     m.def("track_f64_combine(Tensor a_starts, Tensor a_values, Tensor b_starts, Tensor b_values, int op) "
           "-> (Tensor, Tensor, Tensor)");
+    m.def("runs_column_sum(Tensor run_starts, Tensor values, Tensor q_start, int width, Tensor? reverse=None) "
+          "-> Tensor");
+    m.def("track_f64_column_sum(Tensor run_starts, Tensor values, Tensor q_start, int width, Tensor? reverse=None) "
+          "-> Tensor");
 }
 
 TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
@@ -983,4 +1029,6 @@ TORCH_LIBRARY_IMPL(bnpk, CUDA, m) {
     m.impl("parse_float", &parse_float);
     m.impl("track_f64_reduce", &track_f64_reduce);
     m.impl("track_f64_combine", &track_f64_combine);
+    m.impl("runs_column_sum", &runs_column_sum);
+    m.impl("track_f64_column_sum", &track_f64_column_sum);
 }

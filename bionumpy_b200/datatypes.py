@@ -124,9 +124,13 @@ class SAMEntry(_Entries):
                "sequence", "quality", "extra")
 
 
+_FLOAT_FIELDS = ("signal_value", "p_value", "q_value")
+
+
 def _interval_field(field, value):
-    """Interval, Bed6 and BedGraph fields: text columns (chromosome, name) as text, integer columns (start, stop, score)
-    as int64 CUDA tensors, a bedGraph value as a CUDA tensor of its own dtype and strand as StrandEncoding codes."""
+    """Interval, Bed6, BedGraph, NarrowPeak and location fields: text columns (chromosome, name) as text, integer
+    columns (start, stop, score, summit, position) as int64 CUDA tensors, a bedGraph value as a CUDA tensor of its own
+    dtype, the narrowPeak scores as float64 CUDA tensors and strand as StrandEncoding codes."""
     if field in ("chromosome", "name"):
         return _from_strings(field, value)
     from . import config
@@ -143,6 +147,8 @@ def _interval_field(field, value):
         return value
     if field == "value":
         return torch.as_tensor(np.asarray(value)).to(config.default_device())     # kept in its dtype
+    if field in _FLOAT_FIELDS:
+        return torch.as_tensor(np.asarray(value, dtype=np.float64)).to(config.default_device())
     if field == "score" and isinstance(value, list):
         value = [0 if v == "." else int(v) for v in value]        # Optional[int]: "." is 0 (io/strops.py:69-83)
     return torch.as_tensor(np.asarray(value, dtype=np.int64)).to(config.default_device())
@@ -182,6 +188,22 @@ class StrandedInterval(_IntervalEntries):
 class Bed6(_IntervalEntries):
     """datatypes/__init__.py:67-70: Interval + name, score (Optional[int]) and strand."""
     _fields = ("chromosome", "start", "stop", "name", "score", "strand")
+
+
+class NarrowPeak(_IntervalEntries):
+    """datatypes/__init__.py:74-78: a MACS2 narrowPeak row, Bed6 + signal_value, p_value and q_value (float64) and
+    summit (int64, the summit's offset from start)."""
+    _fields = Bed6._fields + ("signal_value", "p_value", "q_value", "summit")
+
+
+class LocationEntry(_IntervalEntries):
+    """datatypes/__init__.py:16-18: chromosome and position (0-based)."""
+    _fields = ("chromosome", "position")
+
+
+class StrandedLocationEntry(_IntervalEntries):
+    """datatypes/__init__.py:21-23: LocationEntry + strand."""
+    _fields = ("chromosome", "position", "strand")
 
 
 class BedGraph(_IntervalEntries):

@@ -14,9 +14,18 @@ from .. import _native as nv
 from .. import ops
 from ..arithmetics.intervals import (FloatRunLengthArray, GenomicRunLengthArray, RunsRaggedArray, _add_operators,
                                      _device, _int64, _rtruediv, _truediv, coverage_runs, to_device, track_ufunc)
-from ..datatypes import BedGraph, Interval, replace
+from ..datatypes import BedGraph, Interval, LocationEntry, StrandedInterval, StrandedLocationEntry, replace
 from ..encoded_array import BaseEncoding, EncodedArray, EncodedRaggedArray
+from ..encodings import StrandEncoding
 from ..rows import RowView
+
+MINUS = 1           # StrandEncoding's code of '-' ('+' 0, '.' 2)
+
+
+def _strand_codes(strand, device):
+    """StrandEncoding codes (uint8, on the device) of a record's strand field."""
+    codes = strand.raw() if isinstance(strand, EncodedArray) else torch.as_tensor(np.asarray(strand))
+    return codes.reshape(-1).to(device, torch.uint8)
 
 
 def ignore_underscores(name):
@@ -127,8 +136,47 @@ class Genome:
         return EncodedRaggedArray(EncodedArray(text, BaseEncoding), lens, starts=name_offsets[ids])
 
     def get_intervals(self, intervals, stranded=False) -> "GenomicIntervals":
-        """genome.py:181-209: the intervals of a record (Interval, Bed6, ...) placed on this genome."""
-        return GenomicIntervals.from_intervals(intervals, self)
+        """genome.py:181-209: the intervals of a record (Interval, Bed6, ...) placed on this genome.  ``stranded=True``
+        keeps the record's strand (a record without a strand field raises ValueError): windows on '-' rows are then
+        read back to front when they index a track."""
+        return GenomicIntervals.from_intervals(intervals, self, stranded)
+
+    def get_locations(self, entries) -> "GenomicLocation":
+        """genome.py:328-349: LocationEntry (or StrandedLocationEntry) records placed on this genome, as
+        from_intervals places intervals: an unknown name raises KeyError, a position outside [0, contig size) raises
+        ValueError naming the row, and rows on contigs the genome leaves out are dropped.  A strand field makes the
+        locations stranded.  One synchronisation.
+
+        >>> genome = Genome.from_dict({'chr1': 100, 'chr2': 50})
+        >>> genome.get_locations(LocationEntry(['chr1', 'chr2'], [10, 49])).position.tolist()
+        [10, 49]"""
+        names, text, name_offsets, offset, size = self._name_table()
+        dev = text.device
+        rows = RowView(entries.chromosome)
+        pos = _int64(entries.position, dev)
+        ids, st_names = ops.name_lookup(rows.base, rows.starts, rows.lens, text, name_offsets)
+        _, g_pos, _, st_rows = ops.interval_events(pos, pos + 1, ids, offset, size, keys=False, glob=True)
+        keep = offset[ids.clamp(min=0).to(torch.int64)] >= 0
+        st_names, st_rows, n_keep = ops.read_back(st_names, st_rows, keep.sum())
+        if st_names.fault is not None:
+            raise KeyError(entries.chromosome[st_names.fault].to_string())
+        bad = st_rows.fault
+        if bad is not None:
+            name = entries.chromosome[bad].to_string()
+            raise ValueError(f"location {bad} ({name}:{int(pos[bad])}) is not inside the contig "
+                             f"({self._all[name]} bases)")
+        strand = _strand_codes(entries.strand, dev) if "strand" in entries._fields else None
+        out = GenomicLocation(ids.to(torch.int64), g_pos, pos, self, strand)
+        if n_keep < len(ids):
+            out = out[torch.nonzero_static(keep, size=n_keep).reshape(-1)]
+        return out
+
+    def _rank(self, ids):
+        """The genome-order rank of every row's contig (ids index the name table; left-out contigs rank -1)."""
+        names = self._name_table()[0]
+        order = {n: i for i, n in enumerate(self._sizes)}
+        rank = to_device(np.array([order.get(n, -1) for n in names], dtype=np.int64), ids.device)
+        return rank[ids.to(torch.int64)]
 
     def read_intervals(self, filename, stranded=False, stream=False, buffer_type=None) -> "GenomicIntervals":
         """genome.py:211-261: a BED file, or the alignments of a BAM or SAM file (BamIntervalBuffer, SAMIntervalBuffer),
@@ -244,16 +292,21 @@ def _read_sizes(filename):
 
 class GenomicIntervals:
     """Intervals on a genome (genomic_intervals.py): the record, each row's contig (an index of the genome's sorted
-    name table) and its global start and stop, all on the device."""
+    name table) and its global start and stop, all on the device.  Stranded intervals also carry each row's strand
+    (StrandEncoding codes); a track indexed by them gives the values of '-' rows back to front."""
 
-    def __init__(self, record, ids, g_start, g_stop, genome):
+    def __init__(self, record, ids, g_start, g_stop, genome, strand=None):
         self._record, self._ids, self._g_start, self._g_stop, self._genome = record, ids, g_start, g_stop, genome
+        self._strand = strand
 
     @classmethod
-    def from_intervals(cls, record, genome):
+    def from_intervals(cls, record, genome, stranded=False):
         """The rows' names are looked up on the device.  An unknown name raises KeyError; an interval with start < 0,
         stop < start or stop past its contig raises ValueError naming the first one; rows on contigs the genome
-        leaves out are dropped."""
+        leaves out are dropped.  ``stranded=True`` keeps the record's strand; a record without one raises
+        ValueError."""
+        if stranded and "strand" not in record._fields:
+            raise ValueError(f"stranded intervals need a strand field, which {type(record).__name__} has not")
         names, text, name_offsets, offset, size = genome._name_table()
         dev = text.device
         rows = RowView(record.chromosome)
@@ -269,7 +322,7 @@ class GenomicIntervals:
             name = record.chromosome[bad].to_string()
             raise ValueError(f"interval {bad} ({name}:{int(start[bad])}-{int(stop[bad])}) is not inside the contig "
                              f"({genome._all[name]} bases)")
-        out = cls(record, ids, g_start, g_stop, genome)
+        out = cls(record, ids, g_start, g_stop, genome, _strand_codes(record.strand, dev) if stranded else None)
         if n_keep < len(ids):
             out = out[torch.nonzero(keep).reshape(-1)]
         return out
@@ -298,6 +351,20 @@ class GenomicIntervals:
     def stop(self):
         return self._record.stop
 
+    @property
+    def strand(self):
+        """The strand of every row; unstranded intervals raise ValueError, as in the reference."""
+        if self._strand is None:
+            raise ValueError("Unstranded interval has not strand")
+        return self._record.strand
+
+    def is_stranded(self) -> bool:
+        return self._strand is not None
+
+    def _location_strand(self):
+        """The strand codes get_location and extended_to_size go by, or None."""
+        return self._strand
+
     def get_data(self):
         return self._record
 
@@ -310,7 +377,56 @@ class GenomicIntervals:
             idx = torch.as_tensor(np.asarray(idx))
         if isinstance(idx, torch.Tensor):
             idx = idx.to(self._ids.device)
-        return type(self)(self._record[idx], self._ids[idx], self._g_start[idx], self._g_stop[idx], self._genome)
+        strand = None if self._strand is None else self._strand[idx]
+        return type(self)(self._record[idx], self._ids[idx], self._g_start[idx], self._g_stop[idx], self._genome,
+                          strand)
+
+    def _contig_bounds(self):
+        """Each row's contig offset and size (int64 device tensors)."""
+        _, _, _, offset, size = self._genome._name_table()
+        ids = self._ids.to(torch.int64)
+        return offset[ids], size[ids]
+
+    def _with(self, start, stop):
+        """These intervals with new local starts and stops, clipped to [0, contig size); the record keeps its type
+        and every other field."""
+        offset, size = self._contig_bounds()
+        start, stop = start.clamp(min=0), torch.minimum(stop, size)
+        return type(self)(replace(self._record, start=start, stop=stop), self._ids, offset + start, offset + stop,
+                          self._genome, self._strand)
+
+    def clip(self) -> "GenomicIntervals":
+        """The intervals clipped to [0, contig size) (genomic_intervals.py:819-830); no synchronisation."""
+        offset, _ = self._contig_bounds()
+        return self._with(self._g_start - offset, self._g_stop - offset)
+
+    def extended_to_size(self, size: int) -> "GenomicIntervals":
+        """Every interval made ``size`` long along its strand (genomic_intervals.py:755-768), then clipped: '+' rows
+        keep their start, '-' rows their stop; '.' and unstranded rows behave as '+'.  ``reads.extended_to_size(200)
+        .get_pileup()`` is a fragment pileup.  No synchronisation."""
+        offset, _ = self._contig_bounds()
+        start, stop = self._g_start - offset, self._g_stop - offset
+        strand = self._location_strand()
+        if strand is None:
+            return self._with(start, start + size)
+        minus = strand == MINUS
+        return self._with(torch.where(minus, stop - size, start), torch.where(minus, stop, start + size))
+
+    def get_location(self, where: str = "start") -> "GenomicLocation":
+        """The 'start', 'stop' or 'center' of every interval (genomic_intervals.py:705-733), stranded when the
+        intervals are.  On a '-' row 'start' is stop - 1 and 'stop' is start; on '+', '.' and unstranded rows 'start'
+        is start and 'stop' is stop - 1; 'center' is (start + stop) // 2.  No synchronisation."""
+        if where not in ("start", "stop", "center"):
+            raise ValueError(f"where must be 'start', 'stop' or 'center', not {where!r}")
+        offset, _ = self._contig_bounds()
+        start, stop = self._g_start - offset, self._g_stop - offset
+        strand = self._location_strand()
+        if where == "center":
+            pos = torch.div(start + stop, 2, rounding_mode="floor")
+        else:
+            first, last = (start, stop - 1) if where == "start" else (stop - 1, start)
+            pos = first if strand is None else torch.where(strand == MINUS, last, first)
+        return GenomicLocation(self._ids.to(torch.int64), offset + pos, pos, self._genome, strand)
 
     def __repr__(self):
         names = list(self._genome._sizes)
@@ -334,16 +450,13 @@ class GenomicIntervals:
         """The intervals in genome order, then by start, then by stop, stably (genomic_intervals.py:691-699); on the
         device, no synchronisation."""
         from ..arithmetics.intervals import lexsort_order
-        names = self._genome._name_table()[0]
-        order = {n: i for i, n in enumerate(self._genome._sizes)}
-        rank = to_device(np.array([order.get(n, -1) for n in names], dtype=np.int64), self._ids.device)
-        return self[lexsort_order(self._g_stop, self._g_start, rank[self._ids.to(torch.int64)])]
+        return self[lexsort_order(self._g_stop, self._g_start, self._genome._rank(self._ids))]
 
     def merged(self, distance=0) -> "GenomicIntervals":
         """merge_intervals on every contig, in genome order: the rows are sorted by global start on the device, a
-        merge never crosses a contig, one synchronisation."""
+        merge never crosses a contig, one synchronisation.  The result is unstranded, as in the reference."""
         if len(self) == 0:
-            return self
+            return GenomicIntervals(self._record, self._ids, self._g_start, self._g_stop, self._genome)
         order = torch.sort(self._g_start, stable=True).indices
         g_start, g_stop, ids = self._g_start[order], self._g_stop[order], self._ids[order]
         same = torch.cat([torch.zeros(1, dtype=torch.bool, device=ids.device), ids[1:] == ids[:-1]]).to(torch.uint8)
@@ -357,11 +470,19 @@ class GenomicIntervals:
 
 
 class Genes(GenomicIntervals):
-    """annotation.py Genes: gene intervals with their strand and gene_id."""
+    """annotation.py Genes: gene intervals with their strand and gene_id.  They always carry a strand, so
+    get_location and extended_to_size go by it and give stranded results, as the reference's stranded annotation does;
+    a track indexed by the features themselves is read forward on every strand, as before."""
 
     @property
     def strand(self):
         return self._record.strand
+
+    def is_stranded(self) -> bool:
+        return True
+
+    def _location_strand(self):
+        return self._strand if self._strand is not None else _strand_codes(self._record.strand, self._ids.device)
 
     @property
     def gene_id(self):
@@ -378,6 +499,76 @@ class Exons(Transcripts):
     @property
     def exon_id(self):
         return self._record.exon_id
+
+
+class GenomicLocation:
+    """Positions on a genome (genomic_intervals.py GenomicLocation): each row's contig (an index of the genome's sorted
+    name table), its global and local position and, for stranded locations, its strand (StrandEncoding codes), all on
+    the device.  Made by Genome.get_locations and GenomicIntervals.get_location."""
+
+    def __init__(self, ids, g_pos, pos, genome, strand=None):
+        self._ids, self._g_pos, self._pos, self._genome, self._strand = ids, g_pos, pos, genome, strand
+
+    @property
+    def chromosome(self):
+        return self._genome._names_of(self._ids)
+
+    @property
+    def position(self):
+        return self._pos
+
+    @property
+    def strand(self):
+        if self._strand is None:
+            raise ValueError("Unstranded location has not strand")
+        return EncodedArray(self._strand, StrandEncoding)
+
+    def is_stranded(self) -> bool:
+        return self._strand is not None
+
+    def __len__(self):
+        return self._ids.numel()
+
+    def __getitem__(self, idx):
+        """The selected locations (a bool mask, an index tensor/array/list)."""
+        if isinstance(idx, (list, np.ndarray)):
+            idx = torch.as_tensor(np.asarray(idx))
+        if isinstance(idx, torch.Tensor):
+            idx = idx.to(self._ids.device)
+        strand = None if self._strand is None else self._strand[idx]
+        return GenomicLocation(self._ids[idx], self._g_pos[idx], self._pos[idx], self._genome, strand)
+
+    def sorted(self) -> "GenomicLocation":
+        """The locations in genome order, then by position, stably; on the device, no synchronisation."""
+        from ..arithmetics.intervals import lexsort_order
+        return self[lexsort_order(self._pos, self._genome._rank(self._ids))]
+
+    def get_data(self):
+        """The locations as LocationEntry records, or StrandedLocationEntry when stranded."""
+        if self._strand is None:
+            return LocationEntry(self.chromosome, self._pos)
+        return StrandedLocationEntry(self.chromosome, self._pos, self.strand)
+
+    def get_windows(self, flank=None, window_size=None) -> GenomicIntervals:
+        """Windows around the locations (genomic_intervals.py:212-243): [p - flank, p + flank + 1) with ``flank``, else
+        [p - window_size // 2, p + window_size // 2 + window_size % 2), clipped to the contig and stranded when the
+        locations are.  No synchronisation."""
+        if (flank is None) == (window_size is None):
+            raise ValueError("give one of flank and window_size")
+        left, right = (flank, flank + 1) if flank is not None else (window_size // 2, window_size // 2 + window_size % 2)
+        names = self.chromosome
+        if self._strand is None:
+            record = Interval(names, self._pos - left, self._pos + right)
+        else:
+            record = StrandedInterval(names, self._pos - left, self._pos + right, self.strand)
+        offset = self._g_pos - self._pos
+        windows = GenomicIntervals(record, self._ids, offset + record.start, offset + record.stop, self._genome,
+                                   self._strand)
+        return windows.clip()
+
+    def __repr__(self):
+        names = list(self._genome._sizes)
+        return f"Genomic Locations on {names[:10] + ['...'] * (len(names) > 10)}: {len(self)} locations"
 
 
 class GenomicAnnotation:
@@ -448,18 +639,25 @@ class GenomicArray:
 
     def __getitem__(self, idx):
         """``track["chr1"]``: one contig's runs.  ``track[intervals]`` (GenomicIntervals, or a record placed on the
-        genome here): the lazy per-interval values, one row per interval.  A record with rows on contigs the genome
-        leaves out raises ValueError, since those rows would be dropped and the rows would no longer line up with the
-        record; place it with genome.get_intervals first to drop them."""
+        genome here): the lazy per-interval values, one row per interval; the rows of stranded intervals on '-' are
+        read back to front.  A record with rows on contigs the genome leaves out raises ValueError, since those rows
+        would be dropped and the rows would no longer line up with the record; place it with genome.get_intervals first
+        to drop them.  ``track[locations]`` (GenomicLocation): the value at every location in the track's dtype, with
+        no synchronisation."""
         if isinstance(idx, str):
             return self._contig(idx)
+        if isinstance(idx, GenomicLocation):
+            track, n = self._global, len(idx)
+            offsets = torch.arange(n + 1, dtype=torch.int64, device=idx._g_pos.device)
+            return track._cast(ops.runs_extract(track._events, track._values64(), idx._g_pos.contiguous(), offsets, n))
         if not isinstance(idx, GenomicIntervals):
             placed = self._genome.get_intervals(idx)
             if len(placed) != len(idx):
                 raise ValueError(f"{len(idx) - len(placed)} of the {len(idx)} intervals are on contigs the genome leaves "
                                  "out; index the track with genome.get_intervals(intervals) to drop them")
             idx = placed
-        return RunsRaggedArray(self._global, idx._g_start, idx._g_stop)
+        reverse = None if idx._strand is None else idx._strand == MINUS
+        return RunsRaggedArray(self._global, idx._g_start, idx._g_stop, reverse)
 
     def _contig(self, name):
         """The contig's runs, split off on the device: the run that holds its first position and every run that starts
@@ -502,5 +700,5 @@ class GenomicArray:
 _add_operators(GenomicArray)
 GenomicArray.__truediv__, GenomicArray.__rtruediv__ = _truediv, _rtruediv
 
-__all__ = ["Genome", "GenomicIntervals", "GenomicArray", "GenomicAnnotation", "Genes", "Transcripts", "Exons",
-           "ignore_underscores", "keep_all"]
+__all__ = ["Genome", "GenomicIntervals", "GenomicLocation", "GenomicArray", "GenomicAnnotation", "Genes", "Transcripts",
+           "Exons", "ignore_underscores", "keep_all"]

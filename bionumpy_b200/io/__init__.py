@@ -7,7 +7,8 @@ from .write import NpBufferedWriter
 from .parser import CudaFileReader, NpDataclassReader
 from .multiline import CudaMultiLineFastaBuffer, MultiLineFastaBuffer
 from .indexed_fasta import IndexedFasta, read_index, create_index, open_indexed
-from .delimited import DelimitedBuffer, BedBuffer, Bed6Buffer, BdgBuffer, BedGraphBuffer, GTFBuffer, GFFBuffer
+from .delimited import DelimitedBuffer, BedBuffer, Bed6Buffer, BdgBuffer, BedGraphBuffer, GTFBuffer, GFFBuffer, \
+    NarrowPeakBuffer
 from .motifs import read_motif
 from .bam import BamBuffer, BamIntervalBuffer
 from .sam import SAMBuffer, SAMIntervalBuffer

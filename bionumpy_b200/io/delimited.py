@@ -11,7 +11,7 @@ import torch
 
 from .. import _native as nv
 from .. import ops
-from ..datatypes import Bed6, BedGraph, GFFEntry, GTFEntry, Interval, StrandedInterval
+from ..datatypes import Bed6, BedGraph, GFFEntry, GTFEntry, Interval, NarrowPeak, StrandedInterval
 from ..encoded_array import EncodedArray, EncodedRaggedArray, BaseEncoding
 from ..encodings import StrandEncoding
 from .buffers import FieldView, _to_device_bytes
@@ -31,6 +31,7 @@ class DelimitedBuffer:
     n_lines_per_entry = 1
     dataclass = None
     _kinds = ()                 # nv.COL_* of the record type's fields, in column order
+    _float_columns = ()         # the COL_TEXT columns read as float64 values (bnpk_parse_float)
 
     def __init__(self, data, n_lines, fields):
         self._data = data       # device bytes, complete lines only
@@ -70,6 +71,7 @@ class DelimitedBuffer:
             raise IncompleteEntryException("No complete line in the buffer. Try increasing chunk_size.")
         starts, lens, _ = ops.line_split(chunk, 1, 0, 0, ord(cls.COMMENT), False, 0, max_rows=n_lines)
         cols, status = ops.delimited_columns(chunk, starts, lens, cls._kinds)
+        floats = {c: cls._parse_floats(chunk, cols[c], c, status) for c in cls._float_columns}
         # the one synchronisation of the columns: the first fault and the chunk's size
         st, last_end = ops.read_back(status, starts[-1:] + lens[-1:])
         if st.fault is not None:
@@ -77,14 +79,27 @@ class DelimitedBuffer:
             raise FormatException(f"{_FAULTS.get(kind, 'Invalid line')} (column {col})", line_number=line)
         data = chunk[:last_end + 1]
         fields = []
-        for kind, col in zip(cls._kinds, cols):
-            if kind == nv.COL_TEXT:
+        for i, (kind, col) in enumerate(zip(cls._kinds, cols)):
+            if i in floats:
+                fields.append(floats[i])
+            elif kind == nv.COL_TEXT:
                 fields.append(FieldView(data, col[1], col[0]))
             elif kind == nv.COL_STRAND:
                 fields.append(EncodedArray(col, StrandEncoding))
             else:
                 fields.append(col)
         return cls(data, n_lines, fields)
+
+    @staticmethod
+    def _parse_floats(chunk, view, column, status):
+        """The float64 values of one text column (bnpk_parse_float into the chunk's status block, no synchronisation).
+        A line without the column leaves its view unwritten: the parse is kept inside the chunk, and the column fault
+        of such a line is smaller than any value fault of it."""
+        from .decimal import pow5_table
+        v_start = view[0].clamp(0, chunk.numel())
+        v_lens = torch.minimum(view[1].clamp(min=0).to(torch.int64), chunk.numel() - v_start).to(torch.int32)
+        values, _ = ops.parse_float(chunk, v_start, v_lens, column, pow5_table(chunk.device), status)
+        return values
 
     @property
     def size(self) -> int:
@@ -153,6 +168,9 @@ class BedGraphBuffer(BdgBuffer):
     so nan, inf and longer significands raise FormatException naming the line.  Leading ``#``, ``track`` and
     ``browser`` lines are the header."""
     _kinds = (nv.COL_TEXT, nv.COL_INT, nv.COL_INT, nv.COL_TEXT)
+    _float_columns = (3,)
+
+    from_raw_buffer = DelimitedBuffer.__dict__["from_raw_buffer"]       # read as every delimited buffer; BdgBuffer's refuses
 
     @classmethod
     def read_header(cls, file_object):
@@ -164,26 +182,22 @@ class BedGraphBuffer(BdgBuffer):
             header.append(line.decode("utf-8"))
         return "".join(header)
 
+
+class NarrowPeakBuffer(DelimitedBuffer):
+    """MACS2 narrowPeak read on the device (delimited_buffers.py NarrowPeakBuffer): the six BED6 columns, signal_value,
+    p_value and q_value (float64) and summit (int64).  The columns are read as a BED chunk's are, then the three float
+    columns' text is parsed by bnpk_parse_float into the same status block, so a chunk takes the two synchronisations
+    of a BED chunk; a bad value raises FormatException naming its line (the grammar of BedGraphBuffer).  Read only."""
+    dataclass = NarrowPeak
+    _kinds = (nv.COL_TEXT, nv.COL_INT, nv.COL_INT, nv.COL_TEXT, nv.COL_INT_OR_DOT, nv.COL_STRAND, nv.COL_TEXT,
+              nv.COL_TEXT, nv.COL_TEXT, nv.COL_INT)
+    _float_columns = (6, 7, 8)
+
     @classmethod
-    def from_raw_buffer(cls, chunk, header_data=None):
-        from .decimal import pow5_table
-        chunk = _to_device_bytes(chunk)
-        n_lines = ops.count_byte(chunk, 10) if chunk.numel() else 0
-        if n_lines == 0:
-            raise IncompleteEntryException("No complete line in the buffer. Try increasing chunk_size.")
-        starts, lens, _ = ops.line_split(chunk, 1, 0, 0, ord(cls.COMMENT), False, 0, max_rows=n_lines)
-        cols, status = ops.delimited_columns(chunk, starts, lens, cls._kinds)
-        # a line without a value column leaves its view unwritten: keep the parse inside the chunk (the column fault
-        # of such a line is smaller than any value fault of it)
-        v_start = cols[3][0].clamp(0, chunk.numel())
-        v_lens = torch.minimum(cols[3][1].clamp(min=0).to(torch.int64), chunk.numel() - v_start).to(torch.int32)
-        values, _ = ops.parse_float(chunk, v_start, v_lens, 3, pow5_table(chunk.device), status)
-        st, last_end = ops.read_back(status, starts[-1:] + lens[-1:])
-        if st.fault is not None:
-            line, col, kind = st.column_fault()
-            raise FormatException(f"{_FAULTS.get(kind, 'Invalid line')} (column {col})", line_number=line)
-        data = chunk[:last_end + 1]
-        return cls(data, n_lines, [FieldView(data, cols[0][1], cols[0][0]), cols[1], cols[2], values])
+    def formatted(cls, entries):
+        raise NotImplementedError("writing narrowPeak is not supported: it is read only")
+
+    from_data = formatted
 
 
 _GTF_KINDS = (nv.COL_TEXT, nv.COL_TEXT, nv.COL_TEXT, nv.COL_INT, nv.COL_INT, nv.COL_TEXT, nv.COL_STRAND, nv.COL_TEXT,

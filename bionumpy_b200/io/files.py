@@ -43,9 +43,12 @@ def _buffer_type_for(suffix):
     if suffix == ".sam":
         from .sam import SAMBuffer
         return SAMBuffer
+    if suffix == ".narrowPeak":
+        from .delimited import NarrowPeakBuffer
+        return NarrowPeakBuffer
     raise RuntimeError(f"File format {suffix} does not have a default buffer type on the CUDA path "
-                       f"(supported: .fq .fastq .fa .fasta .bed .bdg .gtf .gff .gff3 .sam and their .gz forms, and "
-                       f".bam); pass buffer_type=")
+                       f"(supported: .fq .fastq .fa .fasta .bed .bdg .gtf .gff .gff3 .sam .narrowPeak and their .gz "
+                       f"forms, and .bam); pass buffer_type=")
 
 
 def _suffix(path):
@@ -65,7 +68,8 @@ def _read_buffer_type_for(suffix):
 
 def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
     """files.py:85-182.  Reading ("r", "rb") gives an NpDataclassReader; writing ("w", "wb", "write") or appending
-    ("a", "ab", "append") gives an NpBufferedWriter, which writes ``.gz`` files as BGZF.  ``.bdg`` (bedGraph) is
+    ("a", "ab", "append") gives an NpBufferedWriter, which writes ``.gz`` files as BGZF.  ``.narrowPeak`` is read
+    only, with NarrowPeakBuffer.  ``.bdg`` (bedGraph) is
     read with float64 values (BedGraphBuffer) and written with integer values (BdgBuffer), ``.sam`` read only (opening it for writing raises the RuntimeError it raised before SAM could be
     read), ``.bam`` read only (as BGZF, whatever the suffix says).  BED is written with the buffer type named: ``bnp.open("x.bed", "w", buffer_type=BedBuffer)`` (or
     Bed6Buffer; either writes a record's own fields).  Opening ``.bed`` for writing by its suffix alone raises
@@ -83,6 +87,8 @@ def bnp_open(filename, mode=None, buffer_type=None, lazy=None):
                            f".bam); pass buffer_type=")
     if mode in WRITE_MODES and buffer_type is None and suffix in (".gtf", ".gff", ".gff3"):
         raise NotImplementedError(f"writing {suffix} is not supported: GTF and GFF are read only")
+    if mode in WRITE_MODES and buffer_type is None and suffix == ".narrowPeak":
+        raise NotImplementedError("writing .narrowPeak is not supported: narrowPeak is read only")
     if mode in WRITE_MODES and buffer_type is None and suffix == ".bed":
         raise NotImplementedError("writing .bed by its suffix alone is not supported: name the format with "
                                   "buffer_type=bnp.io.BedBuffer (or Bed6Buffer)")

@@ -1052,3 +1052,34 @@ def track_f64_combine(a_starts, a_values, b_starts, b_values, op):
     check(lib().bnpk_track_f64_combine(*a, *b, op, _pointer(starts), _pointer(values), _pointer(n_runs), _pointer(ws),
                                        ws.numel(), stream_ptr()))
     return starts, values, n_runs
+
+
+
+def _column_sum(fn, runs, values, q_start, width, reverse):
+    q_p = _pointer(q_start, "q_start", torch.int64)
+    n = q_start.numel()
+    rev_p = _pointer(reverse, "reverse", torch.uint8, n=n, optional=True)
+    width = int(width)
+    if not 0 <= width < 2 ** 31:
+        check(fn(*runs, q_p, rev_p, n, width, None, None, stream_ptr()))       # the library's BNPK_E_BADARG
+    out = torch.empty(width, dtype=values.dtype, device=q_start.device)
+    partial = torch.empty(-(-n // nv.COLUMN_BLOCK_ROWS) * width, dtype=values.dtype, device=q_start.device)
+    check(fn(*runs, q_p, rev_p, n, width, _pointer(out), _pointer(partial), stream_ptr()))
+    return out
+
+
+@_on_device
+def runs_column_sum(run_starts, values, q_start, width, reverse=None):
+    """bnpk_runs_column_sum: int64[width], out[j] the wrapping sum over rows q of the track's value at q_start[q] + j,
+    or at q_start[q] + width - 1 - j where reverse[q] (uint8[Q], optional) is not 0.  Every such position must lie in
+    the track.  No synchronisation."""
+    runs = _runs_args(run_starts, values, 1)
+    return _column_sum(lib().bnpk_runs_column_sum, runs, values, q_start, width, reverse)
+
+
+@_on_device
+def track_f64_column_sum(run_starts, values, q_start, width, reverse=None):
+    """bnpk_track_f64_column_sum: float64[width], runs_column_sum over a float64 track, added in the fixed block order
+    of include/bnpk.h, so the sum has the same bits on every call.  No synchronisation."""
+    runs = _f64_runs_args(run_starts, values, 1)
+    return _column_sum(lib().bnpk_track_f64_column_sum, runs, values, q_start, width, reverse)

@@ -535,6 +535,27 @@ int bnpk_track_f64_combine(const int64_t *a_starts, const double *a_values, size
                            const double *b_values, size_t n_b, int op, int64_t *out_starts, double *out_values,
                            int64_t *n_out, void *workspace, size_t workspace_bytes, void *stream);
 
+/* K18  column sums of equal-length windows of a track (the meta-profile track[windows].mean(axis=0) around TSSs or
+ *   peak summits; GenomicArray indexed by windows, genomic_data/genomic_track.py).
+ * bnpk_runs_column_sum / bnpk_track_f64_column_sum: the track is R >= 1 runs (run_starts int64[R + 1] from 0 to the
+ *   size S, values int64[R] or double[R]).  out[j] (j < width) is the sum over rows q < n_q of the track's value at
+ *   q_start[q] + j, or at q_start[q] + width - 1 - j when reverse[q] != 0 (reverse NULL: no row is reversed).  Every
+ *   such position must lie in [0, S), as for bnpk_runs_extract; the caller guarantees it.  n_q == 0 writes zeros.
+ *   Summation order, fixed: rows are cut into blocks of BNPK_COLUMN_BLOCK_ROWS consecutive rows; partial[b * width + j]
+ *   is block b's values added in row order starting from +0.0, and out[j] is the block partials added in block order
+ *   starting from +0.0.  So the int64 sum wraps and is exact, the double sum has the same bits on every call whatever
+ *   the grid, and for n_q <= BNPK_COLUMN_BLOCK_ROWS it is NumPy's dense.sum(axis=0) of the rows bit for bit.  No
+ *   atomics.  partial holds ceil(n_q / BNPK_COLUMN_BLOCK_ROWS) * width elements (q_start and partial may be NULL when
+ *   n_q == 0, out when width == 0).  Device work: n_q x width adds and two launches; no synchronisation.  BNPK_E_BADARG
+ *   for a width outside [0, 2^31), no runs and a missing pointer. */
+#define BNPK_COLUMN_BLOCK_ROWS 256
+int bnpk_runs_column_sum(const int64_t *run_starts, const int64_t *values, size_t n_runs, const int64_t *q_start,
+                         const uint8_t *reverse, size_t n_q, int64_t width, int64_t *out, int64_t *partial,
+                         void *stream);
+int bnpk_track_f64_column_sum(const int64_t *run_starts, const double *values, size_t n_runs, const int64_t *q_start,
+                              const uint8_t *reverse, size_t n_q, int64_t width, double *out, double *partial,
+                              void *stream);
+
 /* Bloom filter over k-mer hashes (sequence/bloom_filter.py:15-42): hash function i is v ^ offsets[i]; the filter is
  * one byte per position (the reference's bool mask).  insert: mask[(v ^ offsets[i]) % mask_size] = 1 for every value and
  * function; query: out[j] = AND over the functions. */
